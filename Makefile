@@ -1,4 +1,4 @@
-# libalq.so (CUDA, sm_100a).  `make` == `python -m active_learning_b200.build`
+# libalq.so (CUDA, sm_90a).  `make` == `python -m active_learning_b200.build`
 PY ?= python
 
 all:

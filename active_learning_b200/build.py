@@ -1,10 +1,10 @@
-"""In-tree build of libalq.so (the C-ABI CUDA library) for sm_100a.
+"""In-tree build of libalq.so (the C-ABI CUDA library) for sm_90a (H100).
 
     python -m active_learning_b200.build            # or: make
 
 nvcc cross-compiles without a GPU.  The .so is written next to this file
-(active_learning_b200/libalq.so): git-ignored, but it travels with the repo snapshot to the
-GPU box.  Nothing is JIT-compiled at import time.
+(active_learning_b200/libalq.so, git-ignored), so the package is importable from the source
+tree.  Nothing is JIT-compiled at import time.
 """
 from __future__ import annotations
 
@@ -19,8 +19,9 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libalq.so")
 OBJ = os.path.join(HERE, "csrc", "_obj")
 
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    *GENCODE,
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC,-O3,-Wall,-Wno-unused-function",
 ]
@@ -62,7 +63,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         list(ex.map(run, jobs))
     objs = [os.path.join(OBJ, s[:-3] + ".o") for s in sources()]
     if force or jobs or _stale(OUT, objs):
-        run([nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", OUT, *objs])
+        run([nvcc, "-shared", *GENCODE, "-o", OUT, *objs])
     return OUT
 
 

@@ -1,4 +1,4 @@
-// Shared device/host helpers for libalq (sm_100a only).
+// Shared device/host helpers for libalq (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -12,8 +12,8 @@
 
 #include "../../include/alq.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "libalq is written for sm_100a (B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
+#error "libalq is written for sm_90a (H100) only"
 #endif
 
 constexpr int ALQ_MAX_WORLD = 8;
@@ -61,7 +61,7 @@ __device__ __forceinline__ bool wait_flag(const unsigned long long* p, unsigned 
 
 struct alq_ctx {
     int device = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     int clock_khz = 1900000;              // SM clock (cached: the attribute query costs about a millisecond)
     size_t smem_optin = 0;
     cudaStream_t side_stream = nullptr;   // H2D pipelining for the *_host entry points
@@ -83,11 +83,11 @@ struct alq_ctx {
     int sel_ring_next = 0;
     unsigned int* sel_last_ctr = nullptr;    // counters / stamps of the last fused launch (alq_uncertainty_tail_timing)
     AlqComm comm;
-    int k3_impl = 0;          // 0 auto, 1 fp32 SIMT, 2 tcgen05 3xTF32
+    int k3_impl = 0;          // 0 auto, 1 fp32 SIMT, 2 wgmma 3xTF32
     int select_impl = 0;      // 0 auto, 1 multi-kernel radix select, 2 cluster-resident single launch
     int greedy_variant = 0;   // 0 auto, 1 direct loads, 2 bulk-copy pipeline, 3 persistent cooperative loop
-    int l2_resident_mb = 64;  // persistent selection loop: MB of streamed rows kept in L2 across steps (evict_last hints); 0 = off.
-                              // Sweep on one B200 (tools/gpu_r2m.sh): 48-72 MB best, 96 MB worse, 112 MB back to no gain
+    int l2_resident_mb = 24;  // persistent selection loop: MB of streamed rows kept in L2 across steps (evict_last hints); 0 = off.
+                              // About half of the 50 MB L2: the rest serves the streamed rows and the agreement words
     int d2_fast_path = 1;     // D^2 draw of the persistent loop: certified per-CTA-mass path first (0: exact tree machinery only)
     int tail_buckets = 1;     // fused uncertainty tail on one GPU: route candidates to per-CTA score buckets (0: every CTA ranks
                               // its candidates against the whole list -- the general route, also the fallback for tie groups)
@@ -260,7 +260,7 @@ __device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src_gmem, u
 }
 
 
-// bulk copy with an L2 eviction policy (createpolicy): rows that should stay resident in the 126 MB L2 across the steps of
+// bulk copy with an L2 eviction policy (createpolicy): rows that should stay resident in the 50 MB L2 across the steps of
 // a selection loop are fetched evict_last, the rest evict_first so that the stream does not push them out
 __device__ __forceinline__ uint64_t l2_policy_evict_last() {
     uint64_t p;

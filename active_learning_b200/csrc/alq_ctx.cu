@@ -23,9 +23,9 @@ extern "C" int alq_create(alq_ctx** out, int device) {
         delete ctx;
         return ALQ_ERR_CUDA;
     }
-    if (prop.major != 10) {
+    if (prop.major != 9 || prop.minor != 0) {
         delete ctx;
-        return ALQ_ERR_CUDA;  // built for sm_100a only
+        return ALQ_ERR_CUDA;  // built for sm_90a only
     }
     ctx->sm_count = prop.multiProcessorCount;
     if (prop.clockRate > 0) ctx->clock_khz = prop.clockRate;

@@ -1,6 +1,6 @@
 // K4 / K5: the sequential selection loop of CoreSet (greedy k-center) and BADGE (k-means++ D^2
 // seeding) -- the device replacement of `CoresetSampler.coreset` (coreset_sampler.py:66-105 under
-// /root/reference/src/query_strategies).
+// active_learning/src/query_strategies).
 //
 // Per step the reference re-gathers an N x L slice of the dense distance matrix and re-mins it
 // (:79).  Here each step streams the candidate rows once: d2(i, centre) in the reference's own

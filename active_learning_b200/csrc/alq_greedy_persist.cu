@@ -1,5 +1,5 @@
 // K4 / K5 as ONE persistent cooperative launch: the whole B-step selection loop of
-// `CoresetSampler.coreset` (coreset_sampler.py:66-105 under /root/reference/src/query_strategies) runs
+// `CoresetSampler.coreset` (coreset_sampler.py:66-105 under active_learning/src/query_strategies) runs
 // inside one kernel, one CTA per SM, on one GPU or on G GPUs that talk through peer-memory windows.
 //
 // Why: a step is a 100-150 us HBM stream on one GPU but only 12-19 us on eight, and the rows a step

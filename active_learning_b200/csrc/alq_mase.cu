@@ -1,7 +1,7 @@
 // K6: MASE / BASE (SURVEY.md section 8f rank 2) -- distance of every pool embedding to the pairwise decision
 // boundaries of the linear head, and the class-balanced selection built on it.
 //
-// Reference semantics (under /root/reference/src/query_strategies): mase_sampler.py:52-80 broadcasts
+// Reference semantics (under active_learning/src/query_strategies): mase_sampler.py:52-80 broadcasts
 // (B, C, M) tensors per loader batch to get  radius[i, c] = | -(w_p - w_c) * lam / 2 |,
 // lam = 2 (h_i.(w_p - w_c) + b_p - b_c) / |w_p - w_c|^2,  p = argmax_c z_i.  With the algebra carried out,
 // h_i.(w_p - w_c) + b_p - b_c is the logit gap z_ip - z_ic and the radius is |z_ip - z_ic| / |w_p - w_c|:

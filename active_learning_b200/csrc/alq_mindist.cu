@@ -2,7 +2,7 @@
 // of a second set, without ever forming the N x M matrix.  Device replacement of
 // get_pairwise_l2_dist + `[:, labeled].min(dim=1)` (coreset_sampler.py:59-64,79) and of the
 // minimax cold start `.max(dim=1).values.min(dim=0)` (coreset_sampler.py:100), all under
-// /root/reference/src/query_strategies.
+// active_learning/src/query_strategies.
 //
 // This is the one dense contraction on the path (2*N*M*D flop).  This translation unit is the
 // exact-fp32 SIMT version: a 128x128x16 shared-memory tiled SGEMM (8x8 register micro-tiles,
@@ -255,7 +255,7 @@ extern "C" int alq_min_dist(alq_ctx* ctx, const float* x, int64_t ldx, const flo
     if (factored && ((c % 4) || (ldxa % 4) || (ldya % 4) || !aligned16(xa) || !aligned16(ya)))
         ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_min_dist: c, ldxa, ldya must be multiples of 4 (pad with zeros)");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    // tensor-core path (tcgen05 3xTF32) for contractions big enough to amortise the operand split
+    // tensor-core path (wgmma 3xTF32) for contractions big enough to amortise the operand split
     {
         const bool tc_shape = d >= 32 && (!factored || c >= 32) && m > 0;
         const double flop = 2.0 * static_cast<double>(n) * static_cast<double>(m) * (d + (factored ? c : 0));

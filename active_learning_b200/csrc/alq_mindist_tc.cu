@@ -1,25 +1,24 @@
-// K3 on the 5th-generation tensor cores: out[i] = min_j (max_j) fl(fl(xn_i + yn_j) - 2 <x_i, y_j>)
-// for fp32 rows, as a tcgen05 "3xTF32" contraction with the min-epilogue fused on the TMEM
+// K3 on the Hopper tensor cores: out[i] = min_j (max_j) fl(fl(xn_i + yn_j) - 2 <x_i, y_j>)
+// for fp32 rows, as a wgmma "3xTF32" contraction with the min-epilogue fused on the register
 // accumulators.  Same contract as the SIMT kernel in alq_mindist.cu (coreset_sampler.py:59-64,79,100
-// under /root/reference/src/query_strategies); this is the one dense contraction on the query path.
+// of the reference's query_strategies); this is the one dense contraction on the query path.
 //
-// fp32 fidelity.  kind::tf32 keeps 10 mantissa bits, so each operand is split once, ahead of time,
+// fp32 fidelity.  .tf32 keeps 10 mantissa bits, so each operand is split once, ahead of time,
 // into two valid TF32 numbers  x = hi + lo + r,  hi = rna_tf32(x), lo = rna_tf32(x - hi), |r| <= 2^-22|x|,
 // and every k-step issues three MMAs into the same fp32 accumulator:  hi*hi' + hi*lo' + lo*hi'.
 // The dropped lo*lo' and r terms are <= 2^-21 |x||y| per product.  Small integers (the exact-arithmetic
 // parity fixtures) have lo == 0 and give bit-identical results to fp32.
 //
-// Structure (one CTA per SM, persistent over a host-built work list):
-//   warp 0   TMA producer: 4 tensor maps (X_hi, X_lo, Y_hi, Y_lo), boxes of 32 fp32 (=128 B, SWIZZLE_128B)
-//            x 128 / 256 rows into a 2-stage shared-memory ring, mbarrier complete_tx.
-//   warp 1   MMA issuer (one elected lane): tcgen05.mma.cta_group::1.kind::tf32, M=128, N=256, K=8,
-//            12 MMAs per stage, tcgen05.commit frees the stage / publishes the accumulator.
-//   warps 2-5 epilogue: tcgen05.ld 32x32b.x32 (one accumulator row per thread), distance + running
-//            row min in registers across all column tiles of a work item, one float atomic per row at the end.
-//   TMEM: 512 columns = two 128x256 fp32 accumulators (double buffered; the factored/BADGE form uses
-//   them as the <a,a'> and <h,h'> accumulators of one tile and multiplies them in the epilogue).
+// Structure (one CTA per SM, persistent over a host-built work list, 3 warpgroups):
+//   warpgroup 0   TMA producer (one thread): 4 tensor maps (X_hi, X_lo, Y_hi, Y_lo), boxes of 32 fp32
+//                 (=128 B, SWIZZLE_128B) x 128 rows into a 3-stage shared-memory ring, mbarrier complete_tx.
+//   warpgroups 1-2 consumers: each owns 64 of the tile's 128 rows and issues
+//                 wgmma.mma_async.m64n128k8.f32.tf32.tf32 from shared memory (12 per stage, one stage kept
+//                 in flight), then the distance + running row min on its register accumulators; one float
+//                 atomic per row at the end of a work item.  The factored/BADGE form keeps two accumulators
+//                 (<h,h'> and <a,a'>) and multiplies them in the epilogue.
 // Every CTA sweeps the column tiles in the same order, so a Y tile is fetched from HBM once and
-// served to the other 147 CTAs from L2.
+// served to the other CTAs from L2.
 #include <cuda.h>
 #include <stdlib.h>
 
@@ -27,16 +26,15 @@
 
 namespace tc {
 
-constexpr int BM = 128;          // accumulator rows  (UMMA M)
-constexpr int BN = 256;          // accumulator cols  (UMMA N)
+constexpr int BM = 128;          // rows per tile (two m64 warpgroups)
+constexpr int BN = 128;          // cols per tile (wgmma N)
 constexpr int BK = 32;           // fp32 per stage row = 128 bytes = one swizzle span
-constexpr int UK = 8;            // UMMA K for tf32
-constexpr int STAGES = 2;
+constexpr int UK = 8;            // wgmma K for tf32
+constexpr int STAGES = 3;
 constexpr int A_BYTES = BM * BK * 4;              // 16 KB
-constexpr int B_BYTES = BN * BK * 4;              // 32 KB
-constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;   // hi + lo of both operands = 96 KB
-constexpr int THREADS = 192;
-constexpr int TMEM_COLS = 512;
+constexpr int B_BYTES = BN * BK * 4;              // 16 KB
+constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;   // hi + lo of both operands = 64 KB
+constexpr int THREADS = 384;
 
 struct WorkItem {
     int m_blk, n_begin, n_end, pad;   // row block, [first, last) column tile
@@ -57,47 +55,40 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, i
         "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
         ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor):
+// K-major, SWIZZLE_128B shared-memory matrix descriptor (PTX ISA, "Matrix Descriptor Format" of wgmma):
 //   bits [0,14) start address >> 4, [16,30) leading byte offset >> 4 (= 1, unused for swizzled K-major),
-//   [32,46) stride byte offset >> 4 (= 1024 B: 8 rows x 128 B), [46,48) version = 1, [61,64) layout = 2.
+//   [32,46) stride byte offset >> 4 (= 1024 B: 8 rows x 128 B), [62,64) swizzle mode = 1 (128 B).
 __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3fff);
     d |= static_cast<uint64_t>(1) << 16;
     d |= static_cast<uint64_t>(1024 >> 4) << 32;
-    d |= static_cast<uint64_t>(1) << 46;
-    d |= static_cast<uint64_t>(2) << 61;
+    d |= static_cast<uint64_t>(1) << 62;
     return d;
 }
-// cute::UMMA::InstrDescriptor: c_format F32 (1) @4, a/b format TF32 (2) @7/@10, K-major both, N>>3 @17, M>>4 @24
-__device__ __forceinline__ uint32_t make_idesc() {
-    return (1u << 4) | (2u << 7) | (2u << 10) | (static_cast<uint32_t>(BN >> 3) << 17) |
-           (static_cast<uint32_t>(BM >> 4) << 24);
-}
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// d (64 x 128 fp32, the m64n128 register fragment) += A (64 x 8, smem) * B (128 x 8, smem)^T;  scale_d == 0 overwrites d
+__device__ __forceinline__ void wgmma_tf32(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
     asm volatile(
         "{\n\t"
         ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1;\n\t"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(adesc), "l"(bdesc), "r"(scale_d));
 }
 
 template <bool FACTORED, bool RED_MAX>
@@ -113,33 +104,22 @@ min_dist_tc_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_cons
     unsigned char* stage_base = smem_raw;
     uint64_t* full = reinterpret_cast<uint64_t*>(smem_raw + STAGES * STAGE_BYTES);
     uint64_t* empty = full + STAGES;
-    uint64_t* tmem_full = empty + STAGES;      // [2]
-    uint64_t* tmem_empty = tmem_full + 2;      // [2]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-    float* cn_s = reinterpret_cast<float*>(tmem_slot + 4);                  // [2][BN]
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int wg = threadIdx.x >> 7;
     const int n_items = P.item_count[blockIdx.x];
     const WorkItem* items = P.items + static_cast<size_t>(blockIdx.x) * P.items_per_cta;
     const int kb_total = P.kblocks_h + (FACTORED ? P.kblocks_a : 0);
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        for (int b = 0; b < 2; ++b) { mbar_init(&tmem_full[b], 1); mbar_init(&tmem_empty[b], 4); }
+        for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {   // TMEM allocation is warp-collective; the same warp frees it at the end
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (wg == 0) {
         // ================= TMA producer =================
-        if (lane == 0) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+        if (threadIdx.x == 0) {
             uint32_t it = 0;
             for (int w = 0; w < n_items; ++w) {
                 const WorkItem wi = items[w];
@@ -160,102 +140,87 @@ min_dist_tc_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_cons
                 }
             }
         }
-    } else if (warp == 1) {
-        // ================= MMA issuer =================
-        if (lane == 0) {
-            const uint32_t idesc = make_idesc();
-            uint32_t it = 0, tile = 0;
-            for (int w = 0; w < n_items; ++w) {
-                const WorkItem wi = items[w];
-                for (int nt = wi.n_begin; nt < wi.n_end; ++nt, ++tile) {
-                    // dense: accumulator buffer alternates per tile; factored: buffer 0 = <h,h'>, 1 = <a,a'>
-                    if (FACTORED) {
-                        if (tile > 0) { mbar_wait(&tmem_empty[0], (tile - 1) & 1u); }
-                    } else {
-                        const uint32_t use = tile >> 1;
-                        if (use > 0) mbar_wait(&tmem_empty[tile & 1], (use - 1) & 1u);
-                    }
-                    tc_fence_after();
-                    for (int kb = 0; kb < kb_total; ++kb, ++it) {
-                        const int s = it % STAGES;
-                        mbar_wait(&full[s], (it / STAGES) & 1u);
-                        tc_fence_after();
-                        const bool apart = FACTORED && kb >= P.kblocks_h;
-                        const uint32_t buf = FACTORED ? (apart ? 1u : 0u) : (tile & 1u);
-                        const uint32_t d_tmem = tmem_base + buf * BN;
-                        const bool first_kb = apart ? (kb == P.kblocks_h) : (kb == 0);
-                        const uint32_t a_hi = smem_u32(stage_base + static_cast<size_t>(s) * STAGE_BYTES);
-                        const uint32_t a_lo = a_hi + A_BYTES, b_hi = a_hi + 2 * A_BYTES, b_lo = b_hi + B_BYTES;
-#pragma unroll
-                        for (int k = 0; k < BK / UK; ++k) {
-                            const uint32_t off = k * UK * 4;    // bytes along K inside the 128-byte swizzle span
-                            const uint64_t dah = make_desc(a_hi + off), dal = make_desc(a_lo + off);
-                            const uint64_t dbh = make_desc(b_hi + off), dbl = make_desc(b_lo + off);
-                            umma_tf32(d_tmem, dah, dbh, idesc, (first_kb && k == 0) ? 0u : 1u);
-                            umma_tf32(d_tmem, dah, dbl, idesc, 1u);
-                            umma_tf32(d_tmem, dal, dbh, idesc, 1u);
-                        }
-                        umma_commit(&empty[s]);              // stage reusable once these MMAs retire
-                    }
-                    if (FACTORED) { umma_commit(&tmem_full[0]); }
-                    else umma_commit(&tmem_full[tile & 1]);
-                }
-            }
-        }
     } else {
-        // ================= epilogue: 4 warps, one accumulator row per thread =================
-        const int q = warp & 3;                         // TMEM lane quadrant this warp may access
-        const int row_in_tile = q * 32 + lane;
-        const int et = threadIdx.x - 64;                // 0..127
-        uint32_t tile = 0;
+        // ================= consumers: warpgroup wg - 1 owns rows [64 (wg - 1), 64 wg) of the tile =================
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+        const int t = threadIdx.x & 127, warp = t >> 5, lane = t & 31;
+        const uint32_t a_off = static_cast<uint32_t>(wg - 1) * 64 * BK * 4;     // 8 KB: a whole number of swizzle atoms
+        // m64nN fp32 fragment: d[4j + {0,1}] = (r, 8j + 2 (lane % 4) + {0,1}), d[4j + {2,3}] = (r + 8, same cols),
+        // r = 16 warp + lane / 4
+        const int r_in_tile = (wg - 1) * 64 + warp * 16 + (lane >> 2);
+        const int c_in_tile = 2 * (lane & 3);
+        uint32_t it = 0;
         for (int w = 0; w < n_items; ++w) {
             const WorkItem wi = items[w];
-            const int row = wi.m_blk * BM + row_in_tile;
-            const float rn = row < P.n ? P.xn[row] : 0.f;
-            float best = RED_MAX ? ALQ_NEG_INF : ALQ_POS_INF;
-            for (int nt = wi.n_begin; nt < wi.n_end; ++nt, ++tile) {
-                float* cn = cn_s + (tile & 1) * BN;
-                for (int j = et; j < BN; j += 128) {
-                    const int col = nt * BN + j;
-                    cn[j] = col < P.m ? P.yn[col] : (RED_MAX ? ALQ_NEG_INF : ALQ_POS_INF);
-                }
-                asm volatile("bar.sync 1, 128;" ::: "memory");
-                const uint32_t buf = FACTORED ? 0u : (tile & 1u);
-                const uint32_t par = FACTORED ? (tile & 1u) : ((tile >> 1) & 1u);
-                mbar_wait(&tmem_full[buf], par);
-                tc_fence_after();
-                const uint32_t lane_addr = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
-#pragma unroll 1
-                for (int c0 = 0; c0 < BN; c0 += 32) {
-                    uint32_t acc[32];
-                    tmem_ld32(lane_addr + buf * BN + c0, acc);
-                    if (FACTORED) {
-                        uint32_t acc2[32];
-                        tmem_ld32(lane_addr + BN + c0, acc2);
+            const int row0 = wi.m_blk * BM + r_in_tile, row1 = row0 + 8;
+            const float rn0 = row0 < P.n ? P.xn[row0] : 0.f, rn1 = row1 < P.n ? P.xn[row1] : 0.f;
+            float best0 = RED_MAX ? ALQ_NEG_INF : ALQ_POS_INF, best1 = best0;
+            for (int nt = wi.n_begin; nt < wi.n_end; ++nt) {
+                float acc[64];
+                float acc_a[FACTORED ? 64 : 1];
+                int prev = -1;
+                for (int kb = 0; kb < kb_total; ++kb, ++it) {
+                    const int s = it % STAGES;
+                    mbar_wait(&full[s], (it / STAGES) & 1u);
+                    const bool apart = FACTORED && kb >= P.kblocks_h;
+                    const bool first_kb = apart ? (kb == P.kblocks_h) : (kb == 0);
+                    const uint32_t a_hi = smem_u32(stage_base + static_cast<size_t>(s) * STAGE_BYTES) + a_off;
+                    const uint32_t a_lo = a_hi + A_BYTES, b_hi = a_hi - a_off + 2 * A_BYTES, b_lo = b_hi + B_BYTES;
+                    wgmma_fence();
 #pragma unroll
-                        for (int j = 0; j < 32; ++j) acc[j] = __float_as_uint(__uint_as_float(acc[j]) * __uint_as_float(acc2[j]));
+                    for (int k = 0; k < BK / UK; ++k) {
+                        const uint32_t off = k * UK * 4;    // bytes along K inside the 128-byte swizzle span
+                        const uint64_t dah = make_desc(a_hi + off), dal = make_desc(a_lo + off);
+                        const uint64_t dbh = make_desc(b_hi + off), dbl = make_desc(b_lo + off);
+                        const uint32_t sc = (first_kb && k == 0) ? 0u : 1u;
+                        if constexpr (FACTORED) {
+                            if (apart) {
+                                wgmma_tf32(acc_a, dah, dbh, sc);
+                                wgmma_tf32(acc_a, dah, dbl, 1u);
+                                wgmma_tf32(acc_a, dal, dbh, 1u);
+                                continue;
+                            }
+                        }
+                        wgmma_tf32(acc, dah, dbh, sc);
+                        wgmma_tf32(acc, dah, dbl, 1u);
+                        wgmma_tf32(acc, dal, dbh, 1u);
                     }
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) {
-                        const float dist = (rn + cn[c0 + j]) - 2.0f * __uint_as_float(acc[j]);
-                        best = RED_MAX ? fmaxf(best, dist) : fminf(best, dist);
-                    }
+                    wgmma_commit();
+                    wgmma_wait<1>();                          // the previous stage's MMAs have retired: hand it back
+                    if (prev >= 0 && t == 0) mbar_arrive(&empty[prev]);
+                    prev = s;
                 }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&tmem_empty[buf]);
+                wgmma_wait<0>();
+                if (prev >= 0 && t == 0) mbar_arrive(&empty[prev]);
+#pragma unroll
+                for (int j = 0; j < 16; ++j) {
+                    const int col = nt * BN + 8 * j + c_in_tile;
+                    const float pad = RED_MAX ? ALQ_NEG_INF : ALQ_POS_INF;
+                    const float cn0 = col < P.m ? __ldg(P.yn + col) : pad;
+                    const float cn1 = col + 1 < P.m ? __ldg(P.yn + col + 1) : pad;
+                    float v[4] = {acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]};
+                    if constexpr (FACTORED) {
+#pragma unroll
+                        for (int e = 0; e < 4; ++e) v[e] = v[e] * acc_a[4 * j + e];
+                    }
+                    const float d00 = (rn0 + cn0) - 2.0f * v[0], d01 = (rn0 + cn1) - 2.0f * v[1];
+                    const float d10 = (rn1 + cn0) - 2.0f * v[2], d11 = (rn1 + cn1) - 2.0f * v[3];
+                    if (RED_MAX) { best0 = fmaxf(best0, fmaxf(d00, d01)); best1 = fmaxf(best1, fmaxf(d10, d11)); }
+                    else { best0 = fminf(best0, fminf(d00, d01)); best1 = fminf(best1, fminf(d10, d11)); }
+                }
             }
-            if (row < P.n && wi.n_end > wi.n_begin) {
-                if (RED_MAX) atomic_max_float(P.out + row, best);
-                else atomic_min_float(P.out + row, best);
+            // the four lanes of a quad hold the same two rows
+#pragma unroll
+            for (int o = 1; o <= 2; o <<= 1) {
+                const float b0 = __shfl_xor_sync(0xffffffffu, best0, o), b1 = __shfl_xor_sync(0xffffffffu, best1, o);
+                best0 = RED_MAX ? fmaxf(best0, b0) : fminf(best0, b0);
+                best1 = RED_MAX ? fmaxf(best1, b1) : fminf(best1, b1);
+            }
+            if ((lane & 3) == 0 && wi.n_end > wi.n_begin) {
+                if (row0 < P.n) { if (RED_MAX) atomic_max_float(P.out + row0, best0); else atomic_min_float(P.out + row0, best0); }
+                if (row1 < P.n) { if (RED_MAX) atomic_max_float(P.out + row1, best1); else atomic_min_float(P.out + row1, best1); }
             }
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
     }
 }
 
@@ -342,11 +307,11 @@ int alq_min_dist_tc(alq_ctx* ctx, const float* x, int64_t ldx, const float* xn, 
     const int grid = ctx->sm_count;
     const int m_blocks = static_cast<int>((n + BM - 1) / BM), n_tiles = static_cast<int>((m + BN - 1) / BN);
     // Work list.  A CTA re-reads its row block (hi + lo = 2 MB at d = 2048) for every column tile, so the row
-    // blocks that are live at the same time must fit L2 next to the streamed Y tiles: with one row block per CTA
-    // (148 x 2 MB) they do not, and ncu showed 258 GB of DRAM reads for 5 GB of operands.  Instead `split` CTAs
-    // share a row block and divide its column tiles, so only grid / split (~37) row blocks are live per round.
+    // blocks that are live at the same time must fit the 50 MB L2 next to the streamed Y tiles: with one row block
+    // per CTA (132 x 2 MB) they do not.  Instead `split` CTAs share a row block and divide its column tiles, so only
+    // live_mb / 2 MB row blocks are live per round (each Y tile is then read from HBM once per round).
     const size_t blk_bytes = static_cast<size_t>(BM) * (d + cpad) * 8;
-    size_t live_mb = 48;                                                                              // sweep: 32-48 MB best
+    size_t live_mb = 16;
     if (const char* e = getenv("ALQ_K3_LIVE_MB")) live_mb = static_cast<size_t>(std::max(1, atoi(e)));   // tuning aid
     int live = static_cast<int>(std::max<size_t>(1, (live_mb << 20) / std::max<size_t>(blk_bytes, 1)));
     live = std::max(1, std::min(live, grid));
@@ -419,7 +384,7 @@ int alq_min_dist_tc(alq_ctx* ctx, const float* x, int64_t ldx, const float* xn, 
     P.xn = xn_use; P.yn = yn_use; P.out = out; P.items = d_items; P.item_count = d_counts; P.items_per_cta = items_per_cta;
     P.n = static_cast<int>(n); P.m = static_cast<int>(m);
     P.kblocks_h = (d + BK - 1) / BK; P.kblocks_a = factored ? (c + BK - 1) / BK : 0;
-    const size_t smem = static_cast<size_t>(STAGES) * STAGE_BYTES + 256 + 2 * BN * sizeof(float) + 1024;
+    const size_t smem = static_cast<size_t>(STAGES) * STAGE_BYTES + 256 + 1024;
     auto launch = [&](auto kern) -> cudaError_t {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
         if (e != cudaSuccess) return e;

@@ -3,7 +3,7 @@
 // registers between the max pass and the exp pass, loads are 128-bit and L1-bypassing.
 //
 // Reference semantics: margin_sampler.py:33-35, confidence_sampler.py:31-33,
-// badge_sampler.py:33-44, coreset_sampler.py:61 (all under /root/reference/src/query_strategies).
+// badge_sampler.py:33-44, coreset_sampler.py:61 (all under active_learning/src/query_strategies).
 #include <initializer_list>
 #include <stdlib.h>
 
@@ -255,9 +255,8 @@ __device__ __forceinline__ void sel_find_bin(const uint32_t* hist, uint32_t k, u
 // of node k are 2k and 2k + 1; missing nodes hold ~0, which no list word reaches), so the probes of one step are
 // contiguous words.  Height h = smallest with 2^h - 1 >= nc; the sorted index r sits at node
 //     k(r) = 2^(h-1-z) + ((r + 1) >> (z + 1)),  z = trailing zeros of r + 1,
-// and after h steps of  k = 2k + (tree[k] <= x)  the count of candidates <= x is k - 2^h.  Measured on one B200: the stage
-// goes from 13.8 k to 10.6 k cycles, where the ~b shared-memory atomics on the difference array take over (the reason for
-// the bucket route).  It is exact in every one-GPU test, but the same helper produced wrong ranks inside the sharded
+// and after h steps of  k = 2k + (tree[k] <= x)  the count of candidates <= x is k - 2^h.  Without the conflicts the
+// ~b shared-memory atomics on the difference array dominate the stage (the reason for the bucket route).  It is exact in every one-GPU test, but the same helper produced wrong ranks inside the sharded
 // epilogue on 2 GPUs for c = 64 (tools/mgpu_tail_dbg.py; a host emulation of the arithmetic agrees with the sorted
 // search, so the cause is on the device side) -- hence not the default anywhere.  What is known: the wrong positions were
 // exactly the slices of ~12 CTAs per rank (presumably the ones that had streamed rows: 36 claims of 8 tiles, three per
@@ -1422,7 +1421,7 @@ static int uncertainty_tail_impl(alq_ctx* ctx, const float* logits, int64_t n, i
     if (sharded)
         if (int rc0 = alq_comm_check(ctx)) return rc0;       // a previous asynchronous exchange that timed out
     constexpr int kBucketCap = 48;          // per sub-list: a bucket holds up to 16 x 48 words (about b / grid = 68 expected)
-    static_assert(148 * kBucketLanes <= 2 * 2048, "bucket counters live in the slot's cross-rank words");
+    static_assert(132 * kBucketLanes <= 2 * 2048, "bucket counters live in the slot's cross-rank words");
     int rc = alq_scratch_reserve(ctx, scratch_need({static_cast<size_t>(n) * 8 + 16, static_cast<size_t>(ctx->sm_count) * kBucketLanes * kBucketCap * 8}));
     if (rc) return rc;
     SelArgs sel{};

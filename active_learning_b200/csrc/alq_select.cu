@@ -1,6 +1,6 @@
 // K1b: positions of the B smallest scores in ascending (score, position) order -- the device
 // replacement of `torch.sort(scores).indices[:B]` (margin_sampler.py:42, confidence_sampler.py:42
-// under /root/reference/src/query_strategies) with the fixed tie-break "lowest position first".
+// under active_learning/src/query_strategies) with the fixed tie-break "lowest position first".
 //
 //   1. 3-level MSB radix select (11+11+10 bits) over the order-preserving uint32 image of the
 //      scores finds T, the B-th smallest key, and how many keys tie with it inside the budget.

@@ -1,7 +1,7 @@
 // K1b, cluster-resident: the whole stable top-B selection in ONE launch for pools that fit the shared
 // memory of a thread-block cluster (n <= 8 * 32768 scores, b <= 16384).  Same contract and same result as
 // the multi-kernel path in alq_select.cu (`torch.sort(scores).indices[:B]` of margin_sampler.py:42 under
-// /root/reference/src/query_strategies, ties by lowest position).
+// active_learning/src/query_strategies, ties by lowest position).
 //
 // One cluster of 8 CTAs; every CTA keeps its slice of the order-preserving uint32 score keys in shared
 // memory for the whole kernel.  Stages are separated by cluster barriers (~0.4 us) instead of kernel

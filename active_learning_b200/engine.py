@@ -48,7 +48,7 @@ class Engine:
         rc = self.lib.alq_create(C.byref(h), self.device_index)
         if rc != 0:
             raise AlqError(f"alq_create(device={self.device_index}) failed with "
-                           f"{_lib.ERR_NAMES.get(rc, rc)} (needs an sm_100 GPU)")
+                           f"{_lib.ERR_NAMES.get(rc, rc)} (needs an sm_90 GPU: H100)")
         self._h = h
 
     def close(self):
@@ -90,7 +90,7 @@ class Engine:
         return self
 
     def set_option(self, key: str, value: int):
-        """'k3_impl': 0 auto / 1 fp32 SIMT / 2 tcgen05 3xTF32;  'greedy_variant': 0 auto / 1 direct / 2 pipeline / 3 persistent;  'spin_timeout_ms'; 'l2_resident_mb'; 'd2_fast_path'; 'tail_buckets';
+        """'k3_impl': 0 auto / 1 fp32 SIMT / 2 wgmma 3xTF32;  'greedy_variant': 0 auto / 1 direct / 2 pipeline / 3 persistent;  'spin_timeout_ms'; 'l2_resident_mb'; 'd2_fast_path'; 'tail_buckets';
         'select_impl': 0 auto / 1 multi-kernel / 2 cluster;  'base_impl': 0 auto / 1 sequential / 2 parallel lists."""
         self._check(self.lib.alq_set_option(self._h, key.encode(), int(value)), "alq_set_option")
 

@@ -3,4 +3,4 @@ from .strategy import Strategy
 
 
 class BADGESampler(BADGEQuery, Strategy):
-    """Drop-in for /root/reference/src/query_strategies/badge_sampler.py (K2 + K3 + K5, factored)."""
+    """Drop-in for active_learning/src/query_strategies/badge_sampler.py (K2 + K3 + K5, factored)."""

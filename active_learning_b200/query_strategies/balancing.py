@@ -1,6 +1,6 @@
 """BalancingSampler on the device (SURVEY.md section 8f rank 4): "Active Learning for Imbalanced Datasets" (WACV 2020).
 
-Query skeleton of /root/reference/src/query_strategies/balancing_sampler.py:26-134, one pick per step.  The class
+Query skeleton of active_learning/src/query_strategies/balancing_sampler.py:26-134, one pick per step.  The class
 histogram test (:66-82), the RNG draw of the random branch (:124) and the mask updates (:127-128) are host bookkeeping
 and stay literally the reference's (tiny torch-CPU tensors, so every promotion and division rounds the same way).
 What moves to the GPU is the part that scales with the pool: the embeddings never leave the device, class centres are

@@ -3,4 +3,4 @@ from .strategy import Strategy
 
 
 class BalancingSampler(BalancingQuery, Strategy):
-    """Drop-in for /root/reference/src/query_strategies/balancing_sampler.py (K3 distance fields + masked ratio arg-min)."""
+    """Drop-in for active_learning/src/query_strategies/balancing_sampler.py (K3 distance fields + masked ratio arg-min)."""

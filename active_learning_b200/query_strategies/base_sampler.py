@@ -3,4 +3,4 @@ from .strategy import Strategy
 
 
 class BASESampler(BASEQuery, Strategy):
-    """Drop-in for /root/reference/src/query_strategies/base_sampler.py (K6 + per-class K1b)."""
+    """Drop-in for active_learning/src/query_strategies/base_sampler.py (K6 + per-class K1b)."""

@@ -1,7 +1,7 @@
 """CoreSet (greedy k-center) and BADGE (k-means++ D^2 seeding) queries on the device
 (kernels K2, K3, K4, K5).
 
-Host glue of /root/reference/src/query_strategies/coreset_sampler.py:21-41,107-133,
+Host glue of active_learning/src/query_strategies/coreset_sampler.py:21-41,107-133,
 partitioned_coreset_sampler.py:36-84, badge_sampler.py:50-78 and partitioned_badge_sampler.py:
 index bookkeeping and the NumPy RNG stream are reproduced call for call; everything numeric
 (embeddings, distances, the B-step selection loop) stays on the GPU.

@@ -3,4 +3,4 @@ from .strategy import Strategy
 
 
 class CoresetSampler(CoresetQuery, Strategy):
-    """Drop-in for /root/reference/src/query_strategies/coreset_sampler.py (K3 + K4)."""
+    """Drop-in for active_learning/src/query_strategies/coreset_sampler.py (K3 + K4)."""

@@ -1,4 +1,4 @@
-"""`--strategy` dispatch, same contract as /root/reference/src/query_strategies/get_strategy.py:
+"""`--strategy` dispatch, same contract as active_learning/src/query_strategies/get_strategy.py:
 `get_strategy(name)` returns the class called `name`.  The ten accelerated samplers (the seven of the
 north-star path plus MASE / BASE / Balancing, SURVEY.md section 8f) and the default RandomSampler are implemented; the reference's remaining class names resolve to a
 stub that raises a clear error (SURVEY.md section 8: out of scope for this path)."""

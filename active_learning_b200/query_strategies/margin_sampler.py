@@ -3,4 +3,4 @@ from .uncertainty import MarginQuery
 
 
 class MarginSampler(MarginQuery, Strategy):
-    """Drop-in for /root/reference/src/query_strategies/margin_sampler.py (K1 margin + K1b)."""
+    """Drop-in for active_learning/src/query_strategies/margin_sampler.py (K1 margin + K1b)."""

@@ -1,6 +1,6 @@
 """MASE / BASE acquisition on the device (kernel K6 + K1b): SURVEY.md section 8f rank 2.
 
-Query skeletons of /root/reference/src/query_strategies/mase_sampler.py:19-27 and base_sampler.py:12-44.  The
+Query skeletons of active_learning/src/query_strategies/mase_sampler.py:19-27 and base_sampler.py:12-44.  The
 reference broadcasts (B, C, M) tensors per loader batch to measure how far every embedding is from each pairwise
 decision boundary of the linear head; with the algebra carried out that distance is the logit gap over the head
 geometry, |z_p - z_c| / |w_p - w_c| (include/alq.h, K6), so the tail is one C x C table per query and one streaming

@@ -3,4 +3,4 @@ from .strategy import Strategy
 
 
 class MASESampler(MASEQuery, Strategy):
-    """Drop-in for /root/reference/src/query_strategies/mase_sampler.py (K6 + K1b)."""
+    """Drop-in for active_learning/src/query_strategies/mase_sampler.py (K6 + K1b)."""

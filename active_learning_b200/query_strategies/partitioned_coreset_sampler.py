@@ -3,4 +3,4 @@ from .strategy import Strategy
 
 
 class PartitionedCoresetSampler(PartitionedCoresetQuery, Strategy):
-    """Drop-in for /root/reference/src/query_strategies/partitioned_coreset_sampler.py."""
+    """Drop-in for active_learning/src/query_strategies/partitioned_coreset_sampler.py."""

@@ -2,7 +2,7 @@ from .strategy import Strategy
 
 
 class RandomSampler(Strategy):
-    """/root/reference/src/query_strategies/random_sampler.py: the first `budget` entries of the
+    """active_learning/src/query_strategies/random_sampler.py: the first `budget` entries of the
     shuffled pool.  Host-only (no scoring arithmetic); kept because it is `--strategy`'s default."""
 
     def query(self, budget):

@@ -1,7 +1,7 @@
 """Query-path half of the reference's ``Strategy`` base class, plus the plumbing the accelerated
 samplers share.
 
-Mirrors /root/reference/src/query_strategies/strategy.py for everything ``query()`` touches:
+Mirrors active_learning/src/query_strategies/strategy.py for everything ``query()`` touches:
 constructor signature and attributes (:74-124), ``available_query_idxs`` (:126-145),
 ``already_labeled_idxs`` (:147-163), ``update`` (:459-485).  Training / evaluation
 (:249-442) is out of scope (SURVEY.md section 2, row 14): to keep it, bind the samplers onto the

@@ -1,6 +1,6 @@
 """Softmax-uncertainty acquisition on the device (kernels K1 + K1b).
 
-Query skeleton of /root/reference/src/query_strategies/margin_sampler.py:19-45: pool indices in
+Query skeleton of active_learning/src/query_strategies/margin_sampler.py:19-45: pool indices in
 loader order -> frozen-network forward -> per-row score -> the `budget` smallest scores, ascending,
 ties by pool position -> global indices.  What differs from the reference is only *where* the
 tail runs: logits stay in a device slab, the score and the top-B selection are CUDA kernels, and

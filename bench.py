@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- per-round query throughput of the acquisition-scoring engine.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--no-extras]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--no-extras] [--dump-outputs DIR]
 
 Headline (BASELINE.json configs[1]): MarginSampler query tail on an ImageNet-shaped pool of
 80 000 x 1000 fp32 logits per GPU, budget 10 000.  A "step" is one full tail: K1 (softmax margin)
@@ -17,8 +17,13 @@ of the reference's CPU tail on this box's host cores) and, at N = 1, `workloads`
 (K3+K4) and BADGE (K2+K3+K5) tails at 80 000 candidates / 50 000 labeled / B = 10 000 with their own
 roofline objects -- the BADGE k-means++ streaming kernel is the north star's 90 % target.
 
-`--impl reference` times the reference's CPU implementation of the same tail (oracle port: the
-reference is Python and cannot travel to the GPU box) on all host threads.
+`--impl reference` times the reference's CPU implementation of the same tail (oracle port of the
+reference's Python) on all host threads.
+
+`--dump-outputs DIR` writes what the last timed headline step returned to its caller: DIR/scores.npy
+(float32, the margin of every row of this GPU's shard; scores_rank<r>.npy at N > 1) and DIR/positions.npy
+(float64, the B selected positions, global at N > 1).  Inputs are seeded, so two builds run with the same
+arguments can be compared output for output.
 """
 import argparse
 import json
@@ -46,7 +51,7 @@ def measured_peaks():
             p = json.load(fh)
         return float(p["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "fallback (H100 SXM data sheet: 3.35 TB/s HBM3)"
 
 
 _TF32 = {}
@@ -54,8 +59,8 @@ _TF32 = {}
 
 def tf32_peak():
     """Dense TF32 tensor peak, MEASURED here (SURVEY.md section 8d: it is not in MEASURED_PEAKS.json): cuBLAS TF32 GEMM
-    8192^3 through torch.matmul with allow_tf32, best of 10, CUDA events -- the same recipe as the driver's bf16 figure.
-    Only a denominator: nothing on the product path calls it.  Falls back to bf16 / 2 without a GPU."""
+    8192^3 through torch.matmul with allow_tf32, best of 10, CUDA events.  Only a denominator: nothing on the product
+    path calls it.  Falls back to bf16 / 2 without a GPU."""
     if "v" in _TF32:
         return _TF32["v"]
     val, src = None, None
@@ -85,23 +90,14 @@ def tf32_peak():
             with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as fh:
                 val = float(json.load(fh)["bf16_tflops"]) / 2.0
         except Exception:
-            val = 1590.0 / 2.0
+            val = 989.0 / 2.0         # H100 SXM data sheet, dense bf16
         src = "MEASURED_PEAKS.json bf16_tflops / 2 (no live TF32 measurement possible)"
     _TF32["v"], _TF32["src"] = val, src
     return val
 
 
-def ncu_traffic(kernel):
-    """DRAM bytes per launch from the committed ncu --set full capture, if any."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "traffic.json")) as fh:
-            return json.load(fh).get(kernel)
-    except Exception:
-        return None
-
-
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -300,7 +296,7 @@ def workload_config(gpus):
     return {"workload": "MarginSampler query tail (configs[1]): softmax margin + stable top-B",
             "pool_rows_per_gpu": N_ROWS, "pool_rows_total": N_ROWS * gpus, "classes": N_CLASSES,
             "budget": BUDGET, "parallelism": f"row-sharded x{gpus}",
-            "l2": "inputs (320 MB logits per GPU) are larger than the 126 MB L2; no flush needed"}
+            "l2": "inputs (320 MB logits per GPU) are larger than the 50 MB L2; no flush needed"}
 
 
 # ----------------------------------------------------------------------------------------------
@@ -434,15 +430,13 @@ def run_greedy_workload(eng, kind, peak, steps, warmup, world=1, rank=0, check_p
                                "barrier and exchange is inside",
                      "streaming_phase": {"achieved": achieved_stream, "frac": achieved_stream / peak,
                                          "us": acc["stream_ms"] * 1e3, "select_us": acc["select_ms"] * 1e3,
-                                         "timing": "%globaltimer stamps of CTA 0 inside the kernel"},
-                     "traffic": ncu_traffic("persist_factored_sample" if factored else "persist_dense_argmax")},
-        "k3": {"kernel": "min_dist_tc_kernel (tcgen05 3xTF32 contraction, TMEM accumulators, fused min epilogue; "
+                                         "timing": "%globaltimer stamps of CTA 0 inside the kernel"}},
+        "k3": {"kernel": "min_dist_tc_kernel (wgmma 3xTF32 contraction, register accumulators, fused min epilogue; "
                          "time includes the hi/lo operand split)",
                "bound": "tensor", "effective_fp32_tflops": flops / (acc["k3_ms"] * 1e-3) / 1e12,
                "achieved": 3 * flops / (acc["k3_ms"] * 1e-3) / 1e12, "unit": "TFLOP/s",
                "peak": tf32_peak(), "frac": 3 * flops / (acc["k3_ms"] * 1e-3) / 1e12 / tf32_peak(),
-               "peak_source": _TF32.get("src"), "note": "3 tf32 MMAs per fp32 product; ncu sm__pipe_tensor_cycles_active of the same "
-                                                         "kernel is in profiles/README.md"},
+               "peak_source": _TF32.get("src"), "note": "3 tf32 MMAs per fp32 product"},
     }
 
 
@@ -552,7 +546,7 @@ def run_partitioned_workload(eng, kind, peak, steps, warmup, world=1, rank=0):
         "dim": dim, "candidates": PART_P * PART_UNL, "labeled": PART_P * PART_LAB, "budget": PART_P * PART_BUDGET,
         "value": PART_P * PART_UNL / (ms * 1e-3), "unit": "samples/s", "ms_per_step": ms, "picks_unique": unique,
         "picks_match_single_gpu": match, "breakdown_ms": acc, "us_per_selection_step": step_ms * 1e3, "loop_variant": out.get("variant"),
-        "roofline": {"kernel": "greedy_persist_kernel, partitions as CTA groups of one launch", "bound": "hbm (L2 when a rank's rows fit the 126 MB L2)",
+        "roofline": {"kernel": "greedy_persist_kernel, partitions as CTA groups of one launch", "bound": "hbm (L2 when a rank's rows fit the 50 MB L2)",
                      "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "bytes_per_row_per_step": row_bytes,
                      "rows_streamed_per_step_on_busiest_rank": nmax * PART_UNL,
                      "note": "a fraction above 1 means the busiest rank's rows (8 000 x 8 KB per partition) are served from L2"},
@@ -732,7 +726,7 @@ def run_own(args):
     # the K-th (the contract's closing synchronize, which also covers the copy stream).  The headline region
     # runs the steps in order on one stream, for every N, so the per-N values are comparable and the CUDA-event
     # pair around the fused kernel times that kernel alone.  At N = 1 a second region reports the throughput with two independent
-    # queries in flight (even/odd steps on two streams / engine contexts: the 148-SM scoring kernel of query
+    # queries in flight (even/odd steps on two streams / engine contexts: the all-SM scoring kernel of query
     # i+1 overlaps the 8-SM top-B cluster kernel of query i; K1 claims its tiles dynamically so CTAs that start
     # late behind the cluster kernel are not stragglers).
     host_out = [torch.empty(BUDGET, dtype=torch.int32).pin_memory() for _ in range(2)]
@@ -806,13 +800,15 @@ def run_own(args):
         per_step = [a.elapsed_time(b) for a, b in pairs]
         return {"ms_total": ev0.elapsed_time(ev1), "k1_ms": float(np.mean(per_step)), "k1_ms_per_step": per_step,
                 "launches": sum(e.launches for e in engines) - l0, "t": (tw0, tenq, tw1),
-                "res": host_out[(steps - 1) & 1].clone()}
+                "res": host_out[(steps - 1) & 1].clone(), "scores": score_bufs[(steps - 1) % depth].clone()}
 
     # one nvidia-smi poller (rank 0's GPU): eight of them next to eight busy-waiting ranks oversubscribe the host cores
     clocks = ClockSampler(local if rank == 0 else -1)
     clocks.__enter__()
     clocks.wait_first(8.0 if rank == 0 else 0.0)
     R = run_region(1, args.steps, max(args.warmup, 3))
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, R["scores"], R["res"] if rank == 0 else None, "" if world == 1 else f"_rank{rank}")
     t_w0, t_enq, t_w1 = R["t"]
     res, launches, ms_total, k1_ms = R["res"], R["launches"], R["ms_total"], R["k1_ms"]
     launches0 = eng.launches - launches
@@ -903,7 +899,7 @@ def run_own(args):
                                "the CUDA events bracket the WHOLE kernel, selection included", "bound": "hbm",
                      "achieved": N_ROWS * (4 * N_CLASSES + 4) / (k1_ms * 1e-3) / 1e9, "peak": peak, "unit": "GB/s",
                      "frac": N_ROWS * (4 * N_CLASSES + 4) / (k1_ms * 1e-3) / 1e9 / peak,
-                     "traffic": ncu_traffic("fused_tail_margin"), "kernel_ms": k1_ms, "peak_source": peak_src,
+                     "kernel_ms": k1_ms, "peak_source": peak_src,
                      "streaming_phase": (None if not stream_ms else {
                          "us": stream_ms * 1e3, "achieved": N_ROWS * (4 * N_CLASSES + 4) / (stream_ms * 1e-3) / 1e9,
                          "frac": N_ROWS * (4 * N_CLASSES + 4) / (stream_ms * 1e-3) / 1e9 / peak, "kernel_us_in_kernel_clock": kern_ms * 1e3,
@@ -977,6 +973,14 @@ def run_own(args):
         dist.destroy_process_group()
 
 
+def dump_outputs(out_dir, scores, positions, suffix):
+    """The arrays the headline path hands its caller, in float32 / float64 (int32 positions are exact in float64)."""
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, f"scores{suffix}.npy"), scores.float().cpu().numpy())
+    if positions is not None:
+        np.save(os.path.join(out_dir, "positions.npy"), positions.cpu().numpy().astype(np.float64))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -985,7 +989,11 @@ def main():
     ap.add_argument("--impl", default="own", choices=["own", "reference"])
     ap.add_argument("--no-extras", action="store_true", help="skip the CoreSet/BADGE workloads (N=1)")
     ap.add_argument("--extra-steps", type=int, default=2)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's scores and positions as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.impl == "reference":
         run_reference(args)
     else:

@@ -1,7 +1,7 @@
 /*
- * alq.h -- C ABI of libalq.so, the B200 (sm_100a) acquisition-scoring engine that replaces the
+ * alq.h -- C ABI of libalq.so, the H100 (sm_90a) acquisition-scoring engine that replaces the
  * per-round query tail of zeyademam/active_learning (`strategy.query(budget)`,
- * src/main_al.py:156).  Citations below are relative to /root/reference/src/query_strategies/.
+ * src/main_al.py:156).  Citations below are relative to active_learning/src/query_strategies/.
  *
  * Conventions
  *   - Every pointer is a DEVICE pointer owned by the caller unless its name ends in `_host`.
@@ -45,11 +45,11 @@ int alq_create(alq_ctx** out, int device);
 void alq_destroy(alq_ctx* ctx);
 const char* alq_last_error(const alq_ctx* ctx);
 /* Implementation knobs (defaults pick the fastest valid kernel):
- *   "k3_impl"        0 auto | 1 exact-fp32 SIMT contraction | 2 tcgen05 3xTF32 contraction
+ *   "k3_impl"        0 auto | 1 exact-fp32 SIMT contraction | 2 wgmma 3xTF32 contraction
  *   "greedy_variant" 0 auto | 1 direct-load step kernel     | 2 bulk-copy (TMA) pipeline | 3 persistent cooperative loop
  *   "l2_resident_mb" persistent selection loop: MB of the rows a GPU streams that are fetched L2::evict_last (the head of every
- *                    CTA's segment) so that they stay in the 126 MB L2 across the B steps; the rest is fetched evict_first.
- *                    Default 64; 0 turns the hints off
+ *                    CTA's segment) so that they stay in the 50 MB L2 across the B steps; the rest is fetched evict_first.
+ *                    Default 24; 0 turns the hints off
  *   "d2_fast_path"   1 (default): the persistent loop's D^2 draw first tries the certified path (one fp64 mass per CTA, the
  *                    rounding of NumPy's float32 probabilities bounded by a margin); 0: always the exact NumPy-tree machinery
  *   "tail_buckets"   1 (default): alq_uncertainty_tail on one GPU routes the candidates to per-CTA score buckets, each CTA sorts

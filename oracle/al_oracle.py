@@ -7,7 +7,7 @@ functions.  Only ``tests/``, ``__graft_entry__.smoke()`` and the ``cpu_baseline`
 ``active_learning_b200/`` imports it and the product path never falls back to it.
 
 Parity status: PINNED.  Every function below is checked against outputs of the reference's
-own code (imported in the build container from /root/reference/src with a comet_ml stub) by
+own code (imported in the build container from active_learning/src with a comet_ml stub) by
 ``tests/golden/make_golden.py``; the resulting vectors are committed under ``tests/golden/``
 and ``tests/test_oracle_golden.py`` replays them.  The one exception is ``entropy`` scoring:
 the reference has no EntropySampler (SURVEY.md finding 1), so that mode is *parity unpinned*
@@ -15,7 +15,7 @@ and its spec is defined here.  The MASE / BASE functions at the end (SURVEY.md s
 are pinned the same way by ``tests/golden/make_golden_mase.py``, ``balancing_query`` by
 ``tests/golden/make_golden_balancing.py``.
 
-All citations are relative to /root/reference/src/query_strategies/.
+All citations are relative to active_learning/src/query_strategies/.
 """
 from __future__ import annotations
 

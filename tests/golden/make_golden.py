@@ -1,11 +1,12 @@
 """Generate the golden vectors under tests/golden/ by RUNNING THE REFERENCE ITSELF.
 
-Only runs in the build container (needs /root/reference).  The reference is imported in place,
-read-only, with a stub for the one missing dependency (comet_ml).  Outputs are small .npz
-files committed next to this script; tests replay them against oracle/ (CPU) and against the
-CUDA path (GPU).  Nothing at test/bench time reads /root/reference.
+Needs a checkout of the reference (zeyademam/active_learning): ALQ_REFERENCE_SRC names its src/
+directory.  The reference is imported in place, read-only, with a stub for the one missing
+dependency (comet_ml).  Outputs are small .npz files committed next to this script; tests replay
+them against oracle/ (CPU) and against the CUDA path (GPU).  Nothing at test/bench time reads the
+reference.
 
-    python tests/golden/make_golden.py
+    ALQ_REFERENCE_SRC=<checkout>/src python tests/golden/make_golden.py
 """
 import os
 import sys
@@ -16,12 +17,14 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-REF = "/root/reference/src"
+REF = os.environ.get("ALQ_REFERENCE_SRC", "")
 OUT = os.path.dirname(os.path.abspath(__file__))
 
 
 # --- import the reference -----------------------------------------------------------------
 def _import_reference():
+    if not os.path.isdir(REF):
+        raise SystemExit("set ALQ_REFERENCE_SRC to the src/ directory of a zeyademam/active_learning checkout")
     stub = types.ModuleType("comet_ml")
 
     class _Exp:

@@ -3,6 +3,7 @@ embeddings of every pool index, and OracleEngine -- an implementation of the Eng
 CPU tensors built from oracle/al_oracle.py.  OracleEngine exists ONLY so the CPU test tier can
 exercise the samplers' host logic (index bookkeeping, RNG order, partition batching, sharding);
 it is never importable from the product package."""
+import hashlib
 import tempfile
 
 import numpy as np
@@ -10,6 +11,12 @@ import torch
 import torch.nn as nn
 
 from oracle import al_oracle as O
+
+
+def digest(a):
+    """SHA-256 of an array's dtype, shape and bytes: equal digests <=> bit-identical arrays (golden fixtures)."""
+    a = np.ascontiguousarray(a.numpy() if isinstance(a, torch.Tensor) else a)
+    return hashlib.sha256(f"{a.dtype.str}{a.shape}".encode() + a.tobytes()).hexdigest()
 
 
 class IndexDataset(torch.utils.data.Dataset):

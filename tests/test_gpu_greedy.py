@@ -121,7 +121,7 @@ def test_min_dist_float_and_factored(eng):
 @pytest.mark.parametrize("n,m,d,c", [(300, 700, 96, 0), (1000, 1000, 2048, 0), (777, 1313, 516, 0),
                                      (500, 600, 64, 40), (640, 900, 2048, 1000)])
 def test_min_dist_tensor_core_path(eng, n, m, d, c):
-    """tcgen05 3xTF32 contraction (k3_impl=2): bit-identical to fp32 on integer rows (lo == 0), within
+    """wgmma 3xTF32 contraction (k3_impl=2): bit-identical to fp32 on integer rows (lo == 0), within
     1e-5 * (|x|^2 + |y|^2) of the fp64 truth on float rows; min and max epilogues; accumulate."""
     rng = np.random.default_rng(n + m + d + c)
     cu = lambda t: t.cuda()

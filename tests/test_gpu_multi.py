@@ -1,6 +1,6 @@
 """Multi-GPU (one process per GPU, NCCL + peer-memory windows): results must equal the single-GPU /
 reference results for every world size.  Needs >= 2 GPUs (skipped otherwise; run with
-`gpurun --gpus 2 -- python -m pytest tests/test_gpu_multi.py -m gpu`)."""
+`python -m pytest tests/test_gpu_multi.py -m gpu` on a machine with two or more H100s)."""
 import os
 import socket
 import sys

@@ -10,7 +10,7 @@ exact iff (1) the key <-> float maps are inverse order isomorphisms, (2) every c
 conditions under which it does so are restated here too."""
 import numpy as np
 
-G = 148
+G = 132                                 # one CTA per SM of an H100
 
 
 def ord_key(f32):                       # alq_ord (alq_common.cuh): monotone float -> uint32

@@ -8,6 +8,7 @@ Every rank holds the full (replicated) arrays -- the engine's multi-GPU contract
 import json
 import os
 import sys
+import tempfile
 import time
 
 import numpy as np
@@ -143,7 +144,7 @@ if ARG in ("big", "bigonly", "tailonly", "tails"):
 dist.barrier()
 if rank == 0:
     print("MGPU GREEDY", "PASS" if ok else "FAIL", flush=True)
-    out = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "gpurun_out")
+    out = os.environ.get("ALQ_CHECK_OUT", tempfile.gettempdir())
     os.makedirs(out, exist_ok=True)
     with open(os.path.join(out, f"mgpu_greedy_check_n{world}.json"), "w") as fh:
         json.dump({"pass": ok, "cases": report}, fh, indent=1)

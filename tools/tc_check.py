@@ -1,4 +1,4 @@
-"""K3 tensor-core path vs the exact SIMT path / torch, with timings (tcgen05 bring-up aid)."""
+"""K3 tensor-core path vs the exact SIMT path / torch, with timings (bring-up aid of the wgmma kernel)."""
 import sys, os, time
 import numpy as np, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
