@@ -242,18 +242,30 @@ def choice_from_uniform(prob32: np.ndarray, u: float) -> int:
     return int(cdf.searchsorted(u, side="right"))
 
 
-def d2_sampling_step(mind32: np.ndarray, labeled: np.ndarray, u: float) -> int:
-    """One randomize=True step of `coreset` with the uniform made explicit
-    (coreset_sampler.py:82-92)."""
+def d2_probabilities(mind32: np.ndarray, labeled: np.ndarray) -> np.ndarray:
+    """The float32 `p` one randomize=True step of `coreset` hands to np.random.choice, including the
+    `sum == 0 -> NaN -> += 1e-5` retry (coreset_sampler.py:82-90)."""
     mind = np.array(mind32, dtype=np.float32, copy=True)
     while True:
         prob = np.clip(mind, 0, None)
         prob[labeled] = 0.0
         prob = prob / np.sum(prob)
         if not np.isnan(prob.sum()):
-            break
+            return prob
         mind += 0.00001
-    return choice_from_uniform(prob, u)
+
+
+def d2_cdf(prob32: np.ndarray) -> np.ndarray:
+    """np.random.choice's normalised fp64 cdf of `prob32` (see `choice_from_uniform`)."""
+    cdf = np.asarray(prob32, dtype=np.float64).cumsum()
+    cdf /= cdf[-1]
+    return cdf
+
+
+def d2_sampling_step(mind32: np.ndarray, labeled: np.ndarray, u: float) -> int:
+    """One randomize=True step of `coreset` with the uniform made explicit
+    (coreset_sampler.py:82-92)."""
+    return choice_from_uniform(d2_probabilities(mind32, labeled), u)
 
 
 def coreset_streaming(feat: torch.Tensor, labeled_indicator: np.ndarray, query_count: int,
@@ -261,7 +273,9 @@ def coreset_streaming(feat: torch.Tensor, labeled_indicator: np.ndarray, query_c
     """Same picks as `coreset(pairwise_l2_dist(feat), ...)` but O(N) memory: running min of
     fl(fl(n_i+n_q) - 2*dot) against each new centre (min is exact, SURVEY.md finding 4).
     Used for the parity cases too large for a dense N x N matrix.  With `uniforms` given the
-    RNG is not touched.
+    RNG is not touched; `uniforms` is either an array (u of step t = uniforms[t]) or a callable
+    u = uniforms(t, cdf) that sees np.random.choice's normalised cdf of step t (`d2_cdf`), so a test can
+    place u exactly on, or just beside, a cdf breakpoint.
 
     factors: BADGE's second factor a[n, C].  The row of the reference's matrix is the gradient embedding
     g_i = a_i (x) h_i (badge_sampler.py:40) with h = feat; it is rank-1 (SURVEY.md finding 6), so
@@ -298,13 +312,13 @@ def coreset_streaming(feat: torch.Tensor, labeled_indicator: np.ndarray, query_c
         if lab.sum() == 0:
             raise ValueError("coreset_streaming needs at least one labeled row")
         if randomize:
-            u = float(uniforms[t]) if uniforms is not None else float(np.random.random_sample())
-            q = d2_sampling_step(mind.numpy(), lab, u)
+            cdf = d2_cdf(d2_probabilities(mind.numpy(), lab))
+            if callable(uniforms):
+                u = float(uniforms(t, cdf))
+            else:
+                u = float(uniforms[t]) if uniforms is not None else float(np.random.random_sample())
+            q = int(cdf.searchsorted(u, side="right"))
             if certificate is not None:
-                prob = np.clip(mind.numpy(), 0, None)
-                prob[lab] = 0.0
-                cdf = (prob / np.sum(prob)).astype(np.float64).cumsum()
-                cdf /= cdf[-1]
                 near = [abs(cdf[q] - u)] + ([abs(u - cdf[q - 1])] if q > 0 else [])
                 certificate.append(float(min(near)))
         else:

@@ -19,6 +19,44 @@ def digest(a):
     return hashlib.sha256(f"{a.dtype.str}{a.shape}".encode() + a.tobytes()).hexdigest()
 
 
+class BoundaryUniforms:
+    """Adversarial uniforms for the D^2 draw, as the callable form of `O.coreset_streaming(uniforms=...)`: step t's u is
+    placed on, or just beside, a breakpoint of that step's cdf, rotating through
+      cdf[k] for a random k with positive mass, nextafter(cdf[k], 0 / 1), cdf[k] +- {1.0, 1.3, 1.5, 2.5, 5}e-7,
+      cdf at the last position of a CTA segment (`seg_end_pos`, if given), u = 0 and u = 1 - 2^-53.
+    The values handed out are kept in `us`, so the GPU can be fed the very same array."""
+    OFFSETS = (1.0e-7, 1.3e-7, 1.5e-7, 2.5e-7, 5e-7)
+    U_MAX = 1.0 - 2.0 ** -53
+
+    def __init__(self, seed, seg_end_pos=None):
+        self.rng = np.random.default_rng(seed)
+        self.seg_end_pos = list(seg_end_pos) if seg_end_pos is not None else []
+        self.kinds = ["at", "below", "above"] + [s * o for o in self.OFFSETS for s in (1, -1)] + ["seg", "zero", "one"]
+        self.us = []
+
+    def __call__(self, t, cdf):
+        kind = self.kinds[t % len(self.kinds)]
+        pos = np.flatnonzero((np.diff(cdf, prepend=0.0) > 0) & (cdf < 1.0))    # breakpoints of positive-mass entries
+        b = float(cdf[pos[self.rng.integers(len(pos))]]) if len(pos) else 0.5
+        if kind == "below":
+            u = np.nextafter(b, 0.0)
+        elif kind == "above":
+            u = np.nextafter(b, 1.0)
+        elif kind == "seg":
+            u = float(cdf[self.seg_end_pos[(t // len(self.kinds)) % len(self.seg_end_pos)]]) if self.seg_end_pos else b
+        elif kind == "zero":
+            u = 0.0
+        elif kind == "one":
+            u = self.U_MAX
+        elif kind == "at":
+            u = b
+        else:
+            u = b + kind
+        u = float(min(max(u, 0.0), self.U_MAX))
+        self.us.append(u)
+        return u
+
+
 class IndexDataset(torch.utils.data.Dataset):
     def __init__(self, n, num_classes):
         self.n, self.num_classes = n, num_classes

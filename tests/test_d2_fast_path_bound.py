@@ -7,7 +7,9 @@ draws many mass vectors (wide dynamic range, zeros, tiny and huge entries) and u
 right at cdf breakpoints -- and checks that EVERY certified decision equals NumPy's, and that certification fails only
 for uniforms within a few 1e-7 of a breakpoint."""
 import numpy as np
+import torch
 
+from helpers import BoundaryUniforms
 from oracle import al_oracle as O
 
 MARGIN = 1.3e-7
@@ -62,6 +64,27 @@ def test_certified_decisions_equal_numpy_and_uncertain_ones_are_near_breakpoints
                 checked += 1
                 assert got == want, (trial, u, got, want)
     assert checked > 8000 and uncertain > 100          # both branches were exercised
+
+
+def test_callable_uniforms_equal_the_array_form():
+    """`coreset_streaming` with u = f(t, cdf) picks what the array form picks when fed the values f returned, and the
+    boundary schedule the GPU tests use really lands on and just beside cdf breakpoints."""
+    rng = np.random.default_rng(5)
+    n, l0, b = 3000, 300, 64
+    for c in (0, 8):
+        h = torch.from_numpy(rng.integers(-1, 2, size=(n, 16)).astype(np.float32))
+        a = torch.from_numpy(rng.integers(-1, 2, size=(n, c)).astype(np.float32)) if c else None
+        ind = np.zeros(n, dtype=bool)
+        ind[rng.choice(n, l0, replace=False)] = True
+        f = BoundaryUniforms(c, seg_end_pos=np.flatnonzero(~ind)[[99, 1999, -1]])
+        cert_f, cert_a = [], []
+        got = O.coreset_streaming(h, ind, b, randomize=True, uniforms=f, factors=a, certificate=cert_f)
+        assert len(f.us) == b and all(0.0 <= u < 1.0 for u in f.us)
+        assert got == O.coreset_streaming(h, ind, b, randomize=True, uniforms=np.array(f.us), factors=a,
+                                          certificate=cert_a)
+        assert cert_f == cert_a
+        assert sum(x < 1e-8 for x in cert_f) >= 10
+        assert sum(1.3e-7 < x <= 5e-7 for x in cert_f) >= 10
 
 
 def test_uncertain_fraction_at_the_north_star_size_is_a_few_percent():

@@ -19,23 +19,24 @@ def _split(feat, ind):
     return cand, lab, feat[cand].cuda(), feat[lab].cuda()
 
 
-def _run(eng, feat, ind, b, randomize=False, uniforms=None, variant=0, first=None, factors=None):
+def _run(eng, feat, ind, b, randomize=False, uniforms=None, variant=0, first=None, factors=None, time_steps=False):
     """Reference-shaped call: dense rows `feat`, boolean labeled indicator -> picks as rows of feat.
     The persistent loop's D^2 draw (variant 3) is run twice -- certified fast path first (default) and exact
-    NumPy-tree machinery only -- and both must give the same list."""
+    NumPy-tree machinery only -- and both must give the same list.  With time_steps the loop reports what ran in
+    `eng.last_greedy_timing` (its "variant" is the one that ran, also under variant=0)."""
     if randomize and variant == 3:
         try:
             eng.set_option("d2_fast_path", 0)
-            exact = _run_once(eng, feat, ind, b, randomize, uniforms, variant, first, factors)
+            exact = _run_once(eng, feat, ind, b, randomize, uniforms, variant, first, factors, time_steps)
         finally:
             eng.set_option("d2_fast_path", 1)
-        fast = _run_once(eng, feat, ind, b, randomize, uniforms, variant, first, factors)
+        fast = _run_once(eng, feat, ind, b, randomize, uniforms, variant, first, factors, time_steps)
         assert fast == exact, "certified fast path and exact path disagree"
         return fast
-    return _run_once(eng, feat, ind, b, randomize, uniforms, variant, first, factors)
+    return _run_once(eng, feat, ind, b, randomize, uniforms, variant, first, factors, time_steps)
 
 
-def _run_once(eng, feat, ind, b, randomize=False, uniforms=None, variant=0, first=None, factors=None):
+def _run_once(eng, feat, ind, b, randomize=False, uniforms=None, variant=0, first=None, factors=None, time_steps=False):
     cand, lab, X, Y = _split(feat, ind)
     xn = eng.row_norm2(X)
     XA = YA = xan = yan = None
@@ -50,7 +51,10 @@ def _run_once(eng, feat, ind, b, randomize=False, uniforms=None, variant=0, firs
                               uniforms=uniforms if randomize else None,
                               vpos=torch.as_tensor(cand.astype(np.int32)).cuda() if randomize else None,
                               full_n=[len(ind)] if randomize else None,
-                              first_pick=[first] if first is not None else None, variant=variant)
+                              first_pick=[first] if first is not None else None, variant=variant,
+                              time_steps=time_steps)
+    if time_steps:
+        picks = picks[0]
     return cand[picks].tolist()
 
 
@@ -118,16 +122,23 @@ def test_min_dist_float_and_factored(eng):
     assert torch.equal(got, d2[:100, 100:].min(1).values)
 
 
+_SUB_TILE = [(n, m, (32, 36)[i % 2], (0, 32, 36)[i % 3]) for i, (n, m) in
+             enumerate((n, m) for n in (1, 127, 129) for m in (1, 127, 129))]
+
+
 @pytest.mark.parametrize("n,m,d,c", [(300, 700, 96, 0), (1000, 1000, 2048, 0), (777, 1313, 516, 0),
-                                     (500, 600, 64, 40), (640, 900, 2048, 1000)])
+                                     (500, 600, 64, 40), (640, 900, 2048, 1000),
+                                     # 24 row blocks of 2 MB at d = 2048, 8 live per round: 3 rounds of the work list
+                                     (3000, 1500, 2048, 0), (3000, 1500, 2048, 1000)] + _SUB_TILE)
 def test_min_dist_tensor_core_path(eng, n, m, d, c):
-    """wgmma 3xTF32 contraction (k3_impl=2): bit-identical to fp32 on integer rows (lo == 0), within
-    1e-5 * (|x|^2 + |y|^2) of the fp64 truth on float rows; min and max epilogues; accumulate."""
+    """wgmma 3xTF32 contraction (k3_impl=2): bit-identical to fp32 on integer rows (lo == 0) and to the SIMT kernel
+    (k3_impl=1), within 1e-5 * (|x|^2 + |y|^2) of the fp64 truth on float rows; min and max epilogues; accumulate.
+    Shapes span several rounds of the work list and blocks smaller than one 128 x 128 tile."""
     rng = np.random.default_rng(n + m + d + c)
     cu = lambda t: t.cuda()
     try:
-        eng.set_option("k3_impl", 2)
         for ints in (True, False):
+            eng.set_option("k3_impl", 2)
             if ints:
                 x = torch.from_numpy(rng.integers(-1, 2, size=(n, d)).astype(np.float32))
                 y = torch.from_numpy(rng.integers(-1, 2, size=(m, d)).astype(np.float32))
@@ -149,14 +160,116 @@ def test_min_dist_tensor_core_path(eng, n, m, d, c):
             assert (got - d2.min(1).values).abs().max() <= tol
             got = eng.min_dist(*args, reduce_max=True).cpu().double()
             assert (got - d2.max(1).values).abs().max() <= tol
+            if ints:
+                tc = eng.min_dist(*args).cpu(), eng.min_dist(*args, reduce_max=True).cpu()
+                eng.set_option("k3_impl", 1)
+                assert torch.equal(tc[0], eng.min_dist(*args).cpu())
+                assert torch.equal(tc[1], eng.min_dist(*args, reduce_max=True).cpu())
+        eng.set_option("k3_impl", 2)
         out = torch.full((n,), float("inf"), device="cuda")      # accumulate over column chunks
         half = m // 2
         for sl in (slice(0, half), slice(half, m)):
+            if sl.stop == sl.start:
+                continue
             a2 = [args[0], args[1], args[2][sl], args[3][sl]]
             if c:
                 a2 += [args[4], args[5], args[6][sl], args[7][sl]]
             eng.min_dist(*a2, out=out, accumulate=True)
         assert (out.cpu().double() - d2.min(1).values).abs().max() <= tol
+    finally:
+        eng.set_option("k3_impl", 0)
+
+
+@pytest.mark.parametrize("c", [0, 1000])
+def test_min_dist_tensor_core_work_split_is_bit_invariant(eng, monkeypatch, c):
+    """How the tensor-core path cuts its work list -- one 2 MB row block per round (ALQ_K3_LIVE_MB=1: 24 rounds, many
+    items per CTA), the default 16 MB (3 rounds of 8 blocks) or all 24 blocks in one round (64) -- only moves which CTA
+    computes a distance: every distance is the same arithmetic and min / max are exact, so the results are bit-identical."""
+    g = torch.Generator().manual_seed(7 + c)
+    n, m, d = 3000, 1500, 2048
+    x, y = torch.relu(torch.randn(n, d, generator=g)).cuda(), torch.relu(torch.randn(m, d, generator=g)).cuda()
+    args = [x, eng.row_norm2(x), y, eng.row_norm2(y)]
+    if c:
+        xa, ya = (torch.randn(n, c, generator=g) * 0.05).cuda(), (torch.randn(m, c, generator=g) * 0.05).cuda()
+        args += [xa, eng.row_norm2(xa), ya, eng.row_norm2(ya)]
+    try:
+        eng.set_option("k3_impl", 2)
+        monkeypatch.delenv("ALQ_K3_LIVE_MB", raising=False)
+        ref = eng.min_dist(*args).cpu(), eng.min_dist(*args, reduce_max=True).cpu()
+        for live_mb in ("1", "64"):
+            monkeypatch.setenv("ALQ_K3_LIVE_MB", live_mb)
+            assert torch.equal(eng.min_dist(*args).cpu(), ref[0]), live_mb
+            assert torch.equal(eng.min_dist(*args, reduce_max=True).cpu(), ref[1]), live_mb
+    finally:
+        eng.set_option("k3_impl", 0)
+
+
+@pytest.mark.parametrize("c", [0, 40])
+def test_min_dist_strided_operands(eng, c):
+    """X, Y and the factors as column slices of wider slabs (leading dimension d + 12): both K3 implementations give
+    bit-for-bit what they give on contiguous copies."""
+    g = torch.Generator().manual_seed(30 + c)
+    n, m, d = 300, 500, 64
+    slab = lambda r, k: torch.relu(torch.randn(r, k + 12, generator=g)).cuda()[:, 4:4 + k]    # 16-byte aligned base
+    x, y = slab(n, d), slab(m, d)
+    ops = [x, y] + ([slab(n, c), slab(m, c)] if c else [])
+    assert all(t.stride(0) == t.shape[1] + 12 for t in ops)
+    dense = [t.contiguous() for t in ops]
+    for t, u in zip(ops, dense):
+        assert torch.equal(eng.row_norm2(t), eng.row_norm2(u))
+    norms = [eng.row_norm2(u) for u in dense]
+
+    def call(o, **kw):
+        a = [o[0], norms[0], o[1], norms[1]]
+        if c:
+            a += [o[2], norms[2], o[3], norms[3]]
+        return eng.min_dist(*a, **kw).cpu()
+    try:
+        for impl in (1, 2):
+            eng.set_option("k3_impl", impl)
+            for kw in ({}, {"reduce_max": True}):
+                assert torch.equal(call(ops, **kw), call(dense, **kw)), (impl, kw)
+    finally:
+        eng.set_option("k3_impl", 0)
+
+
+def test_min_dist_near_duplicates_and_negative_distances(eng):
+    """Y holds exact copies of a third of X's float rows and copies that differ by one ulp in one entry.  The caller's
+    norms of X are a relative 2^-16 low (norms computed in another order or precision differ the same way, only less),
+    so exactly the rows with a copy in Y have a negative minimum, and the float atomics see negative and positive
+    partial results from two column chunks (min and max, `accumulate`).  Both implementations stay within the fp64
+    bound of the same expression and agree with the one-shot call bit for bit."""
+    g = torch.Generator().manual_seed(12)
+    n, d = 699, 256
+    x = torch.relu(torch.randn(n, d, generator=g)) + 0.01
+    third = torch.randperm(n, generator=g)[:n // 3]
+    bumped = x[third].clone()
+    col = torch.randint(0, d, (len(third),), generator=g)
+    rows = torch.arange(len(third))
+    bumped[rows, col] = torch.from_numpy(np.nextafter(bumped[rows, col].numpy(), np.float32(np.inf)))
+    y = torch.cat([x[third], bumped, torch.relu(torch.randn(100, d, generator=g))])
+    y = y[torch.randperm(len(y), generator=g)]
+    X, Y = x.cuda(), y.cuda()
+    xn, yn = eng.row_norm2(X) * (1.0 - 2.0 ** -16), eng.row_norm2(Y)
+    xd, yd = x.double(), y.double()
+    d2 = (xn.cpu().double()[:, None] + yn.cpu().double()[None, :]) - 2 * (xd @ yd.T)
+    tol = 1e-5 * float(xd.square().sum(1).max() + yd.square().sum(1).max())
+    has_copy = torch.zeros(n, dtype=torch.bool)
+    has_copy[third] = True
+    half = len(y) // 2
+    try:
+        for impl in (1, 2):
+            eng.set_option("k3_impl", impl)
+            got = eng.min_dist(X, xn, Y, yn).cpu()
+            assert (got.double() - d2.min(1).values).abs().max() <= tol, impl
+            assert torch.equal(got < 0, has_copy), impl
+            for reduce_max, init, truth in ((False, float("inf"), d2.min(1).values), (True, float("-inf"), d2.max(1).values)):
+                out = torch.full((n,), init, device="cuda")
+                for sl in (slice(0, half), slice(half, len(y))):
+                    eng.min_dist(X, xn, Y[sl], yn[sl], reduce_max=reduce_max, out=out, accumulate=True)
+                assert (out.cpu().double() - truth).abs().max() <= tol, (impl, reduce_max)
+                one = eng.min_dist(X, xn, Y, yn, reduce_max=reduce_max).cpu()
+                assert torch.equal(out.cpu(), one), (impl, reduce_max)
     finally:
         eng.set_option("k3_impl", 0)
 
@@ -266,10 +379,24 @@ def test_badge_factored_equals_materialised_reference(eng):
 
 def test_partitions_are_a_batch_dimension(eng):
     """One batched launch over P partitions == P separate runs (argmax and sampling)."""
+    _check_partition_batch(eng, False, [700, 1301, 64, 999], [80, 0, 10, 200], [30, 29, 5, 30])
+
+
+def test_partitions_with_edge_budgets_equal_the_oracle(eng):
+    """Budgets of 0 between active partitions, a budget equal to the partition size, budget 1 with first_pick (no
+    selection step): the batched launch == P separate runs == the oracle per partition (integer rows, exact)."""
+    _check_partition_batch(eng, True, [300, 57, 400, 120, 90, 64], [20, 5, 0, 7, 30, 0], [25, 0, 1, 0, 90, 12])
+
+
+def _check_partition_batch(eng, ints, sizes, labs, budgets):
+    """Runs P partitions (the first labs[p] rows of each labeled; first_pick 17 where none are) one by one and as one
+    batched launch under variants 2 and 3; with integer rows every partition is also compared with its oracle run."""
     rng = np.random.default_rng(21)
-    sizes, labs, budgets = [700, 1301, 64, 999], [80, 0, 10, 200], [30, 29, 5, 30]
-    feats = [torch.relu(torch.randn(s + l, 512, generator=torch.Generator().manual_seed(i)))
-             for i, (s, l) in enumerate(zip(sizes, labs))]
+    if ints:
+        feats = [torch.from_numpy(rng.integers(-1, 2, size=(s + l, 16)).astype(np.float32)) for s, l in zip(sizes, labs)]
+    else:
+        feats = [torch.relu(torch.randn(s + l, 512, generator=torch.Generator().manual_seed(i)))
+                 for i, (s, l) in enumerate(zip(sizes, labs))]
     for randomize in (False, True):
         us = [rng.random(b) for b in budgets]
         solo, X, mind, vpos, first = [], [], [], [], []
@@ -280,6 +407,14 @@ def test_partitions_are_a_batch_dimension(eng):
             if labs[p] == 0:
                 fp = 17
             solo.append(_run(eng, f, ind, budgets[p], randomize=randomize, uniforms=us[p], first=fp))
+            if ints and budgets[p]:
+                if fp is None:
+                    ref = O.coreset_streaming(f, ind, budgets[p], randomize=randomize, uniforms=us[p])
+                else:                         # the caller's centre 0 is labeled first and uses no uniform
+                    ind0 = ind.copy()
+                    ind0[fp] = True
+                    ref = [fp] + O.coreset_streaming(f, ind0, budgets[p] - 1, randomize=randomize, uniforms=us[p][1:])
+                assert solo[p] == ref, (randomize, p)
             Xp = f[labs[p]:].cuda()
             X.append(Xp)
             m = torch.full((sizes[p],), float("inf"), device="cuda")
@@ -298,7 +433,7 @@ def test_partitions_are_a_batch_dimension(eng):
                                       full_n=[s + l for s, l in zip(sizes, labs)] if randomize else None,
                                       first_pick=first, variant=variant)
             at = 0
-            for p in range(4):
+            for p in range(len(sizes)):
                 got = (picks[at:at + budgets[p]] - off[p] + labs[p]).tolist()
                 assert got == solo[p], (randomize, p, variant)
                 at += budgets[p]
