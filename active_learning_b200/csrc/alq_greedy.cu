@@ -367,7 +367,6 @@ struct SampleArgs {
     int* picks;
     int* status;                 // sticky error flag
     int t;
-    long long* dbg;              // optional phase timestamps (ALQ_SAMPLE_DEBUG=1), 8 per launch
 };
 
 constexpr int kSampThreads = 1024;
@@ -384,8 +383,6 @@ constexpr int kCL = 8;             // CTAs per cluster == per partition (portabl
 // Prefixes are built as ONE sequential chain (rank order, then warp order, then lane order), so the
 // "interval contains u" predicates of neighbouring CTAs / warps / threads are computed from
 // identical values and exactly one thread claims the draw.
-#define ALQ_STAMP(i) do { if (A.dbg && threadIdx.x == 0 && rank == 0) A.dbg[A.t * 8 + (i)] = clock64(); } while (0)
-
 __global__ void __cluster_dims__(kCL, 1, 1) __launch_bounds__(kSampThreads, 1)
 sample_cluster_kernel(SampleArgs A) {
     extern __shared__ float val[];                 // 2*n_leaves tree nodes, then the combine schedule (ints)
@@ -415,7 +412,6 @@ sample_cluster_kernel(SampleArgs A) {
         if (threadIdx.x <= S.n_levels && threadIdx.x < 40) s_level_off[threadIdx.x] = A.level_off[S.level_base + threadIdx.x];
     }
 
-    ALQ_STAMP(0);
     float total32 = 0.f;
     for (int attempt = 0;; ++attempt) {
         // ---- stage A: np.sum(prob) ---------------------------------------------------------------
@@ -431,9 +427,7 @@ sample_cluster_kernel(SampleArgs A) {
                 if (g_lane == 0) leafval[leaf] = v;
             }
         }
-        ALQ_STAMP(1);
         cluster_sync_all();
-        ALQ_STAMP(2);
         for (int i = threadIdx.x; i < K; i += kSampThreads) val[i] = __ldcg(leafval + i);
         asm volatile("cp.async.wait_all;" ::: "memory");
         __syncthreads();
@@ -465,7 +459,6 @@ sample_cluster_kernel(SampleArgs A) {
         cluster_sync_all();
     }
 
-    ALQ_STAMP(3);
     // ---- stage B: np.random.choice == first k with cumsum64(p)[k] / total > u ---------------------
     const double u = A.uniforms[S.pick_off + t];
     const int npad = (n + 3) & ~3;
@@ -501,7 +494,6 @@ sample_cluster_kernel(SampleArgs A) {
             }
         }
     }
-    ALQ_STAMP(7);
     double inc = loc;                                               // inclusive scan inside the warp
 #pragma unroll
     for (int o = 1; o < 32; o <<= 1) {
@@ -517,15 +509,12 @@ sample_cluster_kernel(SampleArgs A) {
         cta_total += sh_w[w];
     }
     if (threadIdx.x == 0) A.cta_part[p * kCL + rank] = cta_total;
-    ALQ_STAMP(4);
     cluster_sync_all();
-    ALQ_STAMP(5);
     double pre = 0.0, total = 0.0;                                  // ... and over CTAs
     for (int q = 0; q < kCL; ++q) {
         if (q == rank) pre = total;
         total += __ldcg(&A.cta_part[p * kCL + q]);
     }
-    ALQ_STAMP(6);
     const double cta_after = pre + cta_total;
     const bool cta_claims = !(rank > 0 && (pre / total) > u) && ((cta_after / total) > u || rank == kCL - 1);
     if (!cta_claims) return;
@@ -584,31 +573,27 @@ sample_cluster_kernel(SampleArgs A) {
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-struct TreeBuilder {
-    std::vector<int> leaf_off;                   // per partition: n_leaves + 1
-    std::vector<std::vector<int>> by_height;     // internal nodes (dst,l,r) grouped by height
-    int next_internal = 0;
-
-    // returns (node id, height)
-    std::pair<int, int> rec(int lo, int m) {
-        if (m <= 128) {
-            leaf_off.push_back(lo);
-            return {static_cast<int>(leaf_off.size()) - 1, 0};
-        }
-        int half = m / 2;
-        half -= half % 8;
-        auto L = rec(lo, half);
-        auto R = rec(lo + half, m - half);
-        const int h = std::max(L.second, R.second) + 1;
-        if (static_cast<int>(by_height.size()) < h) by_height.resize(h);
-        by_height[h - 1].push_back(-1);          // dst patched once the leaf count is known
-        by_height[h - 1].push_back(L.first);
-        by_height[h - 1].push_back(R.first);
-        internal_refs.push_back({h - 1, static_cast<int>(by_height[h - 1].size()) - 3});
-        return {-static_cast<int>(internal_refs.size()), h};   // negative = internal #(k-1)
+// A partition's tree as sample_cluster_kernel reads it: leaf offsets, then the internal nodes as (dst, l, r) triples
+// grouped by height, internal node k (creation order) being node K + k.  Returns the leaf count K.
+int append_sample_tree(const PairTree& tb, PartSched& S, std::vector<int>& leaf_off_all, std::vector<int>& level_off_all,
+                       std::vector<int>& comb_all) {
+    const int K = tb.n_leaves();
+    auto node_id = [K](int v) { return v >= 0 ? v : K + (-v - 1); };
+    S.n_leaves = K;
+    S.leaf_base = static_cast<int>(leaf_off_all.size());
+    leaf_off_all.insert(leaf_off_all.end(), tb.leaf_off.begin(), tb.leaf_off.end());
+    S.root = tb.internal.empty() ? 0 : K + static_cast<int>(tb.internal.size()) - 1;
+    S.n_levels = tb.n_levels();
+    S.level_base = static_cast<int>(level_off_all.size());
+    level_off_all.insert(level_off_all.end(), tb.level_off.begin(), tb.level_off.end());
+    S.comb_base = static_cast<int>(comb_all.size() / 3);
+    for (int k : tb.order) {
+        comb_all.push_back(K + k);
+        comb_all.push_back(node_id(tb.internal[k].l));
+        comb_all.push_back(node_id(tb.internal[k].r));
     }
-    std::vector<std::pair<int, int>> internal_refs;
-};
+    return K;
+}
 
 template <bool FACTORED, bool SAMPLE>
 void launch_step(int variant, int grid, cudaStream_t st, const StepArgs& A, const PipeCfg& cfg, size_t smem_v1,
@@ -694,10 +679,6 @@ extern "C" int alq_greedy_select(alq_ctx* ctx, const alq_greedy_desc* D, void* s
     PipeCfg cfg{};
     size_t smem_v2 = 0;
     int variant = D->variant ? D->variant : ctx->greedy_variant;
-    if (variant == 0) {
-        const char* env = getenv("ALQ_GREEDY_VARIANT");   // debugging aid: force a variant
-        if (env && env[0] >= '1' && env[0] <= '3' && env[1] == 0) variant = env[0] - '0';
-    }
     if (variant == 0 || variant == 3 || comm) {
         // the whole loop as one persistent cooperative launch (alq_greedy_persist.cu)
         const int rc3 = alq_greedy_persist(ctx, D, stream);
@@ -751,33 +732,7 @@ extern "C" int alq_greedy_select(alq_ctx* ctx, const alq_greedy_desc* D, void* s
             S.row_hi = D->part_off_host[p + 1];
             S.pick_off = pick_off[p];
             S.budget = D->budget_host[p];
-            TreeBuilder tb;
-            auto root = tb.rec(0, S.full_n);
-            const int K = static_cast<int>(tb.leaf_off.size());
-            tb.leaf_off.push_back(S.full_n);
-            S.n_leaves = K;
-            S.leaf_base = static_cast<int>(leaf_off_all.size());
-            leaf_off_all.insert(leaf_off_all.end(), tb.leaf_off.begin(), tb.leaf_off.end());
-            // number internal nodes K, K+1, ... in creation order and patch references
-            auto node_id = [&](int v) { return v >= 0 ? v : K + (-v - 1); };
-            for (size_t k = 0; k < tb.internal_refs.size(); ++k) {
-                auto& ref = tb.internal_refs[k];
-                int* e = &tb.by_height[ref.first][ref.second];
-                e[0] = K + static_cast<int>(k);
-                e[1] = node_id(e[1]);
-                e[2] = node_id(e[2]);
-            }
-            S.root = node_id(root.first);
-            S.n_levels = static_cast<int>(tb.by_height.size());
-            S.level_base = static_cast<int>(level_off_all.size());
-            S.comb_base = static_cast<int>(comb_all.size() / 3);
-            int run = 0;
-            for (auto& lv : tb.by_height) {
-                level_off_all.push_back(run);
-                comb_all.insert(comb_all.end(), lv.begin(), lv.end());
-                run += static_cast<int>(lv.size() / 3);
-            }
-            level_off_all.push_back(run);
+            const int K = append_sample_tree(PairTree(S.full_n), S, leaf_off_all, level_off_all, comb_all);
             max_nodes = std::max(max_nodes, 2 * K);
         }
         if (static_cast<size_t>(max_nodes) * sizeof(float) * 5 / 2 > ctx->smem_optin - 16 * 1024)
@@ -860,12 +815,6 @@ extern "C" int alq_greedy_select(alq_ctx* ctx, const alq_greedy_desc* D, void* s
         SA.cfull = d_cfull; SA.posinv = d_posinv;
         SA.leafval = d_leafval; SA.cta_part = d_cta_part; SA.uniforms = d_unif; SA.first_pick = d_first; SA.cur = d_cur;
         SA.picks = D->picks; SA.status = d_status;
-        if (getenv("ALQ_SAMPLE_DEBUG")) {
-            static long long* dbg_buf = nullptr;
-            if (!dbg_buf) cudaMalloc(&dbg_buf, 64 * 8 * sizeof(long long));
-            cudaMemsetAsync(dbg_buf, 0, 64 * 8 * sizeof(long long), st);
-            SA.dbg = bmax <= 64 ? dbg_buf : nullptr;
-        }
         samp_smem = static_cast<size_t>(max_nodes) * sizeof(float) * 5 / 2 + 64;   // nodes + 3 ints per internal node
         if (samp_smem > 32 * 1024)
             ALQ_CUDA(ctx, cudaFuncSetAttribute(sample_cluster_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -932,16 +881,6 @@ extern "C" int alq_greedy_select(alq_ctx* ctx, const alq_greedy_desc* D, void* s
         // the sampling variant reports a sticky numeric status; timing needs the events resolved
         ALQ_CUDA(ctx, cudaMemcpyAsync(&status, d_status, sizeof(int), cudaMemcpyDeviceToHost, st));
         ALQ_CUDA(ctx, cudaStreamSynchronize(st));
-    }
-    if (sample && SA.dbg) {
-        std::vector<long long> hd(64 * 8);
-        cudaMemcpy(hd.data(), SA.dbg, hd.size() * sizeof(long long), cudaMemcpyDeviceToHost);
-        for (int t = 0; t < std::min(bmax, 6); ++t) {
-            fprintf(stderr, "[alq sample dbg] t=%d cycles:", t);
-            for (int i = 1; i < 7; ++i) fprintf(stderr, " %lld", hd[t * 8 + i] - hd[t * 8 + i - 1]);
-            fprintf(stderr, " | stageB loads+loc %lld scan+publish %lld", hd[t * 8 + 7] - hd[t * 8 + 3], hd[t * 8 + 4] - hd[t * 8 + 7]);
-            fprintf(stderr, "\n");
-        }
     }
     if (timing) {
         double acc = 0.0;

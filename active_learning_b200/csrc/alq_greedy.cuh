@@ -87,6 +87,47 @@ static void build_segments(int P, const int32_t* part_off, const int32_t* budget
     }
 }
 
+// NumPy's pairwise-summation tree over n entries: a run of at most 128 entries is a leaf, a longer run of m entries
+// splits at m / 2 rounded down to a multiple of 8.  Every D^2 pick rests on this rule being bit-exact.  Both D^2 loops
+// (and alq_pairwise_leaf_bounds) read their trees from here.
+struct PairTree {
+    std::vector<int> leaf_off;                       // n_leaves + 1 entries, the last one is n
+    struct Node { int height, l, r; };               // children: >= 0 leaf id, < 0 internal #(-v - 1)
+    std::vector<Node> internal;                      // creation (post-) order: the root is the last one
+    std::vector<int> order;                          // internal nodes by height 1, 2, .., creation order within a height
+    std::vector<int> level_off;                      // n_levels + 1 offsets into `order`
+
+    explicit PairTree(int n) {
+        rec(0, n);
+        leaf_off.push_back(n);
+        int hmax = 0;
+        for (const Node& nd : internal) hmax = std::max(hmax, nd.height);
+        level_off.assign(hmax + 1, 0);
+        for (const Node& nd : internal) ++level_off[nd.height];          // count per height, then exclusive prefix
+        for (int h = 1; h <= hmax; ++h) level_off[h] += level_off[h - 1];
+        std::vector<int> at(level_off.begin(), level_off.end() - 1);
+        order.resize(internal.size());
+        for (size_t k = 0; k < internal.size(); ++k) order[at[internal[k].height - 1]++] = static_cast<int>(k);
+    }
+    int n_leaves() const { return static_cast<int>(leaf_off.size()) - 1; }
+    int n_levels() const { return static_cast<int>(level_off.size()) - 1; }
+
+private:
+    std::pair<int, int> rec(int lo, int m) {         // -> (ref, height)
+        if (m <= 128) {
+            leaf_off.push_back(lo);
+            return {static_cast<int>(leaf_off.size()) - 1, 0};
+        }
+        int half = m / 2;
+        half -= half % 8;
+        const auto L = rec(lo, half);
+        const auto R = rec(lo + half, m - half);
+        const int h = std::max(L.second, R.second) + 1;
+        internal.push_back({h, L.first, R.first});
+        return {-static_cast<int>(internal.size()), h};
+    }
+};
+
 
 }  // namespace
 

@@ -624,8 +624,6 @@ greedy_persist_kernel(const __grid_constant__ PersistArgs A, const PipeCfg cfg, 
     int centre = -1;
     const bool prof = A.prof != nullptr && blockIdx.x == 0 && ct == 0;
     if (prof) { for (int i = 0; i < 10; ++i) ss.prof[i] = 0; ss.prof[9] = gtime_ns(); }
-    const int dbg_step = G.budget / 2;
-    unsigned long long* const dbg = (A.prof != nullptr && ct == 0) ? A.prof + 8 + 8 * blockIdx.x : nullptr;   // per-CTA stamps of one step
 
     for (int t = 0; t < G.budget; ++t) {
         unsigned long long best_key = 0ull;   // arg-max: ord(min-distance) << 32 | ~(row - seg.row_lo)
@@ -739,7 +737,6 @@ greedy_persist_kernel(const __grid_constant__ PersistArgs A, const PipeCfg cfg, 
             if (lane == 0) sbest[cw] = best_key;
             cons_bar();
             if (prof) ss.prof[8] = gtime_ns();
-            if (dbg && t == dbg_step) dbg[0] = gtime_ns();
             const unsigned int tag16 = 0x8000u | ((A.tag_base >> 12) & 0x7000u) | (++rnd_key & 0xfffu);
             const unsigned int slot = rnd_key & 1u;
             const int stride = G.seg_stride;
@@ -773,8 +770,6 @@ greedy_persist_kernel(const __grid_constant__ PersistArgs A, const PipeCfg cfg, 
             centre = static_cast<int>(alq_maxkey_row(kk));
         } else {
             if (prof) ss.prof[8] = gtime_ns();
-            if (dbg && t == dbg_step) dbg[0] = gtime_ns();
-            if (dbg && t == dbg_step + 9) { dbg[3] = gtime_ns(); unsigned int sm; asm volatile("mov.u32 %0, %%smid;" : "=r"(sm)); dbg[4] = sm; }
             // ================= certified fast path =================
             // np.random.choice picks the first k with cdf[k] > u, cdf = cumsum64(fl32(c / S)) / its last entry.  Every
             // fl32(c_i / S) is c_i / S (1 + e_i), |e_i| <= 2^-24 (or an absolute 2^-150 when it underflows), and S cancels
@@ -817,7 +812,6 @@ greedy_persist_kernel(const __grid_constant__ PersistArgs A, const PipeCfg cfg, 
                               [&](int i, unsigned long long w) { u32[i ^ 1] = static_cast<unsigned int>(w); });
                 }
                 cons_bar();
-                if (dbg && t == dbg_step) dbg[1] = gtime_ns();
                 int e_hit;
                 double e_base, q_tot;
                 if (ne <= 2048) {             // one warp, no block barriers
@@ -833,7 +827,6 @@ greedy_persist_kernel(const __grid_constant__ PersistArgs A, const PipeCfg cfg, 
                 }
                 const bool sane = q_tot > 0.0 && q_tot <= 1.0e300;
                 if (!sane || e_hit < 0 || !((e_base / q_tot) <= u - kMargin)) exact = true;     // same verdict in every CTA of every rank
-                if (dbg && t == dbg_step) dbg[2] = gtime_ns();
                 if (!exact) {
                     const unsigned int ptag = A.tag_base | (++rnd_pick & 0xffffffu);
                     const unsigned int pslot = rnd_pick & 1u;
@@ -857,7 +850,6 @@ greedy_persist_kernel(const __grid_constant__ PersistArgs A, const PipeCfg cfg, 
                             if (r_hit >= 0 && (r_base / q_tot) <= u - kMargin) word = static_cast<unsigned int>(seg.row_lo + r_hit);
                             if (ct < A.world) ll_store(A.peer[ct] + G.pickw + pslot * 8, ptag, word);
                         }
-                        if (dbg && t == dbg_step && ct == 0) dbg[6] = gtime_ns();
                     }
                     if (ct == 0) ss.centre = static_cast<int>(ll_wait(win + G.pickw + pslot * 8, ptag, A));
                     cons_bar();
@@ -873,7 +865,6 @@ greedy_persist_kernel(const __grid_constant__ PersistArgs A, const PipeCfg cfg, 
             }
         }
         if (grank == 0 && ct == 0) A.picks[G.pick_off + t] = centre;
-        if (dbg && t == dbg_step) dbg[7] = gtime_ns();
         if (prof) {
             const unsigned long long t_c = gtime_ns();
             if (t > 0) { ss.prof[0] += ss.prof[8] - ss.prof[6]; ss.prof[1] += t_c - ss.prof[8]; }
@@ -906,26 +897,6 @@ __global__ void persist_ready_kernel(PersistArgs A) {
     }
 }
 
-// ---- NumPy's pairwise-summation tree ---------------------------------------------------------------
-struct PairTree {
-    std::vector<int> leaf_off;                       // n_leaves + 1
-    struct Node { int height, l, r; };               // children: >= 0 leaf id, < 0 internal #(-v - 1)
-    std::vector<Node> internal;                      // creation (post-) order
-    std::pair<int, int> rec(int lo, int m) {         // -> (ref, height)
-        if (m <= 128) {
-            leaf_off.push_back(lo);
-            return {static_cast<int>(leaf_off.size()) - 1, 0};
-        }
-        int half = m / 2;
-        half -= half % 8;
-        const auto L = rec(lo, half);
-        const auto Rr = rec(lo + half, m - half);
-        const int h = std::max(L.second, Rr.second) + 1;
-        internal.push_back({h, L.first, Rr.first});
-        return {-static_cast<int>(internal.size()), h};
-    }
-};
-
 template <bool FACTORED, bool SAMPLE>
 cudaError_t launch_persist(int grid, size_t smem, cudaStream_t st, PersistArgs& A, PipeCfg& cfg, int& k_max, int& lc_max, int& ne_max, int& rm_max) {
     auto* fn = greedy_persist_kernel<FACTORED, SAMPLE>;
@@ -939,12 +910,10 @@ cudaError_t launch_persist(int grid, size_t smem, cudaStream_t st, PersistArgs& 
 
 extern "C" int64_t alq_pairwise_leaf_bounds(int64_t n, int32_t* out_host, int64_t cap) {
     if (n <= 0 || n >= (1LL << 31) || !out_host) return -1;
-    PairTree tb;
-    tb.rec(0, static_cast<int>(n));
-    const int64_t k = static_cast<int64_t>(tb.leaf_off.size());
+    const PairTree tb(static_cast<int>(n));
+    const int64_t k = tb.n_leaves();
     if (cap < k + 1) return -1;
-    for (int64_t i = 0; i < k; ++i) out_host[i] = tb.leaf_off[i];
-    out_host[k] = static_cast<int32_t>(n);
+    std::copy(tb.leaf_off.begin(), tb.leaf_off.end(), out_host);
     return k;
 }
 
@@ -1051,30 +1020,21 @@ int alq_greedy_persist(alq_ctx* ctx, const alq_greedy_desc* D, void* stream) {
         g.cfull_off = cfull_total;
         cfull_off[p] = cfull_total;
         cfull_total += (g.full_n + 3) & ~3;
-        PairTree tb;
-        tb.rec(0, g.full_n);
-        const int K = static_cast<int>(tb.leaf_off.size());
-        if (K > kMaxLeaves) return kPersistNotApplicable;
-        tb.leaf_off.push_back(g.full_n);
+        const PairTree tb(g.full_n);
+        const int K = tb.n_leaves();
+        if (K > kMaxLeaves || tb.n_levels() > 38) return kPersistNotApplicable;
         g.n_leaves = K;
         g.leaf_base = static_cast<int>(leaf_off_all.size());
         leaf_off_all.insert(leaf_off_all.end(), tb.leaf_off.begin(), tb.leaf_off.end());
         // internal nodes in level order; node id = K + position in that order
-        int hmax = 0;
-        for (auto& nd : tb.internal) hmax = std::max(hmax, nd.height);
-        if (hmax > 38) return kPersistNotApplicable;
-        std::vector<int> order, newid(tb.internal.size());
+        g.n_levels = tb.n_levels();
         g.level_base = static_cast<int>(level_off_all.size());
-        for (int h = 1; h <= hmax; ++h) {
-            level_off_all.push_back(static_cast<int>(order.size()));
-            for (size_t k = 0; k < tb.internal.size(); ++k)
-                if (tb.internal[k].height == h) { newid[k] = K + static_cast<int>(order.size()); order.push_back(static_cast<int>(k)); }
-        }
-        level_off_all.push_back(static_cast<int>(order.size()));
-        g.n_levels = hmax;
+        level_off_all.insert(level_off_all.end(), tb.level_off.begin(), tb.level_off.end());
+        std::vector<int> newid(tb.internal.size());
+        for (size_t j = 0; j < tb.order.size(); ++j) newid[tb.order[j]] = K + static_cast<int>(j);
         g.sched_base = static_cast<int>(sched_all.size());
         auto nid = [&](int v) { return v >= 0 ? v : newid[-v - 1]; };
-        for (int k : order)
+        for (int k : tb.order)
             sched_all.push_back(static_cast<unsigned int>(nid(tb.internal[k].l)) | (static_cast<unsigned int>(nid(tb.internal[k].r)) << 16));
         g.leaf_lo = 0;
         g.leaf_hi = K;
@@ -1155,7 +1115,7 @@ int alq_greedy_persist(alq_ctx* ctx, const alq_greedy_desc* D, void* stream) {
                                       leaf_off_all.size() * 4 + 4, level_off_all.size() * 4 + 4, sched_all.size() * 4 + 4,
                                       static_cast<size_t>(cfull_total) * 8 + 16, static_cast<size_t>(cfull_total) * 4 + 16,
                                       static_cast<size_t>(total_picks) * 8 + 8, segtab.size() * 4 + 4, ncta_tab.size() * 4 + 4,
-                                      static_cast<size_t>(P + 1) * 4, static_cast<size_t>(P) * 4, 64, 64 + 64 * static_cast<size_t>(grid), comm ? 0 : win_bytes});
+                                      static_cast<size_t>(P + 1) * 4, static_cast<size_t>(P) * 4, 64, 64, comm ? 0 : win_bytes});
     int rc = alq_scratch_reserve(ctx, need);
     if (rc) return rc;
     ScratchCursor cur(ctx->scratch);
@@ -1172,7 +1132,7 @@ int alq_greedy_persist(alq_ctx* ctx, const alq_greedy_desc* D, void* stream) {
     int* d_part_off = cur.take<int>(P + 1);
     int* d_cfull_off = cur.take<int>(P);
     int* d_status = cur.take<int>(1);
-    unsigned long long* d_prof = cur.take<unsigned long long>(8 + 8 * static_cast<size_t>(grid));
+    unsigned long long* d_prof = cur.take<unsigned long long>(8);
     char* d_win = comm ? Gc.window : cur.take<char>(win_bytes);
 
     ALQ_CUDA(ctx, cudaMemcpyAsync(d_segs, segs.data(), segs.size() * sizeof(BlockSeg), cudaMemcpyHostToDevice, st));
@@ -1180,7 +1140,7 @@ int alq_greedy_persist(alq_ctx* ctx, const alq_greedy_desc* D, void* stream) {
     ALQ_CUDA(ctx, cudaMemcpyAsync(d_segtab, segtab.data(), segtab.size() * 4, cudaMemcpyHostToDevice, st));
     ALQ_CUDA(ctx, cudaMemcpyAsync(d_ncta, ncta_tab.data(), ncta_tab.size() * 4, cudaMemcpyHostToDevice, st));
     ALQ_CUDA(ctx, cudaMemsetAsync(d_status, 0, sizeof(int), st));
-    ALQ_CUDA(ctx, cudaMemsetAsync(d_prof, 0, (8 + 8 * static_cast<size_t>(grid)) * sizeof(unsigned long long), st));
+    ALQ_CUDA(ctx, cudaMemsetAsync(d_prof, 0, 8 * sizeof(unsigned long long), st));
     // LL regions start without any valid tag (after the ready[] words; peers only write them after our ready flag)
     ALQ_CUDA(ctx, cudaMemsetAsync(d_win + up(8 * ALQ_MAX_WORLD), 0, win_bytes - up(8 * ALQ_MAX_WORLD), st));
     if (sample) {
@@ -1220,12 +1180,10 @@ int alq_greedy_persist(alq_ctx* ctx, const alq_greedy_desc* D, void* stream) {
     const int clock_khz = ctx->clock_khz;
     A.timeout_cycles = static_cast<long long>(ctx->spin_timeout_ms) * clock_khz;
     {   // L2 residency: keep `l2_resident_mb` of the rows this GPU streams in L2 across the steps (evict_last), split evenly over the CTAs
-        long long mb = ctx->l2_resident_mb;
-        if (const char* e = getenv("ALQ_L2_RESIDENT_MB")) mb = atoll(e);
+        const long long mb = ctx->l2_resident_mb;
         A.resident_rows = mb > 0 ? static_cast<int>(std::min<long long>((mb << 20) / static_cast<long long>(row_bytes) / std::max(grid, 1), 1 << 30)) : 0;
     }
     A.fast_path = ctx->d2_fast_path;
-    if (const char* e = getenv("ALQ_D2_FAST_PATH")) A.fast_path = atoi(e) != 0;
 
     if (comm) {
         persist_ready_kernel<<<1, 32, 0, st>>>(A);       // after the clears above, in stream order
@@ -1259,34 +1217,6 @@ int alq_greedy_persist(alq_ctx* ctx, const alq_greedy_desc* D, void* stream) {
         D->step_kernel_ms_host[5] = static_cast<float>(prof[4] * 1e-6 / steps);
         D->step_kernel_ms_host[6] = static_cast<float>(prof[5] * 1e-6);      // t = 0 selection, ms
         D->step_kernel_ms_host[7] = static_cast<float>(prof[6] * 1e-6);      // whole kernel, ms
-    }
-    if (D->step_kernel_ms_host && getenv("ALQ_PERSIST_DEBUG")) {      // per-CTA stamps of the middle step: where does the grid wait?
-        std::vector<unsigned long long> h(8 * static_cast<size_t>(grid));
-        cudaMemcpy(h.data(), d_prof + 8, h.size() * 8, cudaMemcpyDeviceToHost);
-        unsigned long long t0 = ~0ull;
-        for (int b = 0; b < grid; ++b) if (h[8 * b] && h[8 * b] < t0) t0 = h[8 * b];
-        static const char* names[8] = {"stream end", "values known", "S known", "mass stored", "masses polled", "leaf located", "search done (owner)", "pick known"};
-        for (int k = 0; k < 8; ++k) {
-            unsigned long long mn = ~0ull, mx = 0;
-            double mean = 0;
-            int cnt = 0;
-            for (int b = 0; b < grid; ++b) {
-                if (!h[8 * b + k]) continue;
-                const unsigned long long v = h[8 * b + k] - t0;
-                mn = std::min(mn, v); mx = std::max(mx, v); mean += v; ++cnt;
-            }
-            if (k == 3 || k == 4) continue;
-            if (cnt) fprintf(stderr, "[alq persist dbg] %-20s min %7.2f mean %7.2f max %7.2f us (%d CTAs) after the first CTA's stream end\n", names[k], mn * 1e-3, mean / cnt * 1e-3, mx * 1e-3, cnt);
-        }
-    }
-    if (D->step_kernel_ms_host && getenv("ALQ_PERSIST_DEBUG") && atoi(getenv("ALQ_PERSIST_DEBUG")) >= 2) {
-        std::vector<unsigned long long> h(8 * static_cast<size_t>(grid));
-        cudaMemcpy(h.data(), d_prof + 8, h.size() * 8, cudaMemcpyDeviceToHost);
-        unsigned long long a0 = ~0ull, b0 = ~0ull;
-        for (int b = 0; b < grid; ++b) { if (h[8 * b]) a0 = std::min(a0, h[8 * b]); if (h[8 * b + 3]) b0 = std::min(b0, h[8 * b + 3]); }
-        fprintf(stderr, "[alq persist skew] cta smid lateness_us(step A) lateness_us(step A+9)\n");
-        for (int b = 0; b < grid; ++b)
-            fprintf(stderr, "[alq persist skew] %d %llu %.2f %.2f\n", b, h[8 * b + 4], (h[8 * b] - a0) * 1e-3, (h[8 * b + 3] - b0) * 1e-3);
     }
     if (status == ALQ_ERR_STATE) ALQ_FAIL(ctx, status, "alq_greedy_select: timed out waiting for a peer GPU (or a CTA of this grid)");
     if (status != 0) ALQ_FAIL(ctx, status, "alq_greedy_select: non-finite or empty probability mass during D^2 sampling");

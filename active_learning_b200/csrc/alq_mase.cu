@@ -458,7 +458,7 @@ extern "C" int alq_mase_margins(alq_ctx* ctx, const float* logits, int64_t n, in
     const int grid = rows_grid(ctx, n, kMaseThreads / 32);
     const bool vec = (c % 4 == 0) && (ld % 4 == 0) && (ldg % 4 == 0) && aligned16(logits) && aligned16(ginv) &&
                      (!radius || ((ldr % 4 == 0) && ldr == c && aligned16(radius))) && c <= 1024;
-    if (vec && ld == c && (radius ? ldr == c : gmin != nullptr) && n >= 4096 && ctx->greedy_variant != 1) {
+    if (vec && ld == c && (radius ? ldr == c : gmin != nullptr) && n >= 4096) {
         // bulk-copy pipelined kernel (the K1 / K2 pipeline with the K6 row code)
         const MaseArgs margs{ginv, ldg, gmin, pred, radius, ldr};
         cudaError_t e = cudaSuccess;

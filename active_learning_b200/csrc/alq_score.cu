@@ -1332,7 +1332,7 @@ extern "C" int alq_score_softmax(alq_ctx* ctx, const float* logits, int64_t n, i
     const bool vec = (c % 4 == 0) && (ld % 4 == 0) && aligned16(logits) && c <= 2048;
     RowPipeCfg cfg{};
     size_t smem = 0;
-    if (vec && ld == c && n >= 4096 && ctx->greedy_variant != 1 && plan_row_pipe(ctx, c, cfg, smem)) {
+    if (vec && ld == c && n >= 4096 && plan_row_pipe(ctx, c, cfg, smem)) {
         cudaError_t e;
         if (mode == ALQ_MODE_MARGIN) e = launch_rows_pipe_nv<ALQ_MODE_MARGIN>(ctx, st, cfg, smem, logits, n, c, scores, 1, 0, n, nullptr, 0);
         else if (mode == ALQ_MODE_LEAST_CONFIDENCE) e = launch_rows_pipe_nv<ALQ_MODE_LEAST_CONFIDENCE>(ctx, st, cfg, smem, logits, n, c, scores, 1, 0, n, nullptr, 0);
@@ -1390,7 +1390,7 @@ static int uncertainty_tail_impl(alq_ctx* ctx, const float* logits, int64_t n, i
     size_t smem = 0;
     const bool vec = (c % 4 == 0) && (ld == c) && aligned16(logits) && c <= 2048;
     // every rank must take the same path: the decision only uses what all ranks know (c, b, the smallest and largest shard)
-    bool fused = vec && rows_min >= 4096 && rows_max < (1LL << 31) && ctx->select_impl != 1 && ctx->greedy_variant != 1 &&
+    bool fused = vec && rows_min >= 4096 && rows_max < (1LL << 31) && ctx->select_impl != 1 &&
                  rows_max * 5 <= static_cast<int64_t>(ctx->sm_count) * kListCap * 4 &&     // the per-CTA lists absorb any imbalance
                  plan_row_pipe(ctx, c, cfg, smem, reserve);
     if (fused && sharded) {
@@ -1547,7 +1547,7 @@ extern "C" int alq_badge_factors(alq_ctx* ctx, const float* logits, int64_t n, i
                      aligned16(a) && c <= 2048;
     RowPipeCfg cfg{};
     size_t smem = 0;
-    if (vec && ld == c && n >= 4096 && ctx->greedy_variant != 1 && plan_row_pipe(ctx, c, cfg, smem)) {
+    if (vec && ld == c && n >= 4096 && plan_row_pipe(ctx, c, cfg, smem)) {
         cudaError_t e = launch_rows_pipe_nv<3>(ctx, st, cfg, smem, logits, n, c, a_norm2, batch_size, row0, n_total, a, lda);
         ctx->launches++;
         if (e != cudaSuccess) ALQ_FAIL(ctx, ALQ_ERR_CUDA, "rows_pipe_kernel launch failed: %s", cudaGetErrorString(e));

@@ -90,7 +90,7 @@ class Engine:
         return self
 
     def set_option(self, key: str, value: int):
-        """'k3_impl': 0 auto / 1 fp32 SIMT / 2 wgmma 3xTF32;  'greedy_variant': 0 auto / 1 direct / 2 pipeline / 3 persistent;  'spin_timeout_ms'; 'l2_resident_mb'; 'd2_fast_path'; 'tail_buckets';
+        """'k3_impl': 0 auto / 1 fp32 SIMT / 2 wgmma 3xTF32;  'greedy_variant' (selection loop only): 0 auto / 1 direct / 2 pipeline / 3 persistent;  'spin_timeout_ms'; 'l2_resident_mb'; 'd2_fast_path'; 'tail_buckets';
         'select_impl': 0 auto / 1 multi-kernel / 2 cluster;  'base_impl': 0 auto / 1 sequential / 2 parallel lists."""
         self._check(self.lib.alq_set_option(self._h, key.encode(), int(value)), "alq_set_option")
 

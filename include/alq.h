@@ -46,7 +46,8 @@ void alq_destroy(alq_ctx* ctx);
 const char* alq_last_error(const alq_ctx* ctx);
 /* Implementation knobs (defaults pick the fastest valid kernel):
  *   "k3_impl"        0 auto | 1 exact-fp32 SIMT contraction | 2 wgmma 3xTF32 contraction
- *   "greedy_variant" 0 auto | 1 direct-load step kernel     | 2 bulk-copy (TMA) pipeline | 3 persistent cooperative loop
+ *   "greedy_variant" selection loop (K4/K5) only: 0 auto | 1 direct-load step kernel | 2 bulk-copy (TMA) pipeline |
+ *                    3 persistent cooperative loop
  *   "l2_resident_mb" persistent selection loop: MB of the rows a GPU streams that are fetched L2::evict_last (the head of every
  *                    CTA's segment) so that they stay in the 50 MB L2 across the B steps; the rest is fetched evict_first.
  *                    Default 24; 0 turns the hints off

@@ -190,23 +190,24 @@ def test_topb_pack_merge_equals_global_select(eng):
 
 @pytest.mark.parametrize("n,c", [(5003, 1000), (4097, 2048), (9000, 64), (70001, 4), (6000, 1024)])
 def test_pipelined_rows_kernels_equal_direct_kernels(eng, n, c):
-    """K1/K2 TMA bulk-copy pipeline (n >= 4096, contiguous rows) vs the direct-load kernels: same row
-    code, so scores and BADGE factors must be bit-identical; and both match the oracle."""
+    """K1/K2 TMA bulk-copy pipeline (n >= 4096, contiguous rows) vs the direct-load kernels, which take rows with a
+    leading dimension ld != c: the same logits once contiguous and once in an [n, c + 4] buffer (NaN padding) sliced to
+    c columns.  Same row code, so scores and BADGE factors must be bit-identical; and both match the oracle."""
     torch.manual_seed(n + c)
     logits = torch.randn(n, c) * 3
-    dev = logits.cuda()
-    try:
-        res = {}
-        for variant in (1, 0):
-            eng.set_option("greedy_variant", variant)
-            res[variant] = [eng.score_softmax(dev, m).cpu() for m in (0, 1, 2)] + \
-                [t.cpu() for t in eng.badge_factors(dev, 128)]
-    finally:
-        eng.set_option("greedy_variant", 0)
-    for a, b in zip(res[1], res[0]):
+    dense = logits.cuda()
+    padded = torch.full((n, c + 4), float("nan"), device="cuda")
+    padded[:, :c] = dense
+    strided = padded[:, :c]
+    assert strided.stride(0) == c + 4
+    res = {}
+    for name, dev in (("direct", strided), ("pipelined", dense)):
+        res[name] = [eng.score_softmax(dev, m).cpu() for m in (0, 1, 2)] + \
+            [t.cpu() for t in eng.badge_factors(dev, 128)]
+    for a, b in zip(res["direct"], res["pipelined"]):
         assert torch.equal(a, b)
-    assert torch.allclose(res[0][0], O.softmax_scores(logits, O.MODE_MARGIN), rtol=0, atol=TOL_PROB)
-    assert torch.allclose(res[0][3][:, :c], O.badge_factors(logits, 128), rtol=0, atol=1e-7)
+    assert torch.allclose(res["pipelined"][0], O.softmax_scores(logits, O.MODE_MARGIN), rtol=0, atol=TOL_PROB)
+    assert torch.allclose(res["pipelined"][3][:, :c], O.badge_factors(logits, 128), rtol=0, atol=1e-7)
 
 
 @pytest.mark.parametrize("n,c,b", [(80000, 1000, 10000), (80000, 1000, 1), (5000, 40, 5000), (4100, 12, 77), (30011, 1000, 3000), (200000, 8, 16000)])
