@@ -9,8 +9,6 @@
 // [N, C] input K1 reads.  NaN (c == p, duplicated class rows: 0/0, x/0 * 0) becomes +inf like :77.
 // base_sampler.py:22-38 then selects class by class; alq_base_select runs that loop on the stream with K1b.
 #include <limits.h>
-#include <stdio.h>
-#include <stdlib.h>
 
 #include <algorithm>
 
@@ -544,7 +542,7 @@ extern "C" int alq_base_select(alq_ctx* ctx, const float* min_margin, const floa
         base_candidates_kernel<<<(c + kBaseGroup - 1) / kBaseGroup, kBaseThreads, cand_smem, st>>>(
             min_margin, radius, ldr, pred, static_cast<int>(n), c, budget, cand, fail);
         ALQ_LAUNCH_CHECK(ctx);
-        int cls = 0, ordinary_steps = 0;
+        int cls = 0;
         while (cls < c) {
             base_resolve_kernel<<<1, kBaseThreads, resolve_smem, st>>>(cand, fail, taken, static_cast<int>(n), c, budget, cls, chunk, out_pos, status);
             ALQ_LAUNCH_CHECK(ctx);
@@ -554,10 +552,8 @@ extern "C" int alq_base_select(alq_ctx* ctx, const float* min_margin, const floa
             if (stopped >= c) break;
             rc = class_step(stopped);          // a list that was too short (or not provably complete): the ordinary step
             if (rc) return rc;
-            ++ordinary_steps;
             cls = stopped + 1;
         }
-        if (getenv("ALQ_BASE_DEBUG")) fprintf(stderr, "alq_base_select: %d of %d classes took the ordinary step\n", ordinary_steps, c);
     } else {
         for (int cls = 0; cls < c; ++cls) {
             rc = class_step(cls);

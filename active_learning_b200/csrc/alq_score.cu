@@ -167,9 +167,8 @@ struct SelArgs {
     unsigned int* g_ctr;            // [4] zeroed: [0] grid-barrier arrivals, [1] candidates appended
     unsigned long long* g_cand;     // [n]
     int32_t* out_pos;               // [b]
-    long long* dbg;                 // optional phase stamps of CTA 0 (ALQ_SELECT_DEBUG)
-    // rows sharded over `world` GPUs (0 / 1: single GPU): the histograms are summed and the candidates gathered through
-    // the peer-memory windows from inside this kernel, every rank ends with the same global list
+    // the sharded call (`world` >= 1 ranks; 0, as zero-initialised, for the one-GPU call): the histograms are summed and
+    // the candidates gathered through the peer-memory windows from inside this kernel, every rank ends with the same list
     int world, rank;
     unsigned int row_base;          // global position of this rank's row 0
     char* peer[ALQ_MAX_WORLD];
@@ -186,8 +185,7 @@ struct SelArgs {
     unsigned long long* g_bucket;   // [grid][kBucketLanes][bucket_cap]
     unsigned int* g_bcnt;           // [grid][kBucketLanes] zeroed
     int bucket_cap;                 // words per sub-list
-    int use_tree;                   // experiment (ALQ_TAIL_TREE=1): the general route searches a breadth-first tree copy of the
-                                    // CTA's candidates instead of the sorted array; off by default, see select_epilogue
+    int ring_off, ring_bars;        // byte offset and count of the tile ring's full[] / empty[] mbarriers
 };
 constexpr int kBucketLanes = 16;
 
@@ -248,53 +246,138 @@ __device__ __forceinline__ void sel_find_bin(const uint32_t* hist, uint32_t k, u
     __syncthreads();
 }
 
-// Ranking stage of the general route.  The CTA's own (ascending) candidates are searched once per word of the global
-// list -- about b searches per CTA.  A plain binary search over a sorted array in shared memory pays bank conflicts: the
-// probes of step k sit a power-of-two stride apart and fall into one or two banks.  EXPERIMENT (ALQ_TAIL_TREE=1, off by
-// default): the candidates are also kept as an implicit perfect search tree in breadth-first order (1-based: children
-// of node k are 2k and 2k + 1; missing nodes hold ~0, which no list word reaches), so the probes of one step are
-// contiguous words.  Height h = smallest with 2^h - 1 >= nc; the sorted index r sits at node
-//     k(r) = 2^(h-1-z) + ((r + 1) >> (z + 1)),  z = trailing zeros of r + 1,
-// and after h steps of  k = 2k + (tree[k] <= x)  the count of candidates <= x is k - 2^h.  Without the conflicts the
-// ~b shared-memory atomics on the difference array dominate the stage (the reason for the bucket route).  It is exact in every one-GPU test, but the same helper produced wrong ranks inside the sharded
-// epilogue on 2 GPUs for c = 64 (tools/mgpu_tail_dbg.py; a host emulation of the arithmetic agrees with the sorted
-// search, so the cause is on the device side) -- hence not the default anywhere.  What is known: the wrong positions were
-// exactly the slices of ~12 CTAs per rank (presumably the ones that had streamed rows: 36 claims of 8 tiles, three per
-// producer); for c = 64 the tree sits at byte 131 056 of the CTA's shared memory and its nodes 2..33 are the words of the
-// tile ring's full[] / empty[] mbarriers (ring = 16 x 8 KB), which the epilogue reuses as plain memory WITHOUT
-// mbarrier.inval -- PTX calls that undefined.  For c = 1000 those words are nodes 2002..2025 (never used), for c = 8
-// they lie inside the list buffer.  Hypothesis, not verified (no GPU time left in round 2): invalidate the 2 x stages
-// ring barriers at the top of the epilogue.  The shipped routes touch those words only transiently (staging copy of the
-// own candidates, written and read back between two barriers), and every parity test passes.
-__device__ __forceinline__ int sel_tree_height(int nc) { return nc > 0 ? 32 - __clz(nc) : 0; }
-__device__ __forceinline__ int sel_tree_node(int r, int h) {
-    const int t = r + 1, z = __ffs(t) - 1;
-    return (1 << (h - 1 - z)) + (t >> (z + 1));
-}
-// s_diff[number of own candidates <= x] += 1 for every word x of buf[0, m)
-__device__ __forceinline__ void sel_count_into_diff(const unsigned long long* buf, int m, const unsigned long long* tree, int h,
-                                                    uint32_t* s_diff) {
-    constexpr int U = 4;                                    // independent searches in flight per thread: each is a chain
-    const int tid = threadIdx.x, nthr = blockDim.x;         // of h dependent shared-memory loads
-    for (int j0 = tid; j0 < m; j0 += U * nthr) {
-        unsigned long long x[U];
-        int k[U];
-#pragma unroll
-        for (int u = 0; u < U; ++u) {
-            const int j = j0 + u * nthr;
-            x[u] = buf[j < m ? j : j0];
-            k[u] = 1;
-        }
-        for (int s = 0; s < h; ++s) {
-#pragma unroll
-            for (int u = 0; u < U; ++u) k[u] = 2 * k[u] + (tree[k[u]] <= x[u] ? 1 : 0);
-        }
-#pragma unroll
-        for (int u = 0; u < U; ++u)
-            if (j0 + u * nthr < m) atomicAdd(&s_diff[k[u] - (1 << h)], 1u);
+// Stages shared by both epilogues.  s_misc: [0] words in s_list, [1] level-0 bin, [2] rank still wanted inside it,
+// [3] offset in the candidate list, [4] own candidates, [5] level-1 bin, [6] 2047 - first populated level-0 bin,
+// [8..9] the list-streaming mbarrier, [16..47] sel_find_bin's scratch, [48..] the bucket route's counters.
+
+// %globaltimer stamp i of CTA 0, read back by alq_uncertainty_tail_timing: [0] kernel start, [1] every CTA of this GPU
+// has streamed its rows, [2] kernel end
+__device__ __forceinline__ void sel_stamp(unsigned int* g_ctr, int i) {
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        unsigned long long t;
+        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+        reinterpret_cast<unsigned long long*>(g_ctr + 4)[i] = t;
     }
 }
-// the same over the sorted array itself (only when the tree does not fit: nc == list_cap)
+
+// this CTA's 2048-bin histogram added into a global one
+__device__ __forceinline__ void sel_push_hist(const uint32_t* s_hist, unsigned int* g) {
+    for (int i = threadIdx.x; i < 2048; i += blockDim.x) {
+        const uint32_t h = s_hist[i];
+        if (h) atomicAdd(g + i, h);
+    }
+}
+
+// a global 2048-bin histogram -> shared memory; with `first` (zero on entry) also the first populated bin, as
+// 2047 - bin in *first
+__device__ __forceinline__ void sel_load_hist(const unsigned int* g, uint32_t* s_hist, int* first) {
+    const int tid = threadIdx.x, nthr = blockDim.x;
+    uint32_t hv[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) hv[k] = (tid + k * nthr) < 2048 ? __ldcg(g + tid + k * nthr) : 0u;
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+        if ((tid + k * nthr) < 2048) {
+            s_hist[tid + k * nthr] = hv[k];
+            if (first && hv[k]) atomicMax(first, 2047 - (tid + k * nthr));
+        }
+}
+
+// Level 1: the next 11 bits of this CTA's keys inside level-0 bin T0 -> s_hist (a float score has few distinct
+// exponents, so one level alone can leave most of the pool in the boundary bin)
+__device__ __forceinline__ void sel_level1_hist(const unsigned long long* s_list, int cnt, uint32_t T0, uint32_t* s_hist) {
+    const int tid = threadIdx.x, nthr = blockDim.x;
+    for (int i = tid; i < 2048; i += nthr) s_hist[i] = 0;
+    __syncthreads();
+    for (int i = tid; i < cnt; i += nthr) {
+        const uint32_t key = static_cast<uint32_t>(s_list[i] >> 32);
+        if ((key >> 21) == T0) atomicAdd(&s_hist[(key >> 10) & 0x7ffu], 1u);
+    }
+    __syncthreads();
+}
+
+// This CTA's candidates -- every word whose 22-bit key prefix is <= T: the winners plus the few other keys sharing the
+// prefix T -- into buf[0, nc), counted in s_misc[4] (zero on entry); nc slots of the candidate count g_ctr[1] are
+// reserved, starting at `off`.  Returns nc.
+__device__ __forceinline__ int sel_gather_candidates(const SelArgs& S, const unsigned long long* s_list, int cnt, uint32_t T,
+                                                     unsigned long long* buf, int* s_misc, int& off) {
+    const int tid = threadIdx.x, nthr = blockDim.x;
+    for (int i = tid; i < cnt; i += nthr) {
+        const unsigned long long w = s_list[i];
+        if (static_cast<uint32_t>(w >> 42) <= T) buf[atomicAdd(&s_misc[4], 1)] = w;
+    }
+    __syncthreads();
+    const int nc = s_misc[4];
+    if (tid == 0) s_misc[3] = static_cast<int>(atomicAdd(S.g_ctr + 1, static_cast<unsigned int>(nc)));
+    __syncthreads();
+    off = s_misc[3];
+    return nc;
+}
+
+// Score buckets of the bucket route.  Every candidate score lies in [lo, hi] = [lower edge of the first populated
+// level-0 bin, upper edge of prefix T]; bucket(score) = floor((score - lo) * nb / (hi - lo)), clamped, is monotone in the
+// key, so bucket q holds exactly the ranks [words in the buckets below q, ...).  Scores that do not spread and non-finite
+// edges leave `spread` false; every thread of every CTA computes the same value from the same histogram.
+struct SelBuckets {
+    float lo, scale;
+    int nb;
+    bool spread;
+    __device__ __forceinline__ SelBuckets(int first_bin, uint32_t T, int nbuckets) : nb(nbuckets) {
+        lo = sel_key_to_float(static_cast<uint32_t>(first_bin) << 21);
+        const float hi = sel_key_to_float((T << 10) | 0x3ffu);
+        scale = static_cast<float>(nb) / (hi - lo);
+        spread = isfinite(lo) && isfinite(hi) && hi > lo && isfinite(scale);
+    }
+    __device__ __forceinline__ int of(unsigned long long w) const {
+        const float sc = sel_key_to_float(static_cast<uint32_t>(w >> 32));
+        return min(nb - 1, max(0, __float2int_rd((sc - lo) * scale)));
+    }
+};
+
+// One bucket w[0, mine) ordered by counting (the words are distinct: the row is part of them); `base` words lie in the
+// buckets below.  Rank < b -> out_pos[rank] = row.
+__device__ __forceinline__ void sel_rank_bucket(const unsigned long long* w, int mine, int base, int b, int32_t* out_pos) {
+    for (int i = threadIdx.x; i < mine; i += blockDim.x) {
+        const unsigned long long x = w[i];
+        int r = base;
+        for (int q = 0; q < mine; ++q) r += w[q] < x;
+        if (r < b) out_pos[r] = static_cast<int32_t>(x & 0xffffffffu);
+    }
+}
+
+// Streams src[0, total) through buf[0, buf_cap) with the whole CTA: one TMA bulk copy per chunk, completing on `bar`,
+// then body(words in the chunk).  overlap() runs while the first chunk is in flight.  `bar` is initialised here and
+// invalidated before the return; buf must be free on entry.
+template <class Overlap, class Body>
+__device__ __forceinline__ void sel_stream_list(const unsigned long long* src, int total, unsigned long long* buf, int buf_cap,
+                                                uint64_t* bar, Overlap&& overlap, Body&& body) {
+    const int tid = threadIdx.x;
+    auto copy = [&](int base, int m) {
+        const uint32_t bytes = static_cast<uint32_t>((m + 1) & ~1) * 8u;
+        mbar_expect_tx(bar, bytes);
+        bulk_g2s(buf, src + base, bytes, bar);
+    };
+    if (tid == 0) {
+        mbar_init(bar, 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    if (tid == 0 && total > 0) copy(0, min(buf_cap, total));
+    overlap();
+    uint32_t phase = 0;
+    for (int base = 0; base < total; base += buf_cap) {
+        const int m = min(buf_cap, total - base);
+        __syncthreads();                                    // the previous chunk is consumed
+        if (base > 0 && tid == 0) copy(base, m);
+        mbar_wait(bar, phase);
+        phase ^= 1u;
+        body(m);
+    }
+    __syncthreads();
+    if (tid == 0) mbar_inval(bar);
+}
+
+// s_diff[number of own candidates <= x] += 1 for every word x of buf[0, m): a binary search in the sorted own[0, nc)
 __device__ __forceinline__ void sel_count_into_diff_sorted(const unsigned long long* buf, int m, const unsigned long long* own,
                                                            int nc, uint32_t* s_diff) {
     const int tid = threadIdx.x, nthr = blockDim.x;
@@ -309,63 +392,50 @@ __device__ __forceinline__ void sel_count_into_diff_sorted(const unsigned long l
     }
 }
 
-// s_misc: [0] words in s_list, [1] level-0 bin, [2] rank still wanted inside it, [3] offset in g_cand, [4] own
-// candidates, [5] level-1 bin
+// The prefix sum of the difference array is the rank of each sorted own word own[0, nc): rank < b -> out_pos[rank] = row
+// (~0 words pad the sharded list and are never written)
+__device__ __forceinline__ void sel_write_ranks(uint32_t* s_diff, const unsigned long long* own, int nc, int b, int32_t* out_pos) {
+    const int tid = threadIdx.x, nthr = blockDim.x, lane = tid & 31;
+    if (tid < 32) {
+        uint32_t carry = 0;
+        for (int base = 0; base < nc; base += 32) {
+            const int i = base + lane;
+            uint32_t v = i < nc ? s_diff[i] : 0u;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const uint32_t t = __shfl_up_sync(0xffffffffu, v, o);
+                if (lane >= o) v += t;
+            }
+            if (i < nc) s_diff[i] = carry + v;
+            carry += __shfl_sync(0xffffffffu, v, 31);
+        }
+    }
+    __syncthreads();
+    for (int i = tid; i < nc; i += nthr) {
+        const uint32_t r = s_diff[i];
+        const unsigned long long w = own[i];
+        if (r < static_cast<uint32_t>(b) && w != ~0ull) out_pos[r] = static_cast<int32_t>(w & 0xffffffffu);
+    }
+}
+
 __device__ __noinline__ void select_epilogue(const SelArgs& S, uint32_t* s_hist, unsigned long long* s_list, int* s_misc,
                                              unsigned long long* buf, int buf_cap) {
-    const int tid = threadIdx.x, nthr = blockDim.x, lane = tid & 31, warp = tid >> 5;
-    long long* dbg = (S.dbg && blockIdx.x == 0 && tid == 0) ? S.dbg : nullptr;
+    const int tid = threadIdx.x, nthr = blockDim.x, lane = tid & 31;
     __syncthreads();                                        // every consumer warp has appended its rows
-    if (dbg) dbg[0] = clock64();
     const int cnt = s_misc[0];
     // ---- level 0: the 11 top key bits were counted while the rows streamed ----
-    for (int i = tid; i < 2048; i += nthr) {
-        const uint32_t h = s_hist[i];
-        if (h) atomicAdd(S.g_hist + i, h);
-    }
+    sel_push_hist(s_hist, S.g_hist);
     sel_grid_barrier(S.g_ctr, gridDim.x);
-    if (blockIdx.x == 0 && tid == 0) {        // every CTA has finished its rows: the stream ends here
-        unsigned long long t;
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-        reinterpret_cast<unsigned long long*>(S.g_ctr + 4)[1] = t;
-    }
-    {
-        uint32_t hv[4];
-#pragma unroll
-        for (int k = 0; k < 4; ++k) hv[k] = (tid + k * nthr) < 2048 ? __ldcg(S.g_hist + tid + k * nthr) : 0u;
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-            if ((tid + k * nthr) < 2048) {
-                s_hist[tid + k * nthr] = hv[k];
-                if (hv[k]) atomicMax(&s_misc[6], 2047 - (tid + k * nthr));      // first populated bin (s_misc[6] starts at 0)
-            }
-    }
+    sel_stamp(S.g_ctr, 1);                                  // every CTA has finished its rows: the stream ends here
+    sel_load_hist(S.g_hist, s_hist, &s_misc[6]);
     __syncthreads();
     sel_find_bin(s_hist, static_cast<uint32_t>(S.b), reinterpret_cast<uint32_t*>(s_misc + 16), &s_misc[1], &s_misc[2]);
     const uint32_t T0 = static_cast<uint32_t>(s_misc[1]);
-    if (dbg) dbg[1] = clock64();
-    // ---- level 1: the next 11 bits of the keys inside bin T0 (a float score has few distinct exponents, so one level
-    //      alone can leave most of the pool in the boundary bin) ----
-    for (int i = tid; i < 2048; i += nthr) s_hist[i] = 0;
-    __syncthreads();
-    for (int i = tid; i < cnt; i += nthr) {
-        const uint32_t key = static_cast<uint32_t>(s_list[i] >> 32);
-        if ((key >> 21) == T0) atomicAdd(&s_hist[(key >> 10) & 0x7ffu], 1u);
-    }
-    __syncthreads();
-    for (int i = tid; i < 2048; i += nthr) {
-        const uint32_t h = s_hist[i];
-        if (h) atomicAdd(S.g_hist + 2048 + i, h);
-    }
+    // ---- level 1 ----
+    sel_level1_hist(s_list, cnt, T0, s_hist);
+    sel_push_hist(s_hist, S.g_hist + 2048);
     sel_grid_barrier(S.g_ctr, 2u * gridDim.x);
-    {
-        uint32_t hv[4];
-#pragma unroll
-        for (int k = 0; k < 4; ++k) hv[k] = (tid + k * nthr) < 2048 ? __ldcg(S.g_hist + 2048 + tid + k * nthr) : 0u;
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-            if ((tid + k * nthr) < 2048) s_hist[tid + k * nthr] = hv[k];
-    }
+    sel_load_hist(S.g_hist + 2048, s_hist, nullptr);
     __syncthreads();
     {
         const uint32_t want = static_cast<uint32_t>(s_misc[2]);
@@ -375,22 +445,15 @@ __device__ __noinline__ void select_epilogue(const SelArgs& S, uint32_t* s_hist,
     if (tid == 0) s_misc[4] = 0;
     __syncthreads();
     const uint32_t T = (T0 << 11) | static_cast<uint32_t>(s_misc[5]);        // 22-bit prefix of the b-th smallest key
-    if (dbg) dbg[2] = clock64();
     unsigned int barriers = 2;
-    // ---- bucket route.  Every candidate score lies in [lo, hi] = [lower edge of the first populated level-0 bin,
-    //      upper edge of prefix T]; bucket(score) = floor((score - lo) * grid / (hi - lo)), clamped, is monotone in the
-    //      key, so bucket q holds exactly the ranks [sum of the counts of buckets < q, ...): each candidate goes to the
-    //      CTA of its bucket, a CTA sorts ITS bucket (about b / grid words) and nobody ranks against the whole list
-    //      (that stage was bound by ~1 shared-memory atomic per list word per CTA: 5.5 us).  Scores that do not spread
-    //      (tie groups, one bucket beyond bucket_cap) or non-finite edges fall through to the general route below;
-    //      every CTA takes the same decision from the same counts. ----
+    // ---- bucket route: each candidate goes to the CTA of its score bucket, a CTA sorts ITS bucket (about b / grid
+    //      words) and nobody ranks against the whole list (that stage was bound by ~1 shared-memory atomic per list word
+    //      per CTA: 5.5 us).  Scores that do not spread and tie groups (one bucket beyond bucket_cap) fall through to the
+    //      general route below; every CTA takes the same decision from the same counts. ----
     if (S.g_bucket) {
         const int G = static_cast<int>(gridDim.x);
-        const float lo = sel_key_to_float(static_cast<uint32_t>(2047 - s_misc[6]) << 21);
-        const float hi = sel_key_to_float((T << 10) | 0x3ffu);
-        const float scale = static_cast<float>(G) / (hi - lo);
-        const bool spread = isfinite(lo) && isfinite(hi) && hi > lo && isfinite(scale);      // same value in every thread of every CTA
-        if (spread) {
+        const SelBuckets bk(2047 - s_misc[6], T, G);
+        if (bk.spread) {
             // kBucketLanes counters (and sub-lists) per bucket, CTA c appends to lane c % kBucketLanes: ~b appends onto `grid`
             // addresses is a chain of ~b / grid same-address atomics deep (measured 4 us); sixteen lanes cut it to a few
             constexpr int R = kBucketLanes;
@@ -399,15 +462,13 @@ __device__ __noinline__ void select_epilogue(const SelArgs& S, uint32_t* s_hist,
             for (int i = tid; i < cnt; i += nthr) {
                 const unsigned long long w = s_list[i];
                 if (static_cast<uint32_t>(w >> 42) <= T) {
-                    const float sc = sel_key_to_float(static_cast<uint32_t>(w >> 32));
-                    const int q = min(G - 1, max(0, __float2int_rd((sc - lo) * scale)));
+                    const int q = bk.of(w);
                     const unsigned int slot = atomicAdd(S.g_bcnt + q * R + lane_id, 1u);
                     if (slot < static_cast<unsigned int>(sub_cap))
                         S.g_bucket[(static_cast<size_t>(q) * R + lane_id) * sub_cap + slot] = w;
                 }
             }
             sel_grid_barrier(S.g_ctr, ++barriers * gridDim.x);
-            if (dbg) dbg[3] = clock64();
             // my bucket's sub-lists are fetched together with the counters (one L2 round trip); what lies beyond a
             // sub-list's count is dropped once the counts are known
             const unsigned long long* src = S.g_bucket + static_cast<size_t>(blockIdx.x) * R * sub_cap;
@@ -431,7 +492,6 @@ __device__ __noinline__ void select_epilogue(const SelArgs& S, uint32_t* s_hist,
             }
             __syncthreads();
             if (s_misc[48] <= sub_cap && R * sub_cap <= 2 * nthr) {
-                const int base = s_misc[49];
                 int mine = 0;
                 for (int l = 0; l < R; ++l) mine += s_misc[51 + l];
 #pragma unroll
@@ -447,114 +507,45 @@ __device__ __noinline__ void select_epilogue(const SelArgs& S, uint32_t* s_hist,
                     }
                 }
                 __syncthreads();
-                if (dbg) dbg[4] = clock64();
-                for (int i = tid; i < mine; i += nthr) {
-                    const unsigned long long w = buf[i];
-                    int r = base;
-                    for (int q = 0; q < mine; ++q) r += buf[q] < w;
-                    if (r < S.b) S.out_pos[r] = static_cast<int32_t>(w & 0xffffffffu);
-                }
-                if (dbg) { dbg[5] = clock64(); dbg[6] = -1; dbg[7] = mine; }
-                if (blockIdx.x == 0 && tid == 0) {
-                    unsigned long long t;
-                    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-                    reinterpret_cast<unsigned long long*>(S.g_ctr + 4)[2] = t;
-                }
+                sel_rank_bucket(buf, mine, s_misc[49], S.b, S.out_pos);
+                sel_stamp(S.g_ctr, 2);
                 return;
             }
             __syncthreads();
         }
     }
-    // ---- candidates: every key whose prefix is <= T (the winners plus the few other keys sharing the prefix T) ----
-    for (int i = tid; i < cnt; i += nthr) {
-        const unsigned long long w = s_list[i];
-        if (static_cast<uint32_t>(w >> 42) <= T) buf[atomicAdd(&s_misc[4], 1)] = w;
-    }
-    __syncthreads();
-    const int nc = s_misc[4];
-    if (tid == 0) s_misc[3] = static_cast<int>(atomicAdd(S.g_ctr + 1, static_cast<unsigned int>(nc)));
-    __syncthreads();
-    const int off = s_misc[3];
+    // ---- general route: the candidates of every CTA are appended to g_cand ----
+    int off;
+    const int nc = sel_gather_candidates(S, s_list, cnt, T, buf, s_misc, off);
     for (int i = tid; i < nc; i += nthr) {
         const unsigned long long w = buf[i];
         s_list[i] = w;
         S.g_cand[off + i] = w;
     }
     sel_grid_barrier(S.g_ctr, ++barriers * gridDim.x);
-    if (dbg) dbg[3] = clock64();
     const int total = static_cast<int>(__ldcg(S.g_ctr + 1));
     // ---- rank this CTA's candidates among all of them.  Own candidates are sorted first (a few dozen words: counting);
     //      then every word of the global list is located in that sorted list by a binary search and bumps ONE entry of a
     //      difference array: x is smaller than exactly the own candidates from upper_bound(x) on.  O(total log nc) instead
-    //      of the O(total * nc) of plain counting (measured: 22 us of shared-memory bandwidth). ----
-    uint64_t* bar = reinterpret_cast<uint64_t*>(s_misc + 8);          // 8-byte aligned (s_misc follows 2064 words)
-    if (tid == 0) {
-        mbar_init(bar, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-    if (tid == 0) {                                         // one TMA bulk copy brings the list (b + a few words = 80 KB);
-        const uint32_t bytes = static_cast<uint32_t>((min(buf_cap, total) + 1) & ~1) * 8u;   // it lands while the own
-        mbar_expect_tx(bar, bytes);                                                          // candidates are sorted
-        bulk_g2s(buf, S.g_cand, bytes, bar);
-    }
-    unsigned long long* const tree = buf + buf_cap;         // [list_cap] words behind the chunk buffer
-    const int h = sel_tree_height(nc);
-    const bool use_tree = S.use_tree && (1 << h) <= S.list_cap;           // node indices 1 .. 2^h - 1
-    {                                                       // own candidates sorted (rank by counting; the words are
-        for (int i = tid; i < nc; i += nthr) {              // distinct: the row id is part of them)
-            const unsigned long long w = s_list[i];
-            int r = 0;
-            for (int q = 0; q < nc; ++q) r += s_list[q] < w;
-            tree[use_tree ? sel_tree_node(r, h) : r] = w;
-        }
-        if (use_tree)
-            for (int r = nc + tid; r < (1 << h) - 1; r += nthr) tree[sel_tree_node(r, h)] = ~0ull;
-        __syncthreads();
-        for (int i = tid; i < nc; i += nthr) s_list[i] = tree[use_tree ? sel_tree_node(i, h) : i];
-    }
-    for (int i = tid; i <= nc; i += nthr) s_hist[i] = 0;    // difference array (nc + 1 <= 2049 entries: s_hist has 2064)
-    uint32_t phase = 0;
-    for (int base = 0; base < total; base += buf_cap) {
-        const int m = min(buf_cap, total - base);
-        __syncthreads();
-        if (base > 0 && tid == 0) {
-            const uint32_t bytes = static_cast<uint32_t>((m + 1) & ~1) * 8u;
-            mbar_expect_tx(bar, bytes);
-            bulk_g2s(buf, S.g_cand + base, bytes, bar);
-        }
-        mbar_wait(bar, phase);
-        phase ^= 1u;
-        if (dbg && base == 0) dbg[4] = clock64();
-        if (use_tree) sel_count_into_diff(buf, m, tree, h, s_hist);            // s_hist[first own candidate > x] += 1
-        else sel_count_into_diff_sorted(buf, m, s_list, nc, s_hist);
-    }
-    __syncthreads();
-    if (warp == 0) {                                        // prefix of the difference array: rank of own candidate i
-        uint32_t carry = 0;
-        for (int base = 0; base < nc; base += 32) {
-            const int i = base + lane;
-            uint32_t v = i < nc ? s_hist[i] : 0u;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const uint32_t t = __shfl_up_sync(0xffffffffu, v, o);
-                if (lane >= o) v += t;
-            }
-            if (i < nc) s_hist[i] = carry + v;
-            carry += __shfl_sync(0xffffffffu, v, 31);
-        }
-    }
-    __syncthreads();
-    for (int i = tid; i < nc; i += nthr) {
-        const uint32_t r = s_hist[i];
-        if (r < static_cast<uint32_t>(S.b)) S.out_pos[r] = static_cast<int32_t>(s_list[i] & 0xffffffffu);
-    }
-    if (dbg) { dbg[5] = clock64(); dbg[6] = total; dbg[7] = nc; }
-    if (blockIdx.x == 0 && tid == 0) {
-        unsigned long long t;
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-        reinterpret_cast<unsigned long long*>(S.g_ctr + 4)[2] = t;
-    }
+    //      of the O(total * nc) of plain counting (measured: 22 us of shared-memory bandwidth).  The searches' probes
+    //      fall into few banks and the ~b shared-memory atomics on the difference array dominate the stage: the reason
+    //      for the bucket route above. ----
+    unsigned long long* const tmp = buf + buf_cap;          // [list_cap] words behind the chunk buffer
+    sel_stream_list(S.g_cand, total, buf, buf_cap, reinterpret_cast<uint64_t*>(s_misc + 8),
+                    [&] {                                   // while the first chunk (b + a few words = 80 KB) lands: own
+                        for (int i = tid; i < nc; i += nthr) {      // candidates sorted (rank by counting; the words are
+                            const unsigned long long w = s_list[i]; // distinct: the row id is part of them)
+                            int r = 0;
+                            for (int q = 0; q < nc; ++q) r += s_list[q] < w;
+                            tmp[r] = w;
+                        }
+                        __syncthreads();
+                        for (int i = tid; i < nc; i += nthr) s_list[i] = tmp[i];
+                        for (int i = tid; i <= nc; i += nthr) s_hist[i] = 0;    // difference array (nc + 1 <= 2049 entries: s_hist has 2064)
+                    },
+                    [&](int m) { sel_count_into_diff_sorted(buf, m, s_list, nc, s_hist); });
+    sel_write_ranks(s_hist, s_list, nc, S.b, S.out_pos);
+    sel_stamp(S.g_ctr, 2);
 }
 
 __device__ __forceinline__ void sel_ll_store(void* p, unsigned int tag, unsigned int payload) {
@@ -590,37 +581,22 @@ __device__ __forceinline__ unsigned int sel_ll_wait(const void* p, unsigned int 
 // words and sums the same slice of all ranks), so every rank finds the same 22-bit threshold; the candidates (b + a few
 // words over ALL ranks, not b per rank) are stored into every window, each CTA's count follows behind a system fence
 // as an LL word; then every rank ranks the whole list (CTA c takes slice c) -- all ranks end with the same out_pos.
+// With one rank the window is this GPU's own memory and the same stores, waits, fences and tags run.
 __device__ __noinline__ void select_epilogue_mgpu(const SelArgs& S, uint32_t* s_hist, unsigned long long* s_list, int* s_misc,
                                                   unsigned long long* buf, int buf_cap) {
-    const int tid = threadIdx.x, nthr = blockDim.x, lane = tid & 31, warp = tid >> 5;
+    const int tid = threadIdx.x, nthr = blockDim.x, lane = tid & 31;
     const int grid = gridDim.x, W = S.world;
     char* const win = S.peer[S.rank];
-    long long* dbg = (S.dbg && blockIdx.x == 0 && tid == 0) ? S.dbg : nullptr;
+    uint64_t* const bar = reinterpret_cast<uint64_t*>(s_misc + 8);
     __syncthreads();
-    if (dbg) dbg[0] = clock64();
     const int cnt = s_misc[0];
     uint32_t want = static_cast<uint32_t>(S.b), T0 = 0;
     const int per = (2048 + grid - 1) / grid, b_lo = min(2048, static_cast<int>(blockIdx.x) * per), b_hi = min(2048, b_lo + per);
     for (int level = 0; level < 2; ++level) {
-        if (level == 1) {
-            for (int i = tid; i < 2048; i += nthr) s_hist[i] = 0;
-            __syncthreads();
-            for (int i = tid; i < cnt; i += nthr) {
-                const uint32_t key = static_cast<uint32_t>(s_list[i] >> 32);
-                if ((key >> 21) == T0) atomicAdd(&s_hist[(key >> 10) & 0x7ffu], 1u);
-            }
-            __syncthreads();
-        }
-        for (int i = tid; i < 2048; i += nthr) {
-            const uint32_t h = s_hist[i];
-            if (h) atomicAdd(S.g_hist + level * 2048 + i, h);
-        }
+        if (level == 1) sel_level1_hist(s_list, cnt, T0, s_hist);
+        sel_push_hist(s_hist, S.g_hist + level * 2048);
         sel_grid_barrier(S.g_ctr, static_cast<unsigned int>(2 * level + 1) * grid);
-        if (level == 0 && blockIdx.x == 0 && tid == 0) {
-            unsigned long long t;
-            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-            reinterpret_cast<unsigned long long*>(S.g_ctr + 4)[1] = t;
-        }
+        if (level == 0) sel_stamp(S.g_ctr, 1);
         // this CTA's slice of the rank histogram -> every rank; then the same slice summed over the ranks
         for (int i = tid; i < (b_hi - b_lo) * W; i += nthr) {
             const int bin = b_lo + i / W, p = i % W;
@@ -638,17 +614,7 @@ __device__ __noinline__ void select_epilogue_mgpu(const SelArgs& S, uint32_t* s_
         __syncthreads();
         for (int i = tid; i < (b_hi - b_lo); i += nthr) S.g_tot[level * 2048 + b_lo + i] = s_sum[i];
         sel_grid_barrier(S.g_ctr, static_cast<unsigned int>(2 * level + 2) * grid);
-        {
-            uint32_t hv[4];
-#pragma unroll
-            for (int k = 0; k < 4; ++k) hv[k] = (tid + k * nthr) < 2048 ? __ldcg(S.g_tot + level * 2048 + tid + k * nthr) : 0u;
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-                if ((tid + k * nthr) < 2048) {
-                    s_hist[tid + k * nthr] = hv[k];
-                    if (level == 0 && hv[k]) atomicMax(&s_misc[6], 2047 - (tid + k * nthr));   // first populated bin, all ranks
-                }
-        }
+        sel_load_hist(S.g_tot + level * 2048, s_hist, level == 0 ? &s_misc[6] : nullptr);     // first populated bin: all ranks
         __syncthreads();
         sel_find_bin(s_hist, want, reinterpret_cast<uint32_t*>(s_misc + 16), &s_misc[level == 0 ? 1 : 5], &s_misc[2]);
         want = static_cast<uint32_t>(s_misc[2]);
@@ -658,17 +624,9 @@ __device__ __noinline__ void select_epilogue_mgpu(const SelArgs& S, uint32_t* s_
     const uint32_t T = (T0 << 11) | static_cast<uint32_t>(s_misc[5]);
     if (tid == 0) s_misc[4] = 0;
     __syncthreads();
-    if (dbg) dbg[1] = clock64();
     // ---- this CTA's candidates -> the rank's region of every window; the count follows behind a system fence ----
-    for (int i = tid; i < cnt; i += nthr) {
-        const unsigned long long w = s_list[i];
-        if (static_cast<uint32_t>(w >> 42) <= T) buf[atomicAdd(&s_misc[4], 1)] = w;
-    }
-    __syncthreads();
-    const int nc = s_misc[4];
-    if (tid == 0) s_misc[3] = static_cast<int>(atomicAdd(S.g_ctr + 1, static_cast<unsigned int>(nc)));
-    __syncthreads();
-    const int off = s_misc[3];
+    int off;
+    const int nc = sel_gather_candidates(S, s_list, cnt, T, buf, s_misc, off);
     if (off + nc > S.cand_cap && tid == 0) { *reinterpret_cast<volatile int*>(S.status) = ALQ_ERR_STATE; __threadfence_system(); }
     for (int i = tid; i < nc * W; i += nthr) {
         const int k = i / W, p = i % W;
@@ -691,7 +649,6 @@ __device__ __noinline__ void select_epilogue_mgpu(const SelArgs& S, uint32_t* s_
         if (v) atomicAdd(&s_tot[r], v);
     }
     __syncthreads();
-    if (dbg) dbg[2] = clock64();
     // ---- the list = the rank segments one after the other (each padded to an even word count with a ~0 word that sorts
     //      behind everything).  CTA c ranks slice c of it against all of it. ----
     int seg_off[ALQ_MAX_WORLD + 1];
@@ -713,52 +670,29 @@ __device__ __noinline__ void select_epilogue_mgpu(const SelArgs& S, uint32_t* s_
     //      the words of the buckets below; it then orders its bucket alone.  One more grid barrier tells every CTA
     //      whether all buckets fitted; if one did not (tie groups), the general ranking below runs instead. ----
     {
-        const float lo = sel_key_to_float(static_cast<uint32_t>(2047 - s_misc[6]) << 21);
-        const float hi = sel_key_to_float((T << 10) | 0x3ffu);
-        const float scale = static_cast<float>(grid) / (hi - lo);
-        if (isfinite(lo) && isfinite(hi) && hi > lo && isfinite(scale) && S.bucket_cap > 0) {
-            uint64_t* bar = reinterpret_cast<uint64_t*>(s_misc + 8);
-            if (tid == 0) {
-                s_misc[48] = 0; s_misc[49] = 0; s_misc[50] = 0;
-                mbar_init(bar, 1);
-                asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-            }
-            if (dbg) dbg[3] = clock64();
-            uint32_t phase = 0;
+        const SelBuckets bk(2047 - s_misc[6], T, grid);
+        if (bk.spread && S.bucket_cap > 0) {
+            if (tid == 0) { s_misc[48] = 0; s_misc[49] = 0; s_misc[50] = 0; }
             int below = 0;
             const int me = static_cast<int>(blockIdx.x);
-            for (int r = 0; r < W; ++r) {
-                const int tot_r = static_cast<int>(s_tot[r]);
-                for (int base = 0; base < tot_r; base += buf_cap) {
-                    const int m = min(buf_cap, tot_r - base);
-                    __syncthreads();
-                    if (tid == 0) {
-                        const uint32_t bytes = static_cast<uint32_t>((m + 1) & ~1) * 8u;
-                        mbar_expect_tx(bar, bytes);
-                        bulk_g2s(buf, cand + static_cast<size_t>(r) * S.cand_cap + base, bytes, bar);
-                    }
-                    mbar_wait(bar, phase);
-                    phase ^= 1u;
-                    for (int j = tid; j < m; j += nthr) {
-                        const unsigned long long x = buf[j];
-                        const float sc = sel_key_to_float(static_cast<uint32_t>(x >> 32));
-                        const int q = min(grid - 1, max(0, __float2int_rd((sc - lo) * scale)));
-                        if (q < me) ++below;
-                        else if (q == me) {
-                            const int slot = atomicAdd(&s_misc[48], 1);
-                            if (slot < S.list_cap) s_list[slot] = x;
-                        }
-                    }
-                }
-            }
+            for (int r = 0; r < W; ++r)
+                sel_stream_list(cand + static_cast<size_t>(r) * S.cand_cap, static_cast<int>(s_tot[r]), buf, buf_cap, bar, [] {},
+                                [&](int m) {
+                                    for (int j = tid; j < m; j += nthr) {
+                                        const unsigned long long x = buf[j];
+                                        const int q = bk.of(x);
+                                        if (q < me) ++below;
+                                        else if (q == me) {
+                                            const int slot = atomicAdd(&s_misc[48], 1);
+                                            if (slot < S.list_cap) s_list[slot] = x;
+                                        }
+                                    }
+                                });
 #pragma unroll
             for (int o = 16; o > 0; o >>= 1) below += __shfl_xor_sync(0xffffffffu, below, o);
             if (lane == 0 && below) atomicAdd(&s_misc[49], below);
             __syncthreads();
-            if (tid == 0) {
-                asm volatile("mbarrier.inval.shared.b64 [%0];" ::"r"(static_cast<uint32_t>(__cvta_generic_to_shared(bar))) : "memory");
-                S.g_hist[me] = static_cast<unsigned int>(s_misc[48]);          // the rank's level-0 bins are no longer read
-            }
+            if (tid == 0) S.g_hist[me] = static_cast<unsigned int>(s_misc[48]);          // the rank's level-0 bins are no longer read
             sel_grid_barrier(S.g_ctr, 5u * grid);
             {
                 int mx = 0;
@@ -769,19 +703,8 @@ __device__ __noinline__ void select_epilogue_mgpu(const SelArgs& S, uint32_t* s_
             }
             __syncthreads();
             if (s_misc[50] <= S.list_cap) {
-                const int mine = s_misc[48], base = s_misc[49];
-                for (int i = tid; i < mine; i += nthr) {
-                    const unsigned long long w = s_list[i];
-                    int rk = base;
-                    for (int q = 0; q < mine; ++q) rk += s_list[q] < w;
-                    if (rk < S.b) S.out_pos[rk] = static_cast<int32_t>(w & 0xffffffffu);
-                }
-                if (dbg) { dbg[4] = clock64(); dbg[5] = dbg[4]; dbg[6] = -M; dbg[7] = mine; }
-                if (blockIdx.x == 0 && tid == 0) {
-                    unsigned long long t;
-                    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-                    reinterpret_cast<unsigned long long*>(S.g_ctr + 4)[2] = t;
-                }
+                sel_rank_bucket(s_list, s_misc[48], s_misc[49], S.b, S.out_pos);
+                sel_stamp(S.g_ctr, 2);
                 return;
             }
             __syncthreads();
@@ -807,58 +730,13 @@ __device__ __noinline__ void select_epilogue_mgpu(const SelArgs& S, uint32_t* s_
             s_list[r] = w;
         }
     }
-    // (the slice is searched as a sorted array: see the note on the breadth-first tree above sel_tree_height)
     __syncthreads();
     for (int i = tid; i <= n2; i += nthr) s_hist[i] = 0;
-    uint64_t* bar = reinterpret_cast<uint64_t*>(s_misc + 8);
-    if (tid == 0) {
-        mbar_init(bar, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    uint32_t phase = 0;
-    if (dbg) dbg[3] = clock64();
-    for (int r = 0; r < W; ++r) {
-        const int tot_r = static_cast<int>(s_tot[r]);
-        for (int base = 0; base < tot_r; base += buf_cap) { // one TMA bulk copy per chunk of a rank segment
-            const int m = min(buf_cap, tot_r - base);
-            __syncthreads();
-            if (tid == 0) {
-                const uint32_t bytes = static_cast<uint32_t>((m + 1) & ~1) * 8u;
-                mbar_expect_tx(bar, bytes);
-                bulk_g2s(buf, cand + static_cast<size_t>(r) * S.cand_cap + base, bytes, bar);
-            }
-            mbar_wait(bar, phase);
-            phase ^= 1u;
-            sel_count_into_diff_sorted(buf, m, s_list, n2, s_hist);
-        }
-    }
-    __syncthreads();
-    if (warp == 0) {
-        uint32_t carry = 0;
-        for (int base = 0; base < n2; base += 32) {
-            const int i = base + lane;
-            uint32_t v = i < n2 ? s_hist[i] : 0u;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const uint32_t t = __shfl_up_sync(0xffffffffu, v, o);
-                if (lane >= o) v += t;
-            }
-            if (i < n2) s_hist[i] = carry + v;
-            carry += __shfl_sync(0xffffffffu, v, 31);
-        }
-    }
-    __syncthreads();
-    for (int i = tid; i < n2; i += nthr) {
-        const uint32_t r = s_hist[i];
-        const unsigned long long w = s_list[i];
-        if (r < static_cast<uint32_t>(S.b) && w != ~0ull) S.out_pos[r] = static_cast<int32_t>(w & 0xffffffffu);
-    }
-    if (dbg) { dbg[4] = clock64(); dbg[5] = clock64(); dbg[6] = M; dbg[7] = n2; }
-    if (blockIdx.x == 0 && tid == 0) {
-        unsigned long long t;
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-        reinterpret_cast<unsigned long long*>(S.g_ctr + 4)[2] = t;
-    }
+    for (int r = 0; r < W; ++r)                             // the rank segments one after the other
+        sel_stream_list(cand + static_cast<size_t>(r) * S.cand_cap, static_cast<int>(s_tot[r]), buf, buf_cap, bar, [] {},
+                        [&](int m) { sel_count_into_diff_sorted(buf, m, s_list, n2, s_hist); });
+    sel_write_ranks(s_hist, s_list, n2, S.b, S.out_pos);
+    sel_stamp(S.g_ctr, 2);
 }
 
 // MODE 0..2: scores; MODE 3: BADGE factors (writes a[row, :] and a_norm2[row]);
@@ -881,11 +759,7 @@ rows_pipe_kernel(const float* __restrict__ logits, int64_t n, int c, RowPipeCfg 
     if (sel.b > 0) {
         for (int i = threadIdx.x; i < 2048; i += blockDim.x) s_hist[i] = 0;
         if (threadIdx.x < 48) s_misc[threadIdx.x] = 0;
-        if (blockIdx.x == 0 && threadIdx.x == 0) {
-            unsigned long long t;
-            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-            reinterpret_cast<unsigned long long*>(sel.g_ctr + 4)[0] = t;
-        }
+        sel_stamp(sel.g_ctr, 0);
     }
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int R = cfg.rows_per_tile;
@@ -1001,7 +875,15 @@ rows_pipe_kernel(const float* __restrict__ logits, int64_t n, int c, RowPipeCfg 
         }
     }
     if (sel.b > 0) {     // every thread of the CTA (the tile ring is free now: it becomes the candidate buffer)
-        if (sel.world > 1) select_epilogue_mgpu(sel, s_hist, s_list, s_misc, reinterpret_cast<unsigned long long*>(tiles),
+        // Every warp has left the stream, so every bulk copy into the ring has completed and been waited on: the ring's
+        // full[] / empty[] barriers are invalidated before the epilogue reuses their words as plain memory (it starts
+        // with a barrier).
+        __syncthreads();
+        if (threadIdx.x == 0) {                          // full[] and empty[] (SelArgs: nothing stays live across the loop)
+            uint64_t* ring = reinterpret_cast<uint64_t*>(smem_rows + sel.ring_off);
+            for (int s = 0; s < sel.ring_bars; ++s) mbar_inval(&ring[s]);
+        }
+        if (sel.world > 0) select_epilogue_mgpu(sel, s_hist, s_list, s_misc, reinterpret_cast<unsigned long long*>(tiles),
                                                 sel.list_off / 8 - sel.list_cap - 2);
         else select_epilogue(sel, s_hist, s_list, s_misc, reinterpret_cast<unsigned long long*>(tiles),
                              sel.list_off / 8 - sel.list_cap - 2);
@@ -1382,7 +1264,7 @@ static int uncertainty_tail_impl(alq_ctx* ctx, const float* logits, int64_t n, i
     if (!logits || !scores || !out_pos) ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_uncertainty_tail: null pointer");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     AlqComm& G = ctx->comm;
-    if (sharded && (G.world <= 1 || !G.connected)) ALQ_FAIL(ctx, ALQ_ERR_STATE, "alq_uncertainty_tail_sharded: no multi-GPU group (alq_comm_create/connect)");
+    if (sharded && (G.world < 1 || !G.connected)) ALQ_FAIL(ctx, ALQ_ERR_STATE, "alq_uncertainty_tail_sharded: no peer-memory group (alq_comm_create/connect)");
     if (!sharded) { rows_min = rows_max = n; }
     constexpr int kListCap = 2048;
     const size_t reserve = static_cast<size_t>(kListCap) * 8 + 2064 * 4 + 512;      // list, histogram / difference array, s_misc[128]
@@ -1440,11 +1322,6 @@ static int uncertainty_tail_impl(alq_ctx* ctx, const float* logits, int64_t n, i
     sel.g_ctr = slot + 4 * 2048;
     sel.g_tot = slot + 2 * 2048;
     ctx->sel_last_ctr = sel.g_ctr;
-    static long long* dbg_buf = nullptr;
-    if (getenv("ALQ_SELECT_DEBUG")) {
-        if (!dbg_buf) cudaMalloc(&dbg_buf, 8 * sizeof(long long));
-        sel.dbg = dbg_buf;
-    }
     {
         ScratchCursor cur(ctx->scratch);
         sel.g_cand = cur.take<unsigned long long>(n + 2);
@@ -1456,7 +1333,8 @@ static int uncertainty_tail_impl(alq_ctx* ctx, const float* logits, int64_t n, i
         }
     }
     sel.out_pos = out_pos;
-    sel.use_tree = getenv("ALQ_TAIL_TREE") ? 1 : 0;
+    sel.ring_off = cfg.stages * cfg.tile_floats * 4;        // behind the stages' tiles
+    sel.ring_bars = 2 * cfg.stages;
     if (sharded) {
         G.epoch += 1;
         sel.world = G.world; sel.rank = G.rank;
@@ -1484,19 +1362,6 @@ static int uncertainty_tail_impl(alq_ctx* ctx, const float* logits, int64_t n, i
     if (e != cudaSuccess) {
         cudaGetLastError();
         ALQ_FAIL(ctx, ALQ_ERR_CUDA, "alq_uncertainty_tail: cooperative launch failed: %s", cudaGetErrorString(e));
-    }
-    if (sel.dbg && sharded) {
-        long long h[8];
-        cudaStreamSynchronize(st);
-        cudaMemcpy(h, sel.dbg, sizeof(h), cudaMemcpyDeviceToHost);
-        fprintf(stderr, "[alq fused tail dbg, rank %d] cycles: two summed histogram levels %lld, candidates + counts %lld, list load %lld, rank %lld | list %lld words, CTA 0 ranks %lld\n",
-                G.rank, h[1] - h[0], h[2] - h[1], h[3] - h[2], h[4] - h[3], h[6], h[7]);
-    } else if (sel.dbg) {
-        long long h[8];
-        cudaStreamSynchronize(st);
-        cudaMemcpy(h, sel.dbg, sizeof(h), cudaMemcpyDeviceToHost);
-        fprintf(stderr, "[alq fused tail dbg] cycles: level0 %lld level1 %lld candidates %lld load %lld rank %lld | total candidates %lld, CTA 0 holds %lld\n",
-                h[1] - h[0], h[2] - h[1], h[3] - h[2], h[4] - h[3], h[5] - h[4], h[6], h[7]);
     }
     return ALQ_OK;
 }

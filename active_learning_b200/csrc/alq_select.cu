@@ -569,7 +569,7 @@ extern "C" int alq_topb_exchange(alq_ctx* ctx, const float* scores, const int32_
                                  int64_t b, int32_t* out_gpos, void* stream) {
     if (!ctx) return ALQ_ERR_INVALID;
     AlqComm& G = ctx->comm;
-    if (G.world <= 1 || !G.connected) ALQ_FAIL(ctx, ALQ_ERR_STATE, "alq_topb_exchange: no multi-GPU group (alq_comm_create/connect)");
+    if (G.world < 1 || !G.connected) ALQ_FAIL(ctx, ALQ_ERR_STATE, "alq_topb_exchange: no peer-memory group (alq_comm_create/connect)");
     if (k < 0 || b < 1 || k > b || b > static_cast<int64_t>(AlqComm::kTopbWords) || !out_gpos || (k > 0 && (!scores || !pos)))
         ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_topb_exchange: bad arguments (k=%lld b=%lld, b <= %zu)", (long long)k, (long long)b,
                  AlqComm::kTopbWords);

@@ -13,8 +13,6 @@
 //        position order by one warp walking the slice with ballots;
 //   6    every CTA sorts its share (B/8 words) in shared memory (bitonic network) -> barrier;
 //   7    every CTA pulls all sorted shares into shared memory and places its own words by binary searches.
-#include <stdlib.h>
-
 #include "alq_common.cuh"
 
 namespace selc {
@@ -30,9 +28,7 @@ struct Scratch {
     uint32_t* counts;           // [CL][2]  (lt, eq)
     unsigned long long* words;  // [MAX_B]      winners, unordered
     unsigned long long* sorted; // [MAX_B + 2]  per-CTA sorted shares
-    long long* dbg;             // optional phase stamps (ALQ_SELECT_DEBUG)
 };
-#define SELC_STAMP(i) do { if (S.dbg && threadIdx.x == 0 && rank == 0) S.dbg[i] = clock64(); } while (0)
 
 __device__ __forceinline__ uint32_t score_key(float s) { return alq_ord(s + 0.0f); }
 
@@ -52,7 +48,6 @@ select_cluster_kernel(const float* __restrict__ scores, int n, int b, Scratch S,
     const int lo = rank * per, hi = min(n, lo + per);
     const int cnt = max(0, hi - lo);
 
-    SELC_STAMP(0);
     // ---- stage 0: slice -> keys in shared memory, level-0 histogram on the way -------------------------------
     for (int i = threadIdx.x; i < BINS; i += THREADS) hist[i] = 0;
     if (threadIdx.x == 0) { sh_prefix = 0; sh_k = static_cast<unsigned long long>(b); }
@@ -64,7 +59,6 @@ select_cluster_kernel(const float* __restrict__ scores, int n, int b, Scratch S,
     }
     __syncthreads();
 
-    SELC_STAMP(1);
     // ---- stages 1-3: radix levels ---------------------------------------------------------------------------
 #pragma unroll 1
     for (int level = 0; level < 3; ++level) {
@@ -111,7 +105,6 @@ select_cluster_kernel(const float* __restrict__ scores, int n, int b, Scratch S,
         }
         __syncthreads();
     }
-    SELC_STAMP(2);
     const uint32_t T = sh_prefix;
     const unsigned long long ties = sh_k;                       // how many keys equal to T are inside the budget
     const unsigned long long n_less = static_cast<unsigned long long>(b) - ties;
@@ -147,7 +140,6 @@ select_cluster_kernel(const float* __restrict__ scores, int n, int b, Scratch S,
         eq_off += __ldcg(&S.counts[q * 2 + 1]);
     }
 
-    SELC_STAMP(3);
     // ---- stage 5: compaction of the B winners as (key << 32 | position) words ------------------------------------
     {
         uint32_t lt_run = lt_off + lt_before;
@@ -170,7 +162,6 @@ select_cluster_kernel(const float* __restrict__ scores, int n, int b, Scratch S,
     }
     cluster_sync_all();
 
-    SELC_STAMP(4);
     // ---- stage 6: every CTA sorts its share of the words (<= MAX_B / CL = 2048, padded with ~0) with a bitonic
     //      network in shared memory (an all-pairs rank count was measured 3x slower: 79k vs 27k cycles) ---------
     unsigned long long* sk = reinterpret_cast<unsigned long long*>(smem_sel);      // the key slice is no longer needed
@@ -184,7 +175,6 @@ select_cluster_kernel(const float* __restrict__ scores, int n, int b, Scratch S,
     for (int i = threadIdx.x; i < s_cnt; i += THREADS) S.sorted[s_lo + i] = sk[i];
     cluster_sync_all();
 
-    SELC_STAMP(5);
     // ---- stage 7: all sorted shares into shared memory, place this CTA's share by rank counting -------------------
     {
         // one TMA bulk copy per CTA brings all sorted shares (<= 128 KB) into shared memory
@@ -225,7 +215,6 @@ select_cluster_kernel(const float* __restrict__ scores, int n, int b, Scratch S,
         for (int r = 0; r < CL; ++r) rk += l[r];
         out_pos[rk] = static_cast<int32_t>(key & 0xffffffffu);
     }
-    SELC_STAMP(6);
 }
 
 }  // namespace selc
@@ -245,12 +234,6 @@ int alq_select_smallest_cluster(alq_ctx* ctx, const float* scores, int64_t n, in
     S.counts = cur.take<uint32_t>(CL * 2);
     S.words = cur.take<unsigned long long>(MAX_B);
     S.sorted = cur.take<unsigned long long>(MAX_B + 2);
-    S.dbg = nullptr;
-    static long long* dbg_buf = nullptr;
-    if (getenv("ALQ_SELECT_DEBUG")) {
-        if (!dbg_buf) cudaMalloc(&dbg_buf, 8 * sizeof(long long));
-        S.dbg = dbg_buf;
-    }
     const int per = ((static_cast<int>(n) + CL - 1) / CL + 3) & ~3;
     size_t smem = std::max<size_t>(std::max<size_t>(static_cast<size_t>(per) * 4, static_cast<size_t>(b + 2) * 8), 2048 * 8) + 64;
     if (smem > ctx->smem_optin - 24 * 1024) return ALQ_ERR_STATE;
@@ -261,12 +244,5 @@ int alq_select_smallest_cluster(alq_ctx* ctx, const float* scores, int64_t n, in
     }
     select_cluster_kernel<<<CL, THREADS, smem, st>>>(scores, static_cast<int>(n), static_cast<int>(b), S, out_pos);
     ALQ_LAUNCH_CHECK(ctx);
-    if (S.dbg) {
-        long long h[8];
-        cudaStreamSynchronize(st);
-        cudaMemcpy(h, S.dbg, sizeof(h), cudaMemcpyDeviceToHost);
-        fprintf(stderr, "[alq select dbg] load %lld levels %lld counts %lld compact %lld sort %lld merge %lld\n", h[1] - h[0],
-                h[2] - h[1], h[3] - h[2], h[4] - h[3], h[5] - h[4], h[6] - h[5]);
-    }
     return ALQ_OK;
 }

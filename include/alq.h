@@ -102,7 +102,7 @@ int alq_uncertainty_tail(alq_ctx* ctx, const float* logits, int64_t n, int32_t c
  * %globaltimer stamps of CTA 0.  ALQ_ERR_STATE if that call ran the separate kernels instead.                         */
 int alq_uncertainty_tail_timing(alq_ctx* ctx, float* out_ms_host);
 
-/* The same tail with the rows sharded over the G ranks of the peer-memory group (alq_comm_create/connect): rank r holds
+/* The same tail with the rows sharded over the G >= 1 ranks of the peer-memory group (alq_comm_create/connect): rank r holds
  * `n` rows that are positions [row_lo, row_lo + n) of the pool and every rank receives the same out_gpos[0..b): the global
  * positions of the b smallest scores over ALL ranks, ascending (score, position) -- exactly what a single GPU returns for
  * the concatenated pool.  K1, K1b and the exchange are ONE launch per rank: both histogram levels are summed over
@@ -126,8 +126,8 @@ int alq_topb_pack(alq_ctx* ctx, const float* scores, const int32_t* pos, int64_t
 int alq_topb_merge(alq_ctx* ctx, const uint64_t* keys, int64_t n, int64_t list_len, int64_t b,
                    int32_t* out_gpos, void* stream);
 
-/* The same exchange over the peer-memory windows of alq_comm_create/connect instead of a collective library:
- * pack + store into every peer's window + flag, then wait + merge (b <= 16384).  Collective: every rank of the
+/* The same exchange over the peer-memory windows of alq_comm_create/connect (G >= 1 ranks) instead of a collective
+ * library: pack + store into every peer's window + flag, then wait + merge (b <= 16384).  Collective: every rank of the
  * group must call it, in the same order relative to its other group calls.                      */
 int alq_topb_exchange(alq_ctx* ctx, const float* scores, const int32_t* pos, int64_t k, int64_t row_lo,
                       int64_t b, int32_t* out_gpos, void* stream);

@@ -57,6 +57,32 @@ class BoundaryUniforms:
         return u
 
 
+# Pools of the fused uncertainty-tail tests: the one-GPU call and one rank of the sharded call run the same inputs.
+FUSED_TAIL_SHAPES = [(80000, 1000, 10000), (80000, 1000, 1), (5000, 40, 5000), (4100, 12, 77), (30011, 1000, 3000),
+                     (200000, 8, 16000)]
+
+
+def fused_tail_logits(n, c, b, mode):
+    g = torch.Generator(device="cuda").manual_seed(n + c + b + mode)
+    return torch.randn(n, c, device="cuda", generator=g) * 3
+
+
+def skewed_tail_pools(mode):
+    """(logits, b) whose scores do not spread evenly between the candidate range's edges (per-row temperature over five
+    decades: the margins pile up next to 0, the confidences next to 1/C and 1)."""
+    g = torch.Generator(device="cuda").manual_seed(77 + mode)
+    for n, c, b in ((90000, 1000, 10000), (120000, 40, 30000), (50000, 16, 49000)):
+        temp = torch.exp(torch.randn(n, 1, device="cuda", generator=g) * 4)
+        yield torch.randn(n, c, device="cuda", generator=g) * temp, b
+
+
+def tied_tail_pools():
+    """(logits, b) of dyadic logits: thousands of rows share a score exactly."""
+    rng = np.random.default_rng(5)
+    for n, c, b in ((60000, 8, 9000), (150000, 4, 12000)):
+        yield torch.from_numpy(rng.integers(-2, 3, size=(n, c)).astype(np.float32)).cuda(), b
+
+
 class IndexDataset(torch.utils.data.Dataset):
     def __init__(self, n, num_classes):
         self.n, self.num_classes = n, num_classes

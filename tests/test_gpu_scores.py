@@ -4,6 +4,7 @@ import numpy as np
 import pytest
 import torch
 
+from helpers import FUSED_TAIL_SHAPES, fused_tail_logits, skewed_tail_pools, tied_tail_pools
 from oracle import al_oracle as O
 
 pytestmark = pytest.mark.gpu
@@ -210,14 +211,13 @@ def test_pipelined_rows_kernels_equal_direct_kernels(eng, n, c):
     assert torch.allclose(res["pipelined"][3][:, :c], O.badge_factors(logits, 128), rtol=0, atol=1e-7)
 
 
-@pytest.mark.parametrize("n,c,b", [(80000, 1000, 10000), (80000, 1000, 1), (5000, 40, 5000), (4100, 12, 77), (30011, 1000, 3000), (200000, 8, 16000)])
+@pytest.mark.parametrize("n,c,b", FUSED_TAIL_SHAPES)
 @pytest.mark.parametrize("mode", [0, 1, 2])
 def test_fused_tail_equals_score_then_select(eng, n, c, b, mode):
     """alq_uncertainty_tail (K1 + K1b as one launch: per-CTA key lists, two global 11-bit histogram levels, winners
     ordered either through per-CTA score buckets or by ranking against the whole list) against the two separate kernels:
     identical scores, identical ordered positions, on both routes."""
-    g = torch.Generator(device="cuda").manual_seed(n + c + b + mode)
-    logits = torch.randn(n, c, device="cuda", generator=g) * 3
+    logits = fused_tail_logits(n, c, b, mode)
     ref_s = eng.score_softmax(logits, mode)
     ref_p = eng.select_smallest(ref_s, b)
     try:
@@ -235,10 +235,7 @@ def test_fused_tail_with_skewed_scores(eng, mode):
     """Scores that do not spread evenly between the candidate range's edges (per-row temperature over five decades: the
     margins pile up next to 0, the confidences next to 1/C and 1): the score buckets are uneven, and with the 40-row pool
     piled into a few of them one bucket exceeds its capacity and the launch falls back to the general route by itself."""
-    g = torch.Generator(device="cuda").manual_seed(77 + mode)
-    for n, c, b in ((90000, 1000, 10000), (120000, 40, 30000), (50000, 16, 49000)):
-        temp = torch.exp(torch.randn(n, 1, device="cuda", generator=g) * 4)
-        logits = torch.randn(n, c, device="cuda", generator=g) * temp
+    for logits, b in skewed_tail_pools(mode):
         ref_s = eng.score_softmax(logits, mode)
         s, p = eng.uncertainty_tail(logits, mode, b)
         assert torch.equal(s, ref_s)
@@ -248,9 +245,7 @@ def test_fused_tail_with_skewed_scores(eng, mode):
 def test_fused_tail_with_massive_ties(eng):
     """Dyadic logits: thousands of rows share a score exactly, the threshold bin of the fused selection holds far more
     keys than the budget needs (and more than one shared-memory chunk): ties must still resolve by position."""
-    rng = np.random.default_rng(5)
-    for n, c, b in ((60000, 8, 9000), (150000, 4, 12000)):
-        logits = torch.from_numpy(rng.integers(-2, 3, size=(n, c)).astype(np.float32)).cuda()
+    for logits, b in tied_tail_pools():
         for mode in (0, 1, 2):
             ref_s = eng.score_softmax(logits, mode)
             s, p = eng.uncertainty_tail(logits, mode, b)
