@@ -1,0 +1,475 @@
+// K7 / K8: Ward agglomerative clustering with a merge tree identical to scipy's, for MarginClusteringSampler
+// (margin_clustering_sampler.py:59 under active_learning/src/query_strategies runs
+// sklearn.cluster.AgglomerativeClustering(n_clusters=20), i.e. scipy.cluster.hierarchy.ward over the full tree).
+//
+// K7 alq_pdist_f64   the full symmetric n x n fp64 matrix of scipy's pdist(X, 'euclidean'): fp32 rows widened to
+//                    fp64 (exact), s summed k = 0, 1, ... as `d = a - b; s = s + d*d` with no FMA, then sqrt(s).
+//                    One CTA owns a 64 x 64 tile of pairs of the upper triangle (each pair computed once, written to
+//                    (i, j) and (j, i)); 256 threads x 4 x 4 pairs in registers; k-chunks of both row blocks arrive
+//                    with 4-byte cp.async (any ld, any alignment, zero-filled past d and past n) into a two-stage fp32
+//                    ring and are widened once into an fp64 tile that the inner loop reads.
+// K8 alq_ward_nn_chain  scipy's nn_chain (Ward update) as ONE launch of one thread-block cluster (16 CTAs when the GPU
+//                    can place them, else 8).  CTA r owns columns [lo_r, hi_r) with their cluster sizes in shared
+//                    memory.  A scan of row x: per-CTA (value, lowest index) -> DSMEM exchange -> every CTA resolves
+//                    the same winner -> one cluster barrier.  A merge updates the CTA's slice of row y and the
+//                    mirrored entries D[i, y] of its rows, then one cluster barrier.
+//
+// Memory ordering of K8 (entries of D written by one SM and read by another): every write happens before a
+// `barrier.cluster.arrive.release` of its CTA and every read after a `barrier.cluster.wait.acquire` of the reader;
+// all reads of D go through ld.global.cg (L2, never a possibly stale L1 line) and all writes through st.global.cg.
+//
+// Offsets into `dist` are int64 (n^2 passes 2^31 at n = 46 341); row indices themselves are int32.
+#include <cooperative_groups.h>
+#include <math_constants.h>
+
+#include <climits>
+#include <cmath>
+#include <numeric>
+
+#include "alq_common.cuh"
+
+namespace cg = cooperative_groups;
+
+namespace ward {
+
+// ---------------------------------------------------------------------------------------------------------------
+// K7
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int PD_TILE = 64;
+constexpr int PD_KC = 16;
+constexpr int PD_THREADS = 256;
+constexpr int PD_PAD = PD_TILE + 1;      // fp32 staging row pitch: the transposed cp.async stores hit 32 banks
+
+__device__ __forceinline__ void cp_async4(void* smem, const void* gmem, bool pred) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(smem_u32(smem)), "l"(gmem), "r"(pred ? 4 : 0)
+                 : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+
+__global__ void __launch_bounds__(PD_THREADS, 2)
+pdist_f64_kernel(const float* __restrict__ x, int n, int d, int64_t ldx, double* __restrict__ dist, int64_t ldd) {
+    const int ti = blockIdx.y, tj = blockIdx.x;
+    if (ti > tj) return;                                   // upper triangle of tiles only
+    __shared__ float s32[2][2][PD_KC][PD_PAD];             // [stage][operand][k][row]
+    __shared__ double s64[2][PD_KC][PD_TILE];              // [operand][k][row]
+    const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+    const int row_i = ti * PD_TILE, row_j = tj * PD_TILE;
+    const int nch = (d + PD_KC - 1) / PD_KC;
+
+    auto issue = [&](int c, int stage) {
+        const int k0 = c * PD_KC;
+#pragma unroll
+        for (int j = 0; j < (2 * PD_TILE * PD_KC) / PD_THREADS; ++j) {
+            const int idx = tid + j * PD_THREADS;          // consecutive threads: consecutive k of one row
+            const int op = idx / (PD_TILE * PD_KC), rem = idx % (PD_TILE * PD_KC);
+            const int r = rem / PD_KC, k = rem % PD_KC;
+            const int gr = (op ? row_j : row_i) + r, gk = k0 + k;
+            const bool ok = gr < n && gk < d;
+            cp_async4(&s32[stage][op][k][r], ok ? x + static_cast<int64_t>(gr) * ldx + gk : x, ok);
+        }
+        cp_async_commit();
+    };
+
+    double acc[4][4];
+#pragma unroll
+    for (int a = 0; a < 4; ++a)
+#pragma unroll
+        for (int b = 0; b < 4; ++b) acc[a][b] = 0.0;
+
+    issue(0, 0);
+#pragma unroll 1
+    for (int c = 0; c < nch; ++c) {
+        cp_async_wait_all();
+        __syncthreads();                                   // chunk c landed; the previous chunk's fp64 tile is consumed
+        for (int idx = tid; idx < 2 * PD_KC * PD_TILE; idx += PD_THREADS) {
+            const int op = idx / (PD_KC * PD_TILE), rem = idx % (PD_KC * PD_TILE);
+            const int k = rem / PD_TILE, r = rem % PD_TILE;
+            s64[op][k][r] = static_cast<double>(s32[c & 1][op][k][r]);
+        }
+        __syncthreads();
+        if (c + 1 < nch) issue(c + 1, (c + 1) & 1);         // overlaps the compute below
+#pragma unroll
+        for (int k = 0; k < PD_KC; ++k) {
+            double av[4], bv[4];
+#pragma unroll
+            for (int a = 0; a < 4; ++a) av[a] = s64[0][k][ty + 16 * a];
+#pragma unroll
+            for (int b = 0; b < 4; ++b) bv[b] = s64[1][k][tx + 16 * b];
+#pragma unroll
+            for (int a = 0; a < 4; ++a)
+#pragma unroll
+                for (int b = 0; b < 4; ++b) {
+                    const double df = __dsub_rn(av[a], bv[b]);
+                    acc[a][b] = __dadd_rn(acc[a][b], __dmul_rn(df, df));
+                }
+        }
+    }
+#pragma unroll
+    for (int a = 0; a < 4; ++a) {
+        const int i = row_i + ty + 16 * a;
+#pragma unroll
+        for (int b = 0; b < 4; ++b) {
+            const int j = row_j + tx + 16 * b;
+            if (i < n && j < n && (ti != tj || i <= j)) {
+                const double v = __dsqrt_rn(acc[a][b]);
+                dist[static_cast<int64_t>(i) * ldd + j] = v;
+                dist[static_cast<int64_t>(j) * ldd + i] = v;
+            }
+        }
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// K8
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int NC_THREADS = 512;
+constexpr int NC_WARPS = NC_THREADS / 32;
+
+struct Cand {               // a scan's partial result: value, lowest column attaining it, that column's cluster size
+    double v;
+    int i;
+    int s;
+};
+
+__device__ __forceinline__ void cand_min(Cand& c, double v, int i, int s) {
+    if (v < c.v || (v == c.v && i < c.i)) { c.v = v; c.i = i; c.s = s; }      // NaN never wins
+}
+__device__ __forceinline__ void warp_cand_min(Cand& c) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const double v = __shfl_xor_sync(0xffffffffu, c.v, o);
+        const int i = __shfl_xor_sync(0xffffffffu, c.i, o);
+        const int s = __shfl_xor_sync(0xffffffffu, c.s, o);
+        cand_min(c, v, i, s);
+    }
+}
+
+// scipy's _ward (_hierarchy_distance_update.pxi), evaluated left to right without contraction
+__device__ __forceinline__ double ward_update(double dxi, double dyi, double dxy, int nx, int ny, int ni) {
+    const double t = __ddiv_rn(1.0, static_cast<double>(nx + ny + ni));
+    const double a = __dmul_rn(__dmul_rn(__dmul_rn(static_cast<double>(ni + nx), t), dxi), dxi);
+    const double b = __dmul_rn(__dmul_rn(__dmul_rn(static_cast<double>(ni + ny), t), dyi), dyi);
+    const double c = __dmul_rn(__dmul_rn(__dmul_rn(static_cast<double>(ni), t), dxy), dxy);
+    return __dsqrt_rn(__dsub_rn(__dadd_rn(a, b), c));
+}
+
+// dist: n x n (ldd), consumed.  chain_all: [cluster size][n] int2 (index, cluster size), one stack per CTA (every CTA
+// walks the same chain; private copies need no cross-CTA ordering).  status: 0, or ALQ_ERR_NUMERIC if a scan of a
+// one-element chain found no finite candidate (non-finite distances).
+__global__ void __launch_bounds__(NC_THREADS, 1)
+ward_chain_kernel(double* __restrict__ D, int n, int64_t ldd, int2* __restrict__ chain_all, int32_t* __restrict__ merge_xy,
+                  double* __restrict__ merge_dist, int* __restrict__ status) {
+    extern __shared__ int sz[];                            // cluster sizes of this CTA's columns, 0 = merged away
+    __shared__ Cand part[2];                               // this CTA's scan result, double-buffered across scans
+    __shared__ Cand wpart[NC_WARPS];
+    __shared__ int2 first_live;                            // (lowest live column of this CTA, its size) or (INT_MAX, 0)
+    cg::cluster_group cluster = cg::this_cluster();
+    const int cs = static_cast<int>(cluster.num_blocks()), rank = static_cast<int>(cluster.block_rank());
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int slice = (n + cs - 1) / cs;
+    const int lo = min(n, rank * slice), hi = min(n, lo + slice), cnt = hi - lo;
+    int2* chain = chain_all + static_cast<int64_t>(rank) * n;
+
+    for (int i = tid; i < cnt; i += NC_THREADS) sz[i] = 1;
+    int fl = 0;                                            // first possibly-live local column (only moves forward)
+    if (tid == 0) first_live = cnt > 0 ? make_int2(lo, 1) : make_int2(INT_MAX, 0);
+    cluster_sync_all();
+
+    int len = 0, par = 0;
+    int x = 0, xs = 0, p = -1, ps = 0;                     // chain top and the element below it
+#pragma unroll 1
+    for (int k = 0; k < n - 1; ++k) {
+        if (len == 0) {                                    // the chain restarts at the lowest live index
+            int2 f = make_int2(INT_MAX, 0);
+            if (lane < cs) f = *cluster.map_shared_rank(&first_live, lane);
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) {
+                const int oi = __shfl_xor_sync(0xffffffffu, f.x, o), os = __shfl_xor_sync(0xffffffffu, f.y, o);
+                if (oi < f.x) { f.x = oi; f.y = os; }
+            }
+            x = f.x; xs = f.y; p = -1; ps = 0;
+            if (tid == 0) chain[0] = f;
+            len = 1;
+        }
+        double cur;
+#pragma unroll 1
+        while (true) {
+            // ---- scan row x over this CTA's live columns -------------------------------------------------------
+            const double* row = D + static_cast<int64_t>(x) * ldd;
+            Cand c{CUDART_INF, INT_MAX, 0};
+            int i = lo + tid;
+#pragma unroll 1
+            for (; i + 3 * NC_THREADS < hi; i += 4 * NC_THREADS) {
+                double v[4];
+                bool live[4];
+#pragma unroll
+                for (int u = 0; u < 4; ++u) {
+                    const int j = i + u * NC_THREADS;
+                    live[u] = sz[j - lo] > 0 && j != x;
+                    v[u] = live[u] ? __ldcg(row + j) : CUDART_INF;
+                }
+#pragma unroll
+                for (int u = 0; u < 4; ++u)
+                    if (live[u] && v[u] < c.v) { c.v = v[u]; c.i = i + u * NC_THREADS; c.s = sz[i + u * NC_THREADS - lo]; }
+            }
+            for (; i < hi; i += NC_THREADS) {
+                const int s = sz[i - lo];
+                if (s > 0 && i != x) {
+                    const double v = __ldcg(row + i);
+                    if (v < c.v) { c.v = v; c.i = i; c.s = s; }
+                }
+            }
+            warp_cand_min(c);
+            if (lane == 0) wpart[warp] = c;
+            __syncthreads();
+            if (warp == 0) {
+                c = lane < NC_WARPS ? wpart[lane] : Cand{CUDART_INF, INT_MAX, 0};
+                warp_cand_min(c);
+                if (lane == 0) part[par] = c;
+            }
+            cluster_sync_all();                            // the scan's one cluster barrier
+            // ---- every warp resolves the same winner from the cs partial results (DSMEM) ----------------------
+            Cand m{CUDART_INF, INT_MAX, 0};
+            if (lane < cs) m = *cluster.map_shared_rank(&part[par], lane);
+            warp_cand_min(m);
+            par ^= 1;                                      // part[par] is rewritten only after one more barrier
+            cur = p >= 0 ? __ldcg(row + p) : CUDART_INF;   // scipy starts from D[x, prev]: ties go to prev
+            int y, ys;
+            if (m.v < cur) { y = m.i; ys = m.s; cur = m.v; }
+            else { y = p; ys = ps; }
+            if (p >= 0 && y == p) break;
+            if (y < 0 || y == INT_MAX) {                   // no finite candidate (non-finite input): give up uniformly
+                if (rank == 0 && tid == 0) *status = ALQ_ERR_NUMERIC;
+                cluster_sync_all();                        // no CTA exits while a peer still reads its part[] (DSMEM)
+                return;
+            }
+            if (tid == 0) chain[len] = make_int2(y, ys);
+            ++len;
+            p = x; ps = xs; x = y; xs = ys;
+        }
+        // ---- merge the mutual nearest neighbours x (top) and p -----------------------------------------------------
+        len -= 2;
+        const int a = min(x, p), b = max(x, p);            // fastcluster's convention: the new cluster keeps index b
+        const int na = a == x ? xs : ps, nb = a == x ? ps : xs;
+        if (rank == 0 && tid == 0) {
+            merge_xy[2 * static_cast<int64_t>(k)] = a;
+            merge_xy[2 * static_cast<int64_t>(k) + 1] = b;
+            merge_dist[k] = cur;
+        }
+        const double* rowa = D + static_cast<int64_t>(a) * ldd;
+        double* rowb = D + static_cast<int64_t>(b) * ldd;
+        for (int i = lo + tid; i < hi; i += NC_THREADS) {
+            const int ni = sz[i - lo];
+            if (ni > 0 && i != a && i != b) {
+                const double v = ward_update(__ldcg(rowa + i), __ldcg(rowb + i), cur, na, nb, ni);
+                __stcg(rowb + i, v);
+                __stcg(D + static_cast<int64_t>(i) * ldd + b, v);
+            }
+        }
+        __syncthreads();
+        if (tid == 0) {
+            if (a >= lo && a < hi) sz[a - lo] = 0;
+            if (b >= lo && b < hi) sz[b - lo] = na + nb;
+            while (fl < cnt && sz[fl] == 0) ++fl;
+            first_live = fl < cnt ? make_int2(lo + fl, sz[fl]) : make_int2(INT_MAX, 0);
+        }
+        if (len > 0) {                                     // the stack below the merged pair is unchanged; its entries
+            const int2 t = __ldcg(chain + len - 1);        // were written by this CTA's thread 0 before a __syncthreads
+            x = t.x; xs = t.y;
+            if (len > 1) { const int2 q = __ldcg(chain + len - 2); p = q.x; ps = q.y; }
+            else { p = -1; ps = 0; }
+        }
+        cluster_sync_all();                                // the merge's one cluster barrier
+    }
+}
+
+int ward_cluster_size(alq_ctx* ctx, size_t smem, int* out) {
+    ALQ_CUDA(ctx, cudaFuncSetAttribute(ward_chain_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    ALQ_CUDA(ctx, cudaFuncSetAttribute(ward_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+    for (int cs : {16, 8}) {
+        cudaLaunchConfig_t cfg = {};
+        cfg.gridDim = dim3(cs);
+        cfg.blockDim = dim3(NC_THREADS);
+        cfg.dynamicSmemBytes = smem;
+        cudaLaunchAttribute attr;
+        attr.id = cudaLaunchAttributeClusterDimension;
+        attr.val.clusterDim.x = cs;
+        attr.val.clusterDim.y = 1;
+        attr.val.clusterDim.z = 1;
+        cfg.attrs = &attr;
+        cfg.numAttrs = 1;
+        int nclusters = 0;
+        if (cudaOccupancyMaxActiveClusters(&nclusters, ward_chain_kernel, &cfg) == cudaSuccess && nclusters > 0) {
+            *out = cs;
+            return ALQ_OK;
+        }
+        (void)cudaGetLastError();
+    }
+    ALQ_FAIL(ctx, ALQ_ERR_CUDA, "alq_ward_nn_chain: no thread-block cluster of 8 or 16 CTAs fits this GPU");
+}
+
+// ---- host twins of scipy's label() and sklearn's _hc_cut ------------------------------------------------------
+struct LinkageUnionFind {                                  // scipy/cluster/_hierarchy.pyx
+    std::vector<int64_t> parent, size;
+    int64_t next_label;
+    explicit LinkageUnionFind(int64_t n) : parent(2 * n - 1), size(2 * n - 1, 1), next_label(n) {
+        std::iota(parent.begin(), parent.end(), 0);
+    }
+    int64_t merge(int64_t x, int64_t y) {
+        parent[x] = next_label;
+        parent[y] = next_label;
+        const int64_t s = size[x] + size[y];
+        size[next_label] = s;
+        ++next_label;
+        return s;
+    }
+    int64_t find(int64_t x) {
+        int64_t p = x;
+        while (parent[x] != x) x = parent[x];
+        while (parent[p] != x) { const int64_t q = parent[p]; parent[p] = x; p = q; }
+        return x;
+    }
+};
+
+// Python's heapq (_siftdown / _siftup), so that the final heap order -- which numbers sklearn's labels -- matches
+void heap_siftdown(std::vector<int64_t>& h, size_t start, size_t pos) {
+    const int64_t item = h[pos];
+    while (pos > start) {
+        const size_t parent = (pos - 1) >> 1;
+        if (item < h[parent]) { h[pos] = h[parent]; pos = parent; continue; }
+        break;
+    }
+    h[pos] = item;
+}
+void heap_siftup(std::vector<int64_t>& h, size_t pos) {
+    const size_t end = h.size(), start = pos;
+    const int64_t item = h[pos];
+    size_t child = 2 * pos + 1;
+    while (child < end) {
+        const size_t right = child + 1;
+        if (right < end && !(h[child] < h[right])) child = right;
+        h[pos] = h[child];
+        pos = child;
+        child = 2 * pos + 1;
+    }
+    h[pos] = item;
+    heap_siftdown(h, start, pos);
+}
+void heap_push(std::vector<int64_t>& h, int64_t item) {
+    h.push_back(item);
+    heap_siftdown(h, 0, h.size() - 1);
+}
+void heap_pushpop(std::vector<int64_t>& h, int64_t item) {
+    if (!h.empty() && h[0] < item) {
+        h[0] = item;
+        heap_siftup(h, 0);
+    }
+}
+
+}  // namespace ward
+
+using namespace ward;
+
+extern "C" int alq_pdist_f64(alq_ctx* ctx, const float* x, int64_t n, int32_t d, int64_t ldx, double* dist, int64_t ldd,
+                             void* stream) {
+    if (!ctx) return ALQ_ERR_INVALID;
+    if (!x || !dist || n < 1 || d < 1 || ldx < d || ldd < n)
+        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_pdist_f64: bad arguments (n=%lld d=%d ldx=%lld ldd=%lld)", (long long)n, d,
+                 (long long)ldx, (long long)ldd);
+    const int64_t nt = (n + PD_TILE - 1) / PD_TILE;
+    if (nt > 65535) ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_pdist_f64: n=%lld exceeds %d rows", (long long)n, 65535 * PD_TILE);
+    ALQ_CUDA(ctx, cudaSetDevice(ctx->device));
+    pdist_f64_kernel<<<dim3(static_cast<unsigned>(nt), static_cast<unsigned>(nt)), PD_THREADS, 0,
+                       static_cast<cudaStream_t>(stream)>>>(x, static_cast<int>(n), d, ldx, dist, ldd);
+    ALQ_LAUNCH_CHECK(ctx);
+    return ALQ_OK;
+}
+
+extern "C" int alq_ward_nn_chain(alq_ctx* ctx, double* dist, int64_t n, int64_t ldd, int32_t* merge_xy, double* merge_dist,
+                                 void* stream) {
+    if (!ctx) return ALQ_ERR_INVALID;
+    if (!dist || !merge_xy || !merge_dist || n < 2 || n >= (1LL << 31) - 1 || ldd < n)
+        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_ward_nn_chain: bad arguments (n=%lld ldd=%lld)", (long long)n, (long long)ldd);
+    ALQ_CUDA(ctx, cudaSetDevice(ctx->device));
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const size_t smem = static_cast<size_t>((n + 7) / 8) * sizeof(int) + 16;   // sized for the 8-CTA fallback
+    if (smem + 4096 > ctx->smem_optin)
+        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_ward_nn_chain: n=%lld does not fit the shared memory of a cluster", (long long)n);
+    int cs = 0;
+    int rc = ward_cluster_size(ctx, smem, &cs);
+    if (rc) return rc;
+    rc = alq_scratch_reserve(ctx, scratch_need({static_cast<size_t>(cs) * n * sizeof(int2), sizeof(int)}));
+    if (rc) return rc;
+    ScratchCursor cur(ctx->scratch);
+    int2* chain = cur.take<int2>(static_cast<size_t>(cs) * n);
+    int* status = cur.take<int>(1);
+    ALQ_CUDA(ctx, cudaMemsetAsync(status, 0, sizeof(int), st));
+
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(cs);
+    cfg.blockDim = dim3(NC_THREADS);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = st;
+    cudaLaunchAttribute attr;
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = cs;
+    attr.val.clusterDim.y = 1;
+    attr.val.clusterDim.z = 1;
+    cfg.attrs = &attr;
+    cfg.numAttrs = 1;
+    ALQ_CUDA(ctx, cudaLaunchKernelEx(&cfg, ward_chain_kernel, dist, static_cast<int>(n), ldd, chain, merge_xy, merge_dist, status));
+    ALQ_LAUNCH_CHECK(ctx);
+    int h_status = 0;
+    ALQ_CUDA(ctx, cudaMemcpyAsync(&h_status, status, sizeof(int), cudaMemcpyDeviceToHost, st));
+    ALQ_CUDA(ctx, cudaStreamSynchronize(st));
+    if (h_status) ALQ_FAIL(ctx, ALQ_ERR_NUMERIC, "alq_ward_nn_chain: a chain scan found no finite distance (non-finite input)");
+    return ALQ_OK;
+}
+
+extern "C" int alq_ward_labels(const int32_t* merge_xy_host, const double* merge_dist_host, int64_t n, int32_t n_clusters,
+                               int32_t* labels_host) {
+    if (!merge_xy_host || !merge_dist_host || !labels_host || n < 2 || n >= (1LL << 31) || n_clusters < 1 || n_clusters > n)
+        return ALQ_ERR_INVALID;
+    const int64_t m = n - 1;
+    for (int64_t k = 0; k < m; ++k) {
+        const int64_t a = merge_xy_host[2 * k], b = merge_xy_host[2 * k + 1];
+        if (a < 0 || b < 0 || a >= n || b >= n || a == b || std::isnan(merge_dist_host[k])) return ALQ_ERR_INVALID;
+    }
+    // scipy's nn_chain epilogue: stable sort by distance (np.argsort kind='mergesort'), then label() by union-find
+    std::vector<int64_t> order(m);
+    std::iota(order.begin(), order.end(), 0);
+    std::stable_sort(order.begin(), order.end(),
+                     [&](int64_t u, int64_t v) { return merge_dist_host[u] < merge_dist_host[v]; });
+    LinkageUnionFind uf(n);
+    std::vector<int64_t> children(2 * m);
+    for (int64_t r = 0; r < m; ++r) {
+        const int64_t k = order[r];
+        const int64_t xr = uf.find(merge_xy_host[2 * k]), yr = uf.find(merge_xy_host[2 * k + 1]);
+        // the n - 1 pairs, taken as edges, must form a spanning tree (in any order: no edge closes a cycle), which is
+        // what makes every leaf end up under the root and labelled
+        if (xr == yr) return ALQ_ERR_INVALID;
+        children[2 * r] = std::min(xr, yr);
+        children[2 * r + 1] = std::max(xr, yr);
+        uf.merge(xr, yr);
+    }
+    // sklearn's _hc_cut: a heap of negated node ids, labels numbered in the heap's final order
+    std::vector<int64_t> nodes{-(std::max(children[2 * (m - 1)], children[2 * (m - 1) + 1]) + 1)};
+    for (int32_t t = 0; t < n_clusters - 1; ++t) {
+        const int64_t node = -nodes[0] - n;
+        heap_push(nodes, -children[2 * node]);
+        heap_pushpop(nodes, -children[2 * node + 1]);
+    }
+    std::vector<int64_t> stack;
+    for (size_t l = 0; l < nodes.size(); ++l) {
+        stack.assign(1, -nodes[l]);
+        while (!stack.empty()) {
+            const int64_t v = stack.back();
+            stack.pop_back();
+            if (v < n) { labels_host[v] = static_cast<int32_t>(l); continue; }
+            stack.push_back(children[2 * (v - n)]);
+            stack.push_back(children[2 * (v - n) + 1]);
+        }
+    }
+    return ALQ_OK;
+}

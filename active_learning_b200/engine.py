@@ -35,6 +35,24 @@ def _ld(t: torch.Tensor) -> int:
     return t.stride(0) if t.dim() == 2 and t.shape[0] > 1 else t.shape[-1]
 
 
+def ward_labels_host(merge_xy: np.ndarray, merge_dist: np.ndarray, n: int, n_clusters: int) -> np.ndarray:
+    """alq_ward_labels (host-only, no GPU): K8's discovery-order merge list -> sklearn's labels for n_clusters (int64)."""
+    lib = _lib.load()
+    xy = np.ascontiguousarray(merge_xy, dtype=np.int32).reshape(-1, 2)
+    md = np.ascontiguousarray(merge_dist, dtype=np.float64).reshape(-1)
+    n = int(n)
+    if xy.shape[0] != n - 1 or md.shape[0] != n - 1:
+        raise AlqError(f"ward labels: need {n - 1} merges for {n} rows, got {xy.shape[0]} / {md.shape[0]}")
+    if int(n_clusters) > n:
+        raise ValueError(f"cannot extract {n_clusters} clusters from a tree with {n} leaves")
+    out = np.empty(n, dtype=np.int32)
+    rc = lib.alq_ward_labels(C.c_void_p(xy.ctypes.data), C.c_void_p(md.ctypes.data), n, int(n_clusters),
+                             C.c_void_p(out.ctypes.data))
+    if rc != 0:
+        raise AlqError(f"alq_ward_labels(n={n}, n_clusters={n_clusters}) failed with {_lib.ERR_NAMES.get(rc, rc)}")
+    return out.astype(np.int64)
+
+
 class Engine:
     """One libalq context bound to one CUDA device."""
 
@@ -301,6 +319,82 @@ class Engine:
         self._check(self.lib.alq_base_select(self._h, _ptr(min_margin), _ptr(radius), _ld(radius), _ptr(pred.contiguous()),
                                              n, c, int(budget), _ptr(out), self._stream()), "alq_base_select")
         return out
+
+    # -- K7 / K8: Ward clustering (MarginClusteringSampler) ---------------------------------------------
+    WARD_HEADROOM_BYTES = 1 << 30     # the chain scratch, the merge list and whatever else the query holds
+
+    def pdist(self, x: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """K7: the n x n fp64 matrix of scipy's pdist(x, 'euclidean') (bit for bit; diagonal 0)."""
+        x = _f32c(x, "x")
+        n, d = x.shape
+        if out is None:
+            out = torch.empty((n, n), dtype=torch.float64, device=x.device)
+        if out.dtype != torch.float64 or out.dim() != 2 or out.shape[0] < n or out.shape[1] < n or out.stride(1) != 1:
+            raise AlqError("pdist: out must be a row-major float64 CUDA tensor of at least n x n")
+        self._check(self.lib.alq_pdist_f64(self._h, _ptr(x), n, d, _ld(x), _ptr(out), out.stride(0), self._stream()),
+                    "alq_pdist_f64")
+        return out
+
+    def nn_chain(self, dist: torch.Tensor, n: Optional[int] = None):
+        """K8: scipy's Ward nn_chain over `dist` (consumed).  (merge_xy [n-1, 2] int32 with x < y, merge_dist [n-1]
+        fp64) on the device, in the chain's discovery order.  `dist` is a row-major float64 CUDA matrix of at least
+        n x n (n defaults to its row count).  Synchronous; AlqError (ALQ_ERR_NUMERIC) if a scan meets no finite
+        distance."""
+        if not dist.is_cuda or dist.dtype != torch.float64 or dist.dim() != 2 or dist.stride(1) != 1:
+            raise AlqError("nn_chain: dist must be a row-major float64 CUDA matrix")
+        n = dist.shape[0] if n is None else int(n)
+        if n < 2 or dist.shape[0] < n or dist.shape[1] < n or dist.stride(0) < n:
+            raise AlqError(f"nn_chain: need n >= 2 and a matrix of at least n x n, got n={n} for {tuple(dist.shape)} "
+                           f"with row stride {dist.stride(0)}")
+        xy = torch.empty((max(n - 1, 1), 2), dtype=torch.int32, device=dist.device)
+        md = torch.empty(max(n - 1, 1), dtype=torch.float64, device=dist.device)
+        self._check(self.lib.alq_ward_nn_chain(self._h, _ptr(dist), n, dist.stride(0), _ptr(xy), _ptr(md), self._stream()),
+                    "alq_ward_nn_chain")
+        return xy[:n - 1], md[:n - 1]
+
+    def ward_bytes(self, n: int) -> int:
+        """Device memory a Ward tree over n rows needs: the 8 n^2 distance matrix plus headroom."""
+        return 8 * int(n) * int(n) + self.WARD_HEADROOM_BYTES
+
+    def _ward_guard(self, n: int):
+        free, _total = torch.cuda.mem_get_info(self.device)
+        cached = torch.cuda.memory_reserved(self.device) - torch.cuda.memory_allocated(self.device)
+        need = self.ward_bytes(n)
+        if need > free + cached:
+            raise AlqError(f"ward: n={n} rows need {need} bytes of device memory (8 * n^2 for the distance matrix plus "
+                           f"{self.WARD_HEADROOM_BYTES} headroom), {free + cached} are free; use a smaller subset_unlabeled")
+
+    def ward_tree(self, x: torch.Tensor):
+        """scipy.cluster.hierarchy.ward(x)'s merges before its sort: (merge_xy [n-1, 2] int32, merge_dist [n-1] fp64) as
+        host arrays, in discovery order.  Checks the device memory first and never attempts an allocation that cannot
+        fit; there is no CPU fallback.  ValueError for fewer than 2 rows or non-finite rows.  The 8 n^2 matrix is
+        returned to the device before this returns (torch.cuda.empty_cache, which also releases the process's other
+        unused cached blocks): at 80 000 rows it is 51.2 GB that the caching allocator would otherwise keep."""
+        x = _f32c(x, "x")
+        n = x.shape[0]
+        if n < 2:
+            raise ValueError(f"ward needs at least 2 rows, got {n}")
+        self._ward_guard(n)
+        if not bool(torch.isfinite(x).all()):
+            raise ValueError("ward: the embeddings contain NaN or infinity")
+        dist = self.pdist(x)
+        try:
+            xy, md = self.nn_chain(dist, n)
+            xy, md = xy.cpu().numpy(), md.cpu().numpy()
+        finally:
+            del dist
+            torch.cuda.empty_cache()
+        return xy, md
+
+    def ward_labels(self, x: torch.Tensor, n_clusters: int) -> np.ndarray:
+        """labels_ of sklearn's AgglomerativeClustering(n_clusters).fit(x) (Ward linkage, full tree), identical, as a host
+        int64 array.  ValueError for fewer rows than clusters or non-finite rows, as sklearn raises."""
+        x = _f32c(x, "x")
+        n = x.shape[0]
+        if n < max(2, int(n_clusters)):
+            raise ValueError(f"cannot extract {n_clusters} clusters from {n} rows")
+        xy, md = self.ward_tree(x)
+        return ward_labels_host(xy, md, n, n_clusters)
 
     # -- K4 / K5 ---------------------------------------------------------------------------------------
     def leaf_bounds(self, n: int) -> np.ndarray:

@@ -16,6 +16,7 @@ from __future__ import annotations
 from .query_strategies.coreset import (BADGEQuery, CoresetQuery, PartitionedBADGEQuery,
                                        PartitionedCoresetQuery)
 from .query_strategies.balancing import BalancingQuery
+from .query_strategies.margin_clustering import MarginClusteringQuery
 from .query_strategies.mase import BASEQuery, MASEQuery
 from .query_strategies.uncertainty import ConfidenceQuery, EntropyQuery, MarginQuery
 
@@ -30,6 +31,7 @@ _MIXINS = {
     "MASESampler": MASEQuery,
     "BASESampler": BASEQuery,
     "BalancingSampler": BalancingQuery,
+    "MarginClusteringSampler": MarginClusteringQuery,
 }
 
 

@@ -1,6 +1,6 @@
 """`--strategy` dispatch, same contract as active_learning/src/query_strategies/get_strategy.py:
-`get_strategy(name)` returns the class called `name`.  The ten accelerated samplers (the seven of the
-north-star path plus MASE / BASE / Balancing, SURVEY.md section 8f) and the default RandomSampler are implemented; the reference's remaining class names resolve to a
+`get_strategy(name)` returns the class called `name`.  The eleven accelerated samplers (the seven of the
+north-star path plus MASE / BASE / Balancing, SURVEY.md section 8f, and MarginClustering) and the default RandomSampler are implemented; the reference's remaining class names resolve to a
 stub that raises a clear error (SURVEY.md section 8: out of scope for this path)."""
 from .badge_sampler import BADGESampler  # noqa: F401
 from .balancing_sampler import BalancingSampler  # noqa: F401
@@ -8,6 +8,7 @@ from .base_sampler import BASESampler  # noqa: F401
 from .confidence_sampler import ConfidenceSampler  # noqa: F401
 from .coreset_sampler import CoresetSampler  # noqa: F401
 from .entropy_sampler import EntropySampler  # noqa: F401
+from .margin_clustering_sampler import MarginClusteringSampler  # noqa: F401
 from .margin_sampler import MarginSampler  # noqa: F401
 from .mase_sampler import MASESampler  # noqa: F401
 from .partitioned_badge_sampler import PartitionedBADGESampler  # noqa: F401
@@ -16,8 +17,8 @@ from .random_sampler import RandomSampler  # noqa: F401
 
 ACCELERATED = ("MarginSampler", "ConfidenceSampler", "EntropySampler", "CoresetSampler",
                "PartitionedCoresetSampler", "BADGESampler", "PartitionedBADGESampler", "MASESampler", "BASESampler",
-               "BalancingSampler")
-NOT_ON_THIS_PATH = ("BalancedRandomSampler", "MarginClusteringSampler", "VAALSampler")
+               "BalancingSampler", "MarginClusteringSampler")
+NOT_ON_THIS_PATH = ("BalancedRandomSampler", "VAALSampler")
 
 
 def _out_of_scope(name):

@@ -1,0 +1,81 @@
+"""Margin clustering acquisition on the device (kernels K1, K7, K8): margin_clustering_sampler.py:47-90 of
+active_learning/src/query_strategies (https://arxiv.org/abs/2107.14263).
+
+The reference clusters the pool embeddings with sklearn's AgglomerativeClustering(n_clusters=20) -- Ward linkage over
+the full tree: scipy's single-threaded pdist (a 25.6 GB condensed matrix at 80 000 rows) and nn_chain on the host --
+then picks round-robin over the clusters, smallest cluster first, the smallest-margin row left in each.  Here one
+pool forward yields logits and embeddings, K1 scores the margins, K7 builds the fp64 distance matrix in HBM and K8
+walks the nearest-neighbour chain in one launch; the merge tree is scipy's bit for bit, so the labels are sklearn's
+(include/alq.h).  The round robin is O(n log n) host NumPy over n margins.
+"""
+from __future__ import annotations
+
+import numpy as np
+
+from .._lib import MODE_MARGIN, AlqError
+from .strategy import EngineMixin
+
+N_CLUSTERS = 20     # margin_clustering_sampler.py:59
+
+
+def round_robin(assignment: np.ndarray, margins: np.ndarray, budget: int):
+    """The pick loop of margin_clustering_sampler.py:64-89: clusters visited by (size, id); pass k takes the k-th row of
+    every cluster larger than k, rows of a cluster ordered by (margin, position); stop after `budget` picks.
+    Returns (positions in pick order, the assignment of the rows not picked, in pool order)."""
+    assignment = np.asarray(assignment)
+    margins = np.asarray(margins, dtype=np.float32)
+    if assignment.shape[0] != margins.shape[0]:
+        raise ValueError(f"cluster assignment has {assignment.shape[0]} rows, the pool has {margins.shape[0]}")
+    n = assignment.shape[0]
+    budget = int(min(n, budget))
+    if budget <= 0:
+        return np.empty(0, dtype=np.int64), assignment.copy()
+    ids, inv, counts = np.unique(assignment, return_inverse=True, return_counts=True)
+    visit = np.lexsort((ids, counts))                   # cluster visiting order: (count, id)
+    visit_rank = np.empty(len(ids), dtype=np.int64)
+    visit_rank[visit] = np.arange(len(ids))
+    # rank of each row inside its cluster by (margin, position): order rows by (cluster, margin, position)
+    by = np.lexsort((np.arange(n), margins, inv))
+    first = np.zeros(len(ids), dtype=np.int64)
+    first[1:] = np.cumsum(counts)[:-1]
+    rank_in = np.empty(n, dtype=np.int64)
+    rank_in[by] = np.arange(n) - first[inv[by]]
+    key = rank_in * len(ids) + visit_rank[inv]
+    picks = np.argsort(key, kind="stable")[:budget]
+    keep = np.ones(n, dtype=bool)
+    keep[picks] = False
+    return picks.astype(np.int64), assignment[keep]
+
+
+class MarginClusteringQuery(EngineMixin):
+    def __init__(self, *args, **kwargs):
+        super().__init__(*args, **kwargs)
+        self.saved_pairwise_l2_dist = None
+        self.freeze_feature = kwargs["freeze_feature"]
+        self.subset_labeled = kwargs["subset_labeled"]
+        self.subset_unlabeled = kwargs["subset_unlabeled"]
+        self.cluster_assignment = None
+
+    # ---- margin_clustering_sampler.py:47-90 --------------------------------------------------------------
+    def query(self, budget):
+        group = getattr(self, "_shard_group", None)
+        if group is not None and group.world_size > 1:
+            raise AlqError("MarginClusteringSampler runs on one GPU: the nearest-neighbour chain of Ward clustering is "
+                           "sequential over the whole pool; query it from a single rank")
+        if self.subset_unlabeled is None:
+            idxs_for_hac = self.available_query_idxs(boolean=False, shuffle=False)
+        else:
+            idxs_for_hac = sorted(self.available_query_idxs(boolean=False, shuffle=True)[:self.subset_unlabeled])
+        eng = self.get_engine()
+        self.feature_net.eval()
+        logits, emb = self._forward_pool(idxs_for_hac, self.feature_net, want_features=True)
+        margins = eng.score_softmax(logits, MODE_MARGIN).cpu().numpy()
+        if self.cluster_assignment is None or self.subset_unlabeled:
+            # cluster in the first round, or every round when a random subset is drawn (:56-59)
+            cluster_assignment = eng.ward_labels(emb, N_CLUSTERS)
+        else:
+            cluster_assignment = self.cluster_assignment
+        budget = int(min(len(idxs_for_hac), budget))
+        picks, self.cluster_assignment = round_robin(cluster_assignment, margins, budget)
+        query_idxs = list(np.asarray(idxs_for_hac, dtype=np.int64)[picks])
+        return query_idxs, budget

@@ -8,8 +8,9 @@
  *   - `stream` is a cudaStream_t passed as void* (NULL = the legacy default stream); calls are
  *     asynchronous on it unless stated otherwise.
  *   - Return value: ALQ_OK (0) or an ALQ_ERR_* code; `alq_last_error(ctx)` describes the failure.
- *   - All arithmetic is IEEE fp32 (fp64 only for the inverse-CDF search); index math is int32 on
- *     the device (n < 2^31).  There is no CPU fallback anywhere in this library.
+ *   - All arithmetic is IEEE fp32 (fp64 only for the inverse-CDF search and the Ward clustering, K7/K8); index
+ *     math is int32 on the device (n < 2^31), except the int64 offsets into K7/K8's n x n matrix.  There is no
+ *     CPU fallback anywhere in this library.
  *   - Matrices are row-major with an explicit leading dimension (`ld*`, in elements).  The fast
  *     paths need the base pointer 16-byte aligned and ld % 4 == 0.
  */
@@ -285,6 +286,35 @@ int alq_mase_margins(alq_ctx* ctx, const float* logits, int64_t n, int32_t c, in
  * ALQ_ERR_NUMERIC if a row would be selected twice -- the condition the reference asserts on (:40).          */
 int alq_base_select(alq_ctx* ctx, const float* min_margin, const float* radius, int64_t ldr, const int32_t* pred,
                     int64_t n, int32_t c, int64_t budget, int32_t* out_pos, void* stream);
+
+/* ---- K7 / K8: Ward agglomerative clustering (MarginClusteringSampler) -----------------------------------------------
+ * margin_clustering_sampler.py:59 clusters the pool embeddings with sklearn's AgglomerativeClustering(n_clusters=20),
+ * i.e. scipy.cluster.hierarchy.ward(X): pdist + nn_chain over the full tree + sklearn's _hc_cut.  The three calls
+ * below reproduce that tree bit for bit, so the labels are sklearn's.
+ *
+ * alq_pdist_f64 (K7): dist[i, j] (row-major, leading dimension ldd >= n) = scipy's pdist(X, 'euclidean') of the fp32
+ *   rows x[i], x[j] in fp64: s summed over k = 0, 1, ... as `d = x[i,k] - x[j,k]; s = s + d*d` (no FMA), dist = sqrt(s).
+ *   Every pair is computed once and written to (i, j) and (j, i); the diagonal holds 0.0 (K8 never reads it).  Zero
+ *   pad columns (the 16-byte row padding of the pool-forward slab) leave every sum unchanged, so d may include them.
+ *   Any ldx >= d and any alignment.  n <= 65535 * 64.  The caller owns `dist` (8 * n * ldd bytes: 51.2 GB at
+ *   n = 80 000), so the caller frees it when the query ends (Engine.ward_tree hands it back to the device) and it
+ *   never sits in the grow-only arena.  Offsets into `dist` are
+ *   int64 -- the one exception to the int32 index rule above (n^2 passes 2^31 at n = 46 341).
+ * alq_ward_nn_chain (K8): scipy's nn_chain with the Ward update, in ONE launch of one thread-block cluster, consuming
+ *   `dist` in place (its contents are unspecified afterwards).  merge_xy[k] = (x, y) with x < y and merge_dist[k], for
+ *   k < n - 1, in the chain's discovery order (before scipy's sort).  n >= 2.  Synchronous; ALQ_ERR_NUMERIC if a scan
+ *   found no finite distance (non-finite input).
+ * alq_ward_labels: host-only, needs no GPU.  From K8's merge list: the stable sort by distance and scipy's union-find
+ *   relabelling (hierarchy.ward's Z), then sklearn's _hc_cut(n_clusters): labels_host[0..n) in [0, n_clusters),
+ *   numbered in the order of the cut's final heap.  ALQ_ERR_INVALID if n_clusters > n, or if the list is not a merge
+ *   tree: an index out of range, x == y, a NaN distance, or a pair whose clusters were already joined (the n - 1
+ *   pairs must form a spanning tree of the n rows), so that every label is written on success.                   */
+int alq_pdist_f64(alq_ctx* ctx, const float* x, int64_t n, int32_t d, int64_t ldx, double* dist, int64_t ldd,
+                  void* stream);
+int alq_ward_nn_chain(alq_ctx* ctx, double* dist, int64_t n, int64_t ldd, int32_t* merge_xy, double* merge_dist,
+                      void* stream);
+int alq_ward_labels(const int32_t* merge_xy_host, const double* merge_dist_host, int64_t n, int32_t n_clusters,
+                    int32_t* labels_host);
 
 #ifdef __cplusplus
 }
