@@ -16,7 +16,7 @@ ALQ_OK = 0
 ERR_NAMES = {1: "ALQ_ERR_INVALID", 2: "ALQ_ERR_CUDA", 3: "ALQ_ERR_NOMEM", 4: "ALQ_ERR_STATE",
              5: "ALQ_ERR_NUMERIC"}
 MODE_MARGIN, MODE_LEAST_CONFIDENCE, MODE_ENTROPY = 0, 1, 2
-ABI_VERSION = 6
+ABI_VERSION = 7
 
 c_f32p = C.c_void_p
 c_i32p = C.c_void_p
@@ -98,6 +98,8 @@ SIGNATURES = {
     "alq_pdist_f64": (C.c_int, [C.c_void_p, c_f32p, C.c_int64, C.c_int32, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p]),
     "alq_ward_nn_chain": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, c_i32p, C.c_void_p, C.c_void_p]),
     "alq_ward_labels": (C.c_int, [c_i32p, C.c_void_p, C.c_int64, C.c_int32, c_i32p]),
+    "alq_vaal_scores": (C.c_int, [C.c_void_p, c_f32p, C.c_int64, C.c_int32, C.c_int64, c_f32p, C.c_int64, c_f32p,
+                                  c_f32p, C.c_int64, c_f32p, c_f32p, c_f32p, C.c_int32, c_f32p, c_f32p, C.c_void_p]),
 }
 
 

@@ -19,17 +19,14 @@
 //                 (<h,h'> and <a,a'>) and multiplies them in the epilogue.
 // Every CTA sweeps the column tiles in the same order, so a Y tile is fetched from HBM once and
 // served to the other CTAs from L2.
-#include <cuda.h>
 #include <stdlib.h>
 
-#include "alq_common.cuh"
+#include "alq_wgmma.cuh"
 
 namespace tc {
 
 constexpr int BM = 128;          // rows per tile (two m64 warpgroups)
 constexpr int BN = 128;          // cols per tile (wgmma N)
-constexpr int BK = 32;           // fp32 per stage row = 128 bytes = one swizzle span
-constexpr int UK = 8;            // wgmma K for tf32
 constexpr int STAGES = 3;
 constexpr int A_BYTES = BM * BK * 4;              // 16 KB
 constexpr int B_BYTES = BN * BK * 4;              // 16 KB
@@ -49,47 +46,6 @@ struct Params {
     int n, m;                              // rows of X / Y
     int kblocks_h, kblocks_a;              // ceil(d / 32), ceil(c / 32) (0 when dense)
 };
-
-__device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
-}
-
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (PTX ISA, "Matrix Descriptor Format" of wgmma):
-//   bits [0,14) start address >> 4, [16,30) leading byte offset >> 4 (= 1, unused for swizzled K-major),
-//   [32,46) stride byte offset >> 4 (= 1024 B: 8 rows x 128 B), [62,64) swizzle mode = 1 (128 B).
-__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3fff);
-    d |= static_cast<uint64_t>(1) << 16;
-    d |= static_cast<uint64_t>(1024 >> 4) << 32;
-    d |= static_cast<uint64_t>(1) << 62;
-    return d;
-}
-__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
-// d (64 x 128 fp32, the m64n128 register fragment) += A (64 x 8, smem) * B (128 x 8, smem)^T;  scale_d == 0 overwrites d
-__device__ __forceinline__ void wgmma_tf32(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %66, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1;\n\t"
-        "}\n"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-        : "l"(adesc), "l"(bdesc), "r"(scale_d));
-}
 
 template <bool FACTORED, bool RED_MAX>
 __global__ void __launch_bounds__(THREADS, 1)
@@ -224,7 +180,7 @@ min_dist_tc_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_cons
     }
 }
 
-// hi = rna_tf32(x), lo = rna_tf32(x - hi): two valid TF32 operands whose sum is x to 2^-22 relative
+// every row of x as its TF32 hi/lo pair (split_tf32)
 __global__ void __launch_bounds__(256)
 split_tf32_kernel(const float* __restrict__ x, int64_t rows, int d, int64_t ld, float* __restrict__ hi,
                   float* __restrict__ lo) {
@@ -238,13 +194,7 @@ split_tf32_kernel(const float* __restrict__ x, int64_t rows, int d, int64_t ld, 
         const float e[4] = {v.x, v.y, v.z, v.w};
         float h[4], l[4];
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            uint32_t hb, lb;
-            asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hb) : "f"(e[j]));
-            h[j] = __uint_as_float(hb);
-            asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(lb) : "f"(e[j] - h[j]));
-            l[j] = __uint_as_float(lb);
-        }
+        for (int j = 0; j < 4; ++j) split_tf32(e[j], h[j], l[j]);
         reinterpret_cast<float4*>(hi + r * d)[k] = make_float4(h[0], h[1], h[2], h[3]);
         reinterpret_cast<float4*>(lo + r * d)[k] = make_float4(l[0], l[1], l[2], l[3]);
     }
@@ -257,35 +207,6 @@ __global__ void mul_norms_kernel(const float* a, const float* b, float* o, int64
 __global__ void fill_kernel(float* p, int64_t n, float v) {
     const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
     if (i < n) p[i] = v;
-}
-
-using EncodeFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                              const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                              CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeFn get_encode() {
-    static EncodeFn fn = nullptr;
-    if (!fn) {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-            q == cudaDriverEntryPointSuccess)
-            fn = reinterpret_cast<EncodeFn>(p);
-    }
-    return fn;
-}
-
-// 2-D fp32 [rows, cols] row-major (contiguous: pitch == cols), box = [32 cols, box_rows], 128-byte swizzle
-bool make_map(CUtensorMap* map, const float* base, int64_t rows, int cols, int box_rows) {
-    EncodeFn enc = get_encode();
-    if (!enc) return false;
-    cuuint64_t dims[2] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows)};
-    cuuint64_t strides[1] = {static_cast<cuuint64_t>(cols) * 4};
-    cuuint32_t box[2] = {static_cast<cuuint32_t>(BK), static_cast<cuuint32_t>(box_rows)};
-    cuuint32_t estr[2] = {1, 1};
-    return enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, estr,
-               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
 }  // namespace tc

@@ -396,6 +396,57 @@ class Engine:
         xy, md = self.ward_tree(x)
         return ward_labels_host(xy, md, n, n_clusters)
 
+    # -- K9: the VAAL discriminator (VAALSampler) ----------------------------------------------------------
+    VAAL_HIDDEN = 512
+
+    @classmethod
+    def vaal_layers(cls, discriminator):
+        """The three Linear layers of the reference's Discriminator (vaal_discriminator.py): `discriminator.net` (or the
+        module itself) must be Sequential(Linear(z, 512), ReLU, Linear(512, 512), ReLU, Linear(512, 1), Sigmoid), with
+        biases.  AlqError for any other layout: K9 computes exactly this network and nothing else."""
+        import torch.nn as nn
+        seq = getattr(discriminator, "net", discriminator)
+        kinds = (nn.Linear, nn.ReLU, nn.Linear, nn.ReLU, nn.Linear, nn.Sigmoid)
+        h = cls.VAAL_HIDDEN
+        if not isinstance(seq, nn.Sequential) or len(seq) != len(kinds) or any(type(m) is not k for m, k in zip(seq, kinds)):
+            raise AlqError("vaal_scores: the discriminator must be the reference's Sequential(Linear(z, 512), ReLU, "
+                           "Linear(512, 512), ReLU, Linear(512, 1), Sigmoid)")
+        l1, l2, l3 = seq[0], seq[2], seq[4]
+        shapes = [(l1.out_features, h), (l2.in_features, h), (l2.out_features, h), (l3.in_features, h), (l3.out_features, 1)]
+        if any(a != b for a, b in shapes) or any(lin.bias is None for lin in (l1, l2, l3)):
+            raise AlqError(f"vaal_scores: the discriminator's Linear layers must be z -> {h} -> {h} -> 1 with biases")
+        return l1, l2, l3
+
+    def vaal_scores(self, mu: torch.Tensor, discriminator, return_logits: bool = False):
+        """K9: p[i] = discriminator(mu[i, :z]) for the reference's Discriminator (vaal_layers), as a CUDA float32 vector
+        (and the pre-sigmoid logits with return_logits).  `mu` is a CUDA float32 [n, >= z] matrix; rows whose leading
+        dimension or base address does not suit the tensor-memory loads are copied into a padded slab first."""
+        l1, l2, l3 = self.vaal_layers(discriminator)
+        mu = _f32c(mu, "mu")
+        z = l1.in_features
+        if mu.dim() != 2 or mu.shape[1] < z:
+            raise AlqError(f"vaal_scores: mu must be [n, >= {z}], got {tuple(mu.shape)}")
+        n, zp, dev = mu.shape[0], (z + 3) & ~3, mu.device
+        ld = _ld(mu)
+        if n and (ld % 4 or mu.data_ptr() % 16):
+            slab = torch.zeros((n, zp), dtype=torch.float32, device=dev)
+            slab[:, :z] = mu[:, :z]
+            mu, ld = slab, zp
+
+        def dev32(t):
+            return t.detach().to(device=dev, dtype=torch.float32).contiguous()
+
+        w1 = torch.zeros((self.VAAL_HIDDEN, zp), dtype=torch.float32, device=dev)
+        w1[:, :z] = dev32(l1.weight)
+        b1, w2, b2 = dev32(l1.bias), dev32(l2.weight), dev32(l2.bias)
+        w3, b3 = dev32(l3.weight).reshape(-1), dev32(l3.bias).reshape(-1)
+        p = torch.empty(n, dtype=torch.float32, device=dev)
+        logits = torch.empty(n, dtype=torch.float32, device=dev) if return_logits else None
+        self._check(self.lib.alq_vaal_scores(self._h, _ptr(mu), n, z, ld, _ptr(w1), zp, _ptr(b1), _ptr(w2), w2.shape[1],
+                                             _ptr(b2), _ptr(w3), _ptr(b3), self.VAAL_HIDDEN, _ptr(p), _ptr(logits),
+                                             self._stream()), "alq_vaal_scores")
+        return (p, logits) if return_logits else p
+
     # -- K4 / K5 ---------------------------------------------------------------------------------------
     def leaf_bounds(self, n: int) -> np.ndarray:
         """Leaf boundaries of NumPy's float32 pairwise summation over n entries (host helper of the library)."""

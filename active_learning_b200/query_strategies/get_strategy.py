@@ -1,7 +1,8 @@
 """`--strategy` dispatch, same contract as active_learning/src/query_strategies/get_strategy.py:
-`get_strategy(name)` returns the class called `name`.  The eleven accelerated samplers (the seven of the
-north-star path plus MASE / BASE / Balancing, SURVEY.md section 8f, and MarginClustering) and the default RandomSampler are implemented; the reference's remaining class names resolve to a
-stub that raises a clear error (SURVEY.md section 8: out of scope for this path)."""
+`get_strategy(name)` returns the class called `name`.  The twelve accelerated samplers (the seven of the
+north-star path plus MASE / BASE / Balancing, SURVEY.md section 8f, MarginClustering and VAAL) and the default RandomSampler
+are implemented; the reference's remaining class name resolves to a stub that raises a clear error (SURVEY.md section 8:
+out of scope for this path)."""
 from .badge_sampler import BADGESampler  # noqa: F401
 from .balancing_sampler import BalancingSampler  # noqa: F401
 from .base_sampler import BASESampler  # noqa: F401
@@ -14,11 +15,12 @@ from .mase_sampler import MASESampler  # noqa: F401
 from .partitioned_badge_sampler import PartitionedBADGESampler  # noqa: F401
 from .partitioned_coreset_sampler import PartitionedCoresetSampler  # noqa: F401
 from .random_sampler import RandomSampler  # noqa: F401
+from .vaal_sampler import VAALSampler  # noqa: F401
 
 ACCELERATED = ("MarginSampler", "ConfidenceSampler", "EntropySampler", "CoresetSampler",
                "PartitionedCoresetSampler", "BADGESampler", "PartitionedBADGESampler", "MASESampler", "BASESampler",
-               "BalancingSampler", "MarginClusteringSampler")
-NOT_ON_THIS_PATH = ("BalancedRandomSampler", "VAALSampler")
+               "BalancingSampler", "MarginClusteringSampler", "VAALSampler")
+NOT_ON_THIS_PATH = ("BalancedRandomSampler",)
 
 
 def _out_of_scope(name):

@@ -8,9 +8,9 @@
  *   - `stream` is a cudaStream_t passed as void* (NULL = the legacy default stream); calls are
  *     asynchronous on it unless stated otherwise.
  *   - Return value: ALQ_OK (0) or an ALQ_ERR_* code; `alq_last_error(ctx)` describes the failure.
- *   - All arithmetic is IEEE fp32 (fp64 only for the inverse-CDF search and the Ward clustering, K7/K8); index
- *     math is int32 on the device (n < 2^31), except the int64 offsets into K7/K8's n x n matrix.  There is no
- *     CPU fallback anywhere in this library.
+ *   - All arithmetic is IEEE fp32 (fp64 only for the inverse-CDF search and the Ward clustering, K7/K8; K3 and K9
+ *     contract on the tensor cores as 3xTF32, fp32 to about 2^-21 per product); index math is int32 on the device
+ *     (n < 2^31), except the int64 offsets into K7/K8's n x n matrix.  There is no CPU fallback anywhere in this library.
  *   - Matrices are row-major with an explicit leading dimension (`ld*`, in elements).  The fast
  *     paths need the base pointer 16-byte aligned and ld % 4 == 0.
  */
@@ -315,6 +315,20 @@ int alq_ward_nn_chain(alq_ctx* ctx, double* dist, int64_t n, int64_t ldd, int32_
                       void* stream);
 int alq_ward_labels(const int32_t* merge_xy_host, const double* merge_dist_host, int64_t n, int32_t n_clusters,
                     int32_t* labels_host);
+
+/* ---- K9: the VAAL discriminator (VAALSampler) ---------------------------------------------------------------------
+ * vaal_sampler.py:57-58 scores every pool row by the discriminator of vaal_discriminator.py on the VAE's mu:
+ *     p[i] = sigmoid(w3 . relu(W2 relu(W1 mu_i + b1) + b2) + b3)
+ * for fp32 rows mu[n, z] (leading dimension ldmu >= z), W1 [hidden, z] (ldw1 >= z), b1 [hidden], W2 [hidden, hidden]
+ * (ldw2 >= hidden), b2 [hidden], w3 [hidden] (the single row of the last Linear) and b3 [1], all device pointers.
+ * hidden must be 512, the reference's only width.  Both contractions run on the tensor cores as 3xTF32 (fp32 to about
+ * 2^-21 per product); the last layer is a fixed-order sum per row, so equal rows give equal p.  logits (optional, may
+ * be NULL) receives the pre-sigmoid value.  mu, w1, w2 16-byte aligned and every ld a multiple of 4, otherwise
+ * ALQ_ERR_INVALID.  The pool runs in slices of at most 131 072 rows, so the scratch is bounded (about 0.6 GB at
+ * z = 64) whatever n is.  Rank the rows with alq_select_smallest on p.                                              */
+int alq_vaal_scores(alq_ctx* ctx, const float* mu, int64_t n, int32_t z, int64_t ldmu, const float* w1, int64_t ldw1,
+                    const float* b1, const float* w2, int64_t ldw2, const float* b2, const float* w3, const float* b3,
+                    int32_t hidden, float* p, float* logits, void* stream);
 
 #ifdef __cplusplus
 }
