@@ -16,7 +16,7 @@ ALQ_OK = 0
 ERR_NAMES = {1: "ALQ_ERR_INVALID", 2: "ALQ_ERR_CUDA", 3: "ALQ_ERR_NOMEM", 4: "ALQ_ERR_STATE",
              5: "ALQ_ERR_NUMERIC"}
 MODE_MARGIN, MODE_LEAST_CONFIDENCE, MODE_ENTROPY = 0, 1, 2
-ABI_VERSION = 7
+ABI_VERSION = 8
 
 c_f32p = C.c_void_p
 c_i32p = C.c_void_p
@@ -100,6 +100,9 @@ SIGNATURES = {
     "alq_ward_labels": (C.c_int, [c_i32p, C.c_void_p, C.c_int64, C.c_int32, c_i32p]),
     "alq_vaal_scores": (C.c_int, [C.c_void_p, c_f32p, C.c_int64, C.c_int32, C.c_int64, c_f32p, C.c_int64, c_f32p,
                                   c_f32p, C.c_int64, c_f32p, c_f32p, c_f32p, C.c_int32, c_f32p, c_f32p, C.c_void_p]),
+    "alq_class_counts": (C.c_int, [C.c_void_p, c_i32p, C.c_void_p, C.c_int64, C.c_int32, c_i32p, C.c_void_p]),
+    "alq_class_pick": (C.c_int, [C.c_void_p, c_i32p, C.c_void_p, C.c_int64, C.c_int32, c_i32p, c_i32p, C.c_int64, c_i32p,
+                                 C.c_void_p]),
 }
 
 

@@ -5,7 +5,7 @@
 
 #include "alq_common.cuh"
 
-extern "C" int alq_version(void) { return 7; }
+extern "C" int alq_version(void) { return 8; }
 
 extern "C" int alq_create(alq_ctx** out, int device) {
     if (!out) return ALQ_ERR_INVALID;

@@ -447,6 +447,59 @@ class Engine:
                                              self._stream()), "alq_vaal_scores")
         return (p, logits) if return_logits else p
 
+    # -- K10: per-class counts and class-balanced picks (BalancedRandomSampler) -----------------------------
+    CLASS_MAX = 32768      # ALQ_CLASS_MAX of include/alq.h
+
+    @staticmethod
+    def _class_inputs(labels: torch.Tensor, avail: torch.Tensor, what: str):
+        if not isinstance(labels, torch.Tensor) or not labels.is_cuda or labels.dtype != torch.int32 or labels.dim() != 1:
+            raise AlqError(f"{what}: labels must be a 1-D CUDA int32 tensor")
+        if not isinstance(avail, torch.Tensor) or not avail.is_cuda or avail.dtype not in (torch.uint8, torch.bool):
+            raise AlqError(f"{what}: avail must be a CUDA uint8 (or bool) tensor")
+        if avail.numel() != labels.numel() or avail.device != labels.device:
+            raise AlqError(f"{what}: avail must hold one entry per label on the labels' device")
+        return labels.contiguous(), avail.contiguous().view(torch.uint8).reshape(-1)
+
+    def class_counts(self, labels: torch.Tensor, avail: torch.Tensor, num_classes: int) -> torch.Tensor:
+        """K10: counts[c] = number of rows with avail != 0 and labels == c, as a CUDA int32 [num_classes] tensor.
+        AlqError (ALQ_ERR_INVALID, naming the row) if an available row's label is outside [0, num_classes).
+        Synchronises the stream once."""
+        labels, avail = self._class_inputs(labels, avail, "class_counts")
+        c = int(num_classes)
+        if not 1 <= c <= self.CLASS_MAX:
+            raise AlqError(f"class_counts: num_classes={c} outside [1, {self.CLASS_MAX}]")
+        counts = torch.empty(c, dtype=torch.int32, device=labels.device)
+        self._check(self.lib.alq_class_counts(self._h, _ptr(labels), _ptr(avail), labels.numel(), c, _ptr(counts),
+                                              self._stream()), "alq_class_counts")
+        return counts
+
+    def class_pick(self, labels: torch.Tensor, avail: torch.Tensor, k, perm) -> torch.Tensor:
+        """K10: for each class c ascending with k[c] > 0, the perm-th available rows of class c (ascending row order), for
+        the k[c] entries of perm that belong to c (perm concatenates the classes' prefixes, classes ascending).  Returns
+        a CUDA int32 [sum(k)] tensor; an entry is -1 where its rank is not below the class's count.  `k` and `perm` are
+        host or device integer sequences; host ones travel in one copy.  Asynchronous."""
+        labels, avail = self._class_inputs(labels, avail, "class_pick")
+        dev = labels.device
+
+        def host(x):
+            return x.detach().cpu().numpy() if isinstance(x, torch.Tensor) else np.asarray(x)
+
+        k_h, perm_h = host(k).reshape(-1), host(perm).reshape(-1)
+        c, b = k_h.size, perm_h.size
+        if not 1 <= c <= self.CLASS_MAX:
+            raise AlqError(f"class_pick: {c} class budgets, need 1 .. {self.CLASS_MAX}")
+        for name, a in (("k", k_h), ("perm", perm_h)):
+            if a.size and (a.dtype.kind not in "iu" or a.min() < 0 or a.max() >= 2 ** 31):
+                raise AlqError(f"class_pick: {name} must hold non-negative int32 values")
+        if int(k_h.sum()) != b:
+            raise AlqError(f"class_pick: sum(k) = {int(k_h.sum())} but perm has {b} entries")
+        both = torch.from_numpy(np.concatenate([k_h, perm_h]).astype(np.int32)).to(dev, non_blocking=False)
+        out = torch.empty(b, dtype=torch.int32, device=dev)
+        self._check(self.lib.alq_class_pick(self._h, _ptr(labels), _ptr(avail), labels.numel(), c, _ptr(both),
+                                            C.c_void_p(both.data_ptr() + 4 * c), b, _ptr(out), self._stream()),
+                    "alq_class_pick")
+        return out
+
     # -- K4 / K5 ---------------------------------------------------------------------------------------
     def leaf_bounds(self, n: int) -> np.ndarray:
         """Leaf boundaries of NumPy's float32 pairwise summation over n entries (host helper of the library)."""

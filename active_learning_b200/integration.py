@@ -16,6 +16,7 @@ from __future__ import annotations
 
 from .query_strategies.coreset import (BADGEQuery, CoresetQuery, PartitionedBADGEQuery,
                                        PartitionedCoresetQuery)
+from .query_strategies.balanced_random import BalancedRandomQuery
 from .query_strategies.balancing import BalancingQuery
 from .query_strategies.margin_clustering import MarginClusteringQuery
 from .query_strategies.mase import BASEQuery, MASEQuery
@@ -34,6 +35,7 @@ _MIXINS = {
     "BASESampler": BASEQuery,
     "BalancingSampler": BalancingQuery,
     "MarginClusteringSampler": MarginClusteringQuery,
+    "BalancedRandomSampler": BalancedRandomQuery,
 }
 
 

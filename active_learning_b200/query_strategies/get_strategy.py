@@ -1,9 +1,9 @@
 """`--strategy` dispatch, same contract as active_learning/src/query_strategies/get_strategy.py:
-`get_strategy(name)` returns the class called `name`.  The twelve accelerated samplers (the seven of the
-north-star path plus MASE / BASE / Balancing, SURVEY.md section 8f, MarginClustering and VAAL) and the default RandomSampler
-are implemented; the reference's remaining class name resolves to a stub that raises a clear error (SURVEY.md section 8:
-out of scope for this path)."""
+`get_strategy(name)` returns the class called `name`.  Every class name the reference dispatches is implemented: the
+thirteen accelerated samplers (the seven of the north-star path plus MASE / BASE / Balancing, SURVEY.md section 8f,
+MarginClustering, VAAL and BalancedRandom) and the default RandomSampler."""
 from .badge_sampler import BADGESampler  # noqa: F401
+from .balanced_random_sampler import BalancedRandomSampler  # noqa: F401
 from .balancing_sampler import BalancingSampler  # noqa: F401
 from .base_sampler import BASESampler  # noqa: F401
 from .confidence_sampler import ConfidenceSampler  # noqa: F401
@@ -19,22 +19,11 @@ from .vaal_sampler import VAALSampler  # noqa: F401
 
 ACCELERATED = ("MarginSampler", "ConfidenceSampler", "EntropySampler", "CoresetSampler",
                "PartitionedCoresetSampler", "BADGESampler", "PartitionedBADGESampler", "MASESampler", "BASESampler",
-               "BalancingSampler", "MarginClusteringSampler", "VAALSampler")
-NOT_ON_THIS_PATH = ("BalancedRandomSampler",)
-
-
-def _out_of_scope(name):
-    class _Stub:
-        def __init__(self, *a, **k):
-            raise NotImplementedError(
-                f"{name} is not part of the accelerated query path; use the reference's own class")
-    _Stub.__name__ = name
-    return _Stub
+               "BalancingSampler", "MarginClusteringSampler", "VAALSampler", "BalancedRandomSampler")
+NOT_ON_THIS_PATH = ()
 
 
 def get_strategy(name):
-    if name in NOT_ON_THIS_PATH:
-        return _out_of_scope(name)
     cls = globals().get(name)
     if not isinstance(cls, type):
         raise NameError(f"name '{name}' is not defined")   # what the reference's eval(name) raises

@@ -330,6 +330,31 @@ int alq_vaal_scores(alq_ctx* ctx, const float* mu, int64_t n, int32_t z, int64_t
                     const float* b1, const float* w2, int64_t ldw2, const float* b2, const float* w3, const float* b3,
                     int32_t hidden, float* p, float* logits, void* stream);
 
+/* ---- K10: per-class counts and class-balanced picks (BalancedRandomSampler) --------------------------------------
+ * balanced_random_sampler.py:29-95 counts the available rows of every class and then, class by class, takes the
+ * rows `cur_available_idxs.nonzero()[torch.randperm(n_c)][:k_c]`.  Inputs: labels[n] (int32, device) and avail[n]
+ * (uint8, device; non-zero = the row may be picked), n < 2^31, 1 <= C <= ALQ_CLASS_MAX.  Rows whose avail is 0 are
+ * never inspected.  Both calls read the pool once: the pool is cut into tiles of ALQ_CLASS_TILE * ceil(C /
+ * ALQ_CLASS_TILE) rows, each tile's histogram is built in shared memory (4 C bytes, hence the bound on C) and
+ * scanned per class.  The table lives in the context's scratch arena: 4 C (ceil(n / tile) + 1) bytes, at most
+ * 4 (n + 2 C), plus 4 (C + 1) bytes of budget offsets for alq_class_pick.  The two calls share no state.
+ *
+ * alq_class_counts: counts[c] (int32, device) = the number of rows with avail != 0 and labels == c.  An available
+ *   row whose label is outside [0, C) makes the call return ALQ_ERR_INVALID; alq_last_error names the smallest such
+ *   row and its label.  Because that can only be seen on the device, this call synchronises the stream once, after
+ *   the pass (the counts themselves stay on the device).
+ * alq_class_pick: k[C] (int32, device) are per-class budgets and perm[B] (int32, device) the concatenated
+ *   permutation prefixes, classes ascending: out[off_c + j] (int32, device; off_c = k_0 + ... + k_{c-1}) = the
+ *   perm[off_c + j]-th (from 0) available row of class c in ascending row order, for j < k_c.  An output whose rank
+ *   is not in [0, n_c), or that lies past the sum of k, is -1; a negative k_c counts as 0; available rows with a label
+ *   outside [0, C) belong to no class.  Asynchronous; four launches whatever C and B are.  Deterministic.       */
+#define ALQ_CLASS_MAX 32768
+#define ALQ_CLASS_TILE 1024
+int alq_class_counts(alq_ctx* ctx, const int32_t* labels, const uint8_t* avail, int64_t n, int32_t c, int32_t* counts,
+                     void* stream);
+int alq_class_pick(alq_ctx* ctx, const int32_t* labels, const uint8_t* avail, int64_t n, int32_t c, const int32_t* k,
+                   const int32_t* perm, int64_t b, int32_t* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
