@@ -209,7 +209,7 @@ mase_rows_generic_kernel(const float* __restrict__ logits, int64_t n, int c, int
         int arg = INT_MAX;
         for (int j = lane; j < c; j += 32) {
             const float z = p[j];
-            if (z > best) { best = z; arg = j; }
+            if (mase_beats(z, best)) { best = z; arg = j; }
         }
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) {

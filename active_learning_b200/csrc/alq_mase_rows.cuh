@@ -29,8 +29,20 @@ struct MaseRowSmem {         // the row sits in shared memory: re-reading it cos
     }
 };
 
+// The arg-max follows torch.max: NaN ranks above every number, so a row with a NaN predicts its first NaN (and every
+// radius of that row is then +inf).  v beats best: v > best, or v is NaN and best is not.
+__device__ __forceinline__ bool mase_beats(float v, float best) { return !(v <= best) && best == best; }
+__device__ __forceinline__ bool mase_same(float a, float b) { return a == b || (a != a && b != b); }
+
+// NaN-propagating maximum (max.NaN: NaN if either operand is NaN)
+__device__ __forceinline__ float mase_fmax_nan(float a, float b) {
+    float r;
+    asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+    return r;
+}
+
 __device__ __forceinline__ void mase_argmax_merge(float& best, int& arg, float ob, int oa) {
-    if (ob > best || (ob == best && oa < arg)) { best = ob; arg = oa; }
+    if (mase_beats(ob, best) || (mase_same(ob, best) && oa < arg)) { best = ob; arg = oa; }
 }
 
 __device__ __forceinline__ float mase_radius_of(float zp, float z, float g, bool is_pred) {
@@ -55,10 +67,10 @@ __device__ __forceinline__ void mase_row_full(const Row& row, int lane, int nvec
     for (int k = 0; k < NV; ++k) {          // ascending index inside a lane: strict > keeps the first maximum
         const int base = (lane + 32 * k) * 4;
         const float4 e = row.get(k, lane);
-        if (e.x > best) { best = e.x; arg = base; }
-        if (e.y > best) { best = e.y; arg = base + 1; }
-        if (e.z > best) { best = e.z; arg = base + 2; }
-        if (e.w > best) { best = e.w; arg = base + 3; }
+        if (mase_beats(e.x, best)) { best = e.x; arg = base; }
+        if (mase_beats(e.y, best)) { best = e.y; arg = base + 1; }
+        if (mase_beats(e.z, best)) { best = e.z; arg = base + 2; }
+        if (mase_beats(e.w, best)) { best = e.w; arg = base + 3; }
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
@@ -106,8 +118,8 @@ __device__ __forceinline__ void mase_row_min(const Row& row, int lane, int c, co
         const float e[4] = {q.x, q.y, q.z, q.w};
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
-            if (e[j] > l1) { l2 = l1; a2 = a1; l1 = e[j]; a1 = base + j; }
-            else if (e[j] > l2) { l2 = e[j]; a2 = base + j; }
+            if (mase_beats(e[j], l1)) { l2 = l1; a2 = a1; l1 = e[j]; a1 = base + j; }
+            else if (mase_beats(e[j], l2)) { l2 = e[j]; a2 = base + j; }
         }
     }
     float best = l1;
@@ -168,17 +180,17 @@ __device__ __forceinline__ void mase_row_min_smem(const float4* __restrict__ p, 
         float m = ALQ_NEG_INF;
         if (idx < nvec) {
             const float4 e = p[idx];
-            m = fmaxf(fmaxf(e.x, e.y), fmaxf(e.z, e.w));
-        }
+            m = mase_fmax_nan(mase_fmax_nan(e.x, e.y), mase_fmax_nan(e.z, e.w));   // a NaN makes best NaN: nothing
+        }                                                                           // is pruned, every radius is +inf
         m4[k] = m;
         t2 = fmaxf(t2, fminf(t1, m));
-        t1 = fmaxf(t1, m);
+        t1 = mase_fmax_nan(t1, m);
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
         const float o1 = __shfl_xor_sync(0xffffffffu, t1, o);
         const float o2 = __shfl_xor_sync(0xffffffffu, t2, o);
-        const float hi = fmaxf(t1, o1);
+        const float hi = mase_fmax_nan(t1, o1);
         t2 = fmaxf(fminf(t1, o1), fmaxf(t2, o2));
         t1 = hi;
     }
@@ -199,10 +211,10 @@ __device__ __forceinline__ void mase_row_min_smem(const float4* __restrict__ p, 
             if (idx < nvec) {
                 const float4 e = p[idx];
                 const int base = idx * 4;
-                if (e.w == best) cand = min(cand, base + 3);
-                if (e.z == best) cand = min(cand, base + 2);
-                if (e.y == best) cand = min(cand, base + 1);
-                if (e.x == best) cand = min(cand, base);
+                if (mase_same(e.w, best)) cand = min(cand, base + 3);
+                if (mase_same(e.z, best)) cand = min(cand, base + 2);
+                if (mase_same(e.y, best)) cand = min(cand, base + 1);
+                if (mase_same(e.x, best)) cand = min(cand, base);
             }
         }
     }

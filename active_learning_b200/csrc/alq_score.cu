@@ -70,10 +70,10 @@ __device__ __forceinline__ RowStats row_stats_vec(const float4 (&v)[NV], int lan
         const float e[4] = {v[k].x, v[k].y, v[k].z, v[k].w};
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
-            const float dz = e[j] - t1;          // -inf in padded slots -> exp 0
+            const float dz = e[j] - t1;          // -inf in padded slots and masked classes -> exp 0
             const float ex = exp_neg(dz);
             s += ex;
-            if (WANT_W) w = (lane + 32 * k < nvec) ? fmaf(ex, dz, w) : w;   // 0 * -inf guard
+            if (WANT_W) w = ex > 0.f ? fmaf(ex, dz, w) : w;   // 0 log 0 = 0: no 0 * -inf
         }
     }
     s = warp_sum(s);
@@ -914,7 +914,7 @@ score_rows_generic_kernel(const float* __restrict__ logits, int64_t n, int c, in
             const float dz = p[j] - t1;
             const float ex = exp_neg(dz);
             s += ex;
-            w += ex * dz;
+            w = ex > 0.f ? fmaf(ex, dz, w) : w;   // 0 log 0 = 0 for masked (-inf) classes
         }
         s = warp_sum(s);
         w = warp_sum(w);

@@ -267,7 +267,9 @@ int64_t alq_pairwise_leaf_bounds(int64_t n, int32_t* out_host, int64_t cap);
  *   the diagonal; columns c..ldg-1 are filled with +inf) and, if gmin != NULL (c + 1 floats), gmin[a] = min_c ginv[a, c]
  *   for a < c plus gmin[c] = max_a (largest finite ginv[a, :]) / gmin[a], the spread of the class rows.
  *   Once per query: the head changes every round.
- * alq_mase_margins: one streaming pass over the logits slab.  pred[i] = p;  radius may be NULL (MASE needs only
+ * alq_mase_margins: one streaming pass over the logits slab.  pred[i] = p, the arg-max of torch.max: the first
+ *   maximum, and in a row with a NaN logit the first NaN (every radius of that row is then +inf, as in the reference,
+ *   where the NaN gap becomes +inf at :77).  radius may be NULL (MASE needs only
  *   the minimum); columns c..ldr-1 of radius are unspecified.  gmin (optional, from alq_class_gap_inv of the same
  *   table) lets the minimum-only pass skip every class that provably cannot attain it (the skip is verified per
  *   row, with a full evaluation if the check fails) -- same result, the table is touched for a handful of

@@ -39,7 +39,9 @@ def softmax_scores(logits: torch.Tensor, mode: int, batch_size: int = 128) -> to
 
     margin           : p(1) - p(2) of softmax(dim=1)            margin_sampler.py:33-35
     least confidence : p(1)                                     confidence_sampler.py:31-33
-    entropy (NEW)    : -H = sum_c p_c * log p_c  (so "smallest first" == most uncertain first)
+    entropy (NEW)    : -H = sum_c p_c * log p_c  (so "smallest first" == most uncertain first), with 0 log 0 = 0:
+                       a masked class (logit -inf, p = 0) adds nothing.  A row with a NaN or +inf logit, or with every
+                       logit -inf, still scores NaN.
     """
     logits = logits.detach().to(torch.float32).cpu()
     out = []
@@ -55,7 +57,8 @@ def softmax_scores(logits: torch.Tensor, mode: int, batch_size: int = 128) -> to
             out.append(top[:, 0])
         elif mode == MODE_ENTROPY:
             logp = F.log_softmax(z, dim=1)
-            out.append((logp.exp() * logp).sum(dim=1))
+            p = logp.exp()
+            out.append(torch.where(p == 0, torch.zeros(()), p * logp).sum(dim=1))
         else:
             raise ValueError(f"unknown mode {mode}")
     if not out:
