@@ -16,7 +16,7 @@ ALQ_OK = 0
 ERR_NAMES = {1: "ALQ_ERR_INVALID", 2: "ALQ_ERR_CUDA", 3: "ALQ_ERR_NOMEM", 4: "ALQ_ERR_STATE",
              5: "ALQ_ERR_NUMERIC"}
 MODE_MARGIN, MODE_LEAST_CONFIDENCE, MODE_ENTROPY = 0, 1, 2
-ABI_VERSION = 8
+ABI_VERSION = 9
 
 c_f32p = C.c_void_p
 c_i32p = C.c_void_p
@@ -44,6 +44,26 @@ class GreedyDesc(C.Structure):
         ("shard_off_host", C.c_void_p),
         ("shard_pos_host", C.c_void_p),
         ("step_kernel_ms_host", C.c_void_p),
+    ]
+
+
+class BalancingDesc(C.Structure):
+    """struct alq_balancing_desc (include/alq.h)."""
+    _fields_ = [
+        ("struct_size", C.c_size_t),
+        ("x", C.c_void_p), ("ldx", C.c_int64), ("d", C.c_int32),
+        ("xn", C.c_void_p),
+        ("labels", C.c_void_p),
+        ("avail", C.c_void_p),
+        ("labeled", C.c_void_p),
+        ("n", C.c_int64),
+        ("c", C.c_int32),
+        ("budget", C.c_int64),
+        ("mt_key_host", C.c_void_p),
+        ("mt_pos_host", C.c_void_p),
+        ("picks", C.c_void_p),
+        ("n_picks_host", C.c_void_p),
+        ("n_balancing_host", C.c_void_p),
     ]
 
 
@@ -103,6 +123,7 @@ SIGNATURES = {
     "alq_class_counts": (C.c_int, [C.c_void_p, c_i32p, C.c_void_p, C.c_int64, C.c_int32, c_i32p, C.c_void_p]),
     "alq_class_pick": (C.c_int, [C.c_void_p, c_i32p, C.c_void_p, C.c_int64, C.c_int32, c_i32p, c_i32p, C.c_int64, c_i32p,
                                  C.c_void_p]),
+    "alq_balancing_select": (C.c_int, [C.c_void_p, C.POINTER(BalancingDesc), C.c_void_p]),
 }
 
 

@@ -178,7 +178,10 @@ class_pick_kernel(const int32_t* __restrict__ labels, const uint8_t* __restrict_
     }
 }
 
-int table_pass(alq_ctx* ctx, const int32_t* labels, const uint8_t* avail, int n, int c, int32_t* tab,
+}  // namespace
+
+// K10's table pass and its size, shared with K11 (alq_balancing.cu): declared in alq_common.cuh
+int alq_class_table_pass(alq_ctx* ctx, const int32_t* labels, const uint8_t* avail, int n, int c, int32_t* tab,
                unsigned int* bad, int32_t* counts, cudaStream_t st) {
     const int tile = class_tile(c);
     const int ntiles = static_cast<int>((static_cast<int64_t>(n) + tile - 1) / tile);
@@ -194,12 +197,10 @@ int table_pass(alq_ctx* ctx, const int32_t* labels, const uint8_t* avail, int n,
     return ALQ_OK;
 }
 
-size_t table_entries(int64_t n, int c) {
+size_t alq_class_table_entries(int64_t n, int c) {
     const int tile = class_tile(c);
     return static_cast<size_t>((n + tile - 1) / tile + 1) * static_cast<size_t>(c);
 }
-
-}  // namespace
 
 extern "C" int alq_class_counts(alq_ctx* ctx, const int32_t* labels, const uint8_t* avail, int64_t n, int32_t c,
                                 int32_t* counts, void* stream) {
@@ -213,14 +214,14 @@ extern "C" int alq_class_counts(alq_ctx* ctx, const int32_t* labels, const uint8
         ALQ_CUDA(ctx, cudaMemsetAsync(counts, 0, static_cast<size_t>(c) * sizeof(int32_t), st));
         return ALQ_OK;
     }
-    const size_t entries = table_entries(n, c);
+    const size_t entries = alq_class_table_entries(n, c);
     int rc = alq_scratch_reserve(ctx, scratch_need({entries * sizeof(int32_t), sizeof(unsigned int)}));
     if (rc != ALQ_OK) return rc;
     ScratchCursor cur(ctx->scratch);
     int32_t* tab = cur.take<int32_t>(entries);
     unsigned int* bad = cur.take<unsigned int>(1);
     ALQ_CUDA(ctx, cudaMemsetAsync(bad, 0xff, sizeof(unsigned int), st));
-    rc = table_pass(ctx, labels, avail, static_cast<int>(n), c, tab, bad, counts, st);
+    rc = alq_class_table_pass(ctx, labels, avail, static_cast<int>(n), c, tab, bad, counts, st);
     if (rc != ALQ_OK) return rc;
     unsigned int bad_row = UINT_MAX;
     ALQ_CUDA(ctx, cudaMemcpyAsync(&bad_row, bad, sizeof(unsigned int), cudaMemcpyDeviceToHost, st));
@@ -248,13 +249,13 @@ extern "C" int alq_class_pick(alq_ctx* ctx, const int32_t* labels, const uint8_t
         ALQ_CUDA(ctx, cudaMemsetAsync(out, 0xff, static_cast<size_t>(b) * sizeof(int32_t), st));
         return ALQ_OK;
     }
-    const size_t entries = table_entries(n, c);
+    const size_t entries = alq_class_table_entries(n, c);
     int rc = alq_scratch_reserve(ctx, scratch_need({entries * sizeof(int32_t), (static_cast<size_t>(c) + 1) * sizeof(int32_t)}));
     if (rc != ALQ_OK) return rc;
     ScratchCursor cur(ctx->scratch);
     int32_t* tab = cur.take<int32_t>(entries);
     int32_t* koff = cur.take<int32_t>(static_cast<size_t>(c) + 1);
-    rc = table_pass(ctx, labels, avail, static_cast<int>(n), c, tab, nullptr, nullptr, st);
+    rc = alq_class_table_pass(ctx, labels, avail, static_cast<int>(n), c, tab, nullptr, nullptr, st);
     if (rc != ALQ_OK) return rc;
     class_budget_prefix_kernel<<<1, 1024, 0, st>>>(k, c, koff);
     ALQ_LAUNCH_CHECK(ctx);

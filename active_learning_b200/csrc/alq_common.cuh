@@ -93,6 +93,7 @@ struct alq_ctx {
                               // its candidates against the whole list -- the general route, also the fallback for tie groups)
     int spin_timeout_ms = 20000;   // bounded spins on peer flags (a dead peer must not hang the GPU)
     int base_impl = 0;        // 0 auto, 1 sequential class loop, 2 parallel candidate lists + in-order resolve
+    int balancing_loop = 0;   // 0 auto, 1 per-step path (alq_balancing_select declines), 2 persistent loop (error beyond its limits)
     std::string err;
 };
 
@@ -130,6 +131,12 @@ void alq_gridsync_begin(alq_ctx* ctx, cudaStream_t st);
 void alq_gridsync_end(alq_ctx* ctx, cudaStream_t st);
 
 int alq_scratch_reserve(alq_ctx* ctx, size_t bytes);
+// K10's tile histogram + per-class scan (alq_classes.cu): counts[k] = rows with avail != 0 and labels == k; an available
+// row with a label outside [0, c) is not counted and, with `bad` given, the smallest such row is atomicMin'ed there.
+// `tab` holds alq_class_table_entries(n, c) int32 entries of scratch.
+int alq_class_table_pass(alq_ctx* ctx, const int32_t* labels, const uint8_t* avail, int n, int c, int32_t* tab,
+                         unsigned int* bad, int32_t* counts, cudaStream_t st);
+size_t alq_class_table_entries(int64_t n, int c);
 int alq_pinned_reserve(alq_ctx* ctx, size_t bytes);
 int alq_arena2_reserve(alq_ctx* ctx, size_t bytes);
 

@@ -109,7 +109,8 @@ class Engine:
 
     def set_option(self, key: str, value: int):
         """'k3_impl': 0 auto / 1 fp32 SIMT / 2 wgmma 3xTF32;  'greedy_variant' (selection loop only): 0 auto / 1 direct / 2 pipeline / 3 persistent;  'spin_timeout_ms'; 'l2_resident_mb'; 'd2_fast_path'; 'tail_buckets';
-        'select_impl': 0 auto / 1 multi-kernel / 2 cluster;  'base_impl': 0 auto / 1 sequential / 2 parallel lists."""
+        'select_impl': 0 auto / 1 multi-kernel / 2 cluster;  'base_impl': 0 auto / 1 sequential / 2 parallel lists;
+        'balancing_loop': 0 auto / 1 per-step path / 2 persistent loop (AlqError beyond its limits)."""
         self._check(self.lib.alq_set_option(self._h, key.encode(), int(value)), "alq_set_option")
 
     @property
@@ -499,6 +500,62 @@ class Engine:
                                             C.c_void_p(both.data_ptr() + 4 * c), b, _ptr(out), self._stream()),
                     "alq_class_pick")
         return out
+
+    # -- K11: BalancingSampler's whole query -----------------------------------------------------------
+    def balancing_select(self, emb: torch.Tensor, xn: torch.Tensor, labels: torch.Tensor, avail: torch.Tensor,
+                         labeled: torch.Tensor, num_classes: int, budget: int):
+        """K11: balancing_sampler.py:58-134 in one persistent launch.  `emb` [n, d] float32 (d and the leading dimension
+        multiples of 4), `xn` = row_norm2(emb), `labels` int32 [n], `avail` / `labeled` uint8 (or bool) [n], all on this
+        device.  The random steps draw from NumPy's global RandomState exactly as `np.random.choice` would: the state is
+        taken from np.random.get_state() and the final one written back with set_state (has_gauss and cached_gaussian
+        unchanged).  Returns (picks: host int64 array in pick order, balancing steps), or None when the per-step path
+        must run instead (option "balancing_loop" = 1, or auto beyond the loop's limits; nothing is drawn then).
+        AlqError for bad inputs, for a labeled or available row whose label is outside [0, num_classes), and, under
+        balancing_loop = 2, for a shape beyond the limits (the message names the limit)."""
+        emb = _f32c(emb, "emb")
+        if emb.dim() != 2:
+            raise AlqError("balancing_select: emb must be [n, d]")
+        n, d = emb.shape
+        dev = emb.device
+        if n >= 2 ** 31:
+            raise AlqError(f"balancing_select: n={n} rows, need n < 2^31")
+        if not isinstance(xn, torch.Tensor) or not xn.is_cuda or xn.dtype != torch.float32 or xn.numel() != n:
+            raise AlqError("balancing_select: xn must be a CUDA float32 tensor with one entry per row")
+        if not isinstance(labels, torch.Tensor) or not labels.is_cuda or labels.dtype != torch.int32 or labels.numel() != n:
+            raise AlqError("balancing_select: labels must be a CUDA int32 tensor with one entry per row")
+        masks = []
+        for name, m in (("avail", avail), ("labeled", labeled)):
+            if (not isinstance(m, torch.Tensor) or not m.is_cuda or m.dtype not in (torch.uint8, torch.bool)
+                    or m.numel() != n or m.device != dev):
+                raise AlqError(f"balancing_select: {name} must be a CUDA uint8 (or bool) tensor with one entry per row")
+            masks.append(m.contiguous().view(torch.uint8).reshape(-1))
+        c, budget = int(num_classes), int(budget)
+        if not 1 <= c <= self.CLASS_MAX:
+            raise AlqError(f"balancing_select: num_classes={c} outside [1, {self.CLASS_MAX}]")
+        if budget < 0:
+            raise AlqError(f"balancing_select: budget={budget} is negative")
+        if emb.shape[1] % 4 or _ld(emb) % 4 or emb.data_ptr() % 16:
+            raise AlqError("balancing_select: emb needs d and its leading dimension multiples of 4 and a 16-byte aligned base")
+        xn, labels = xn.contiguous().reshape(-1), labels.contiguous()
+        name, key, pos, has_gauss, cached = np.random.get_state()
+        key = np.array(key, dtype=np.uint32)
+        pos_c, n_picks, n_bal = C.c_int32(int(pos)), C.c_int64(0), C.c_int64(0)
+        picks = torch.empty(max(budget, 1), dtype=torch.int32, device=dev)
+        desc = _lib.BalancingDesc()
+        desc.struct_size = C.sizeof(_lib.BalancingDesc)
+        desc.x, desc.ldx, desc.d = emb.data_ptr(), _ld(emb), d
+        desc.xn, desc.labels = xn.data_ptr(), labels.data_ptr()
+        desc.avail, desc.labeled = masks[0].data_ptr(), masks[1].data_ptr()
+        desc.n, desc.c, desc.budget = n, c, budget
+        desc.mt_key_host = key.ctypes.data
+        desc.mt_pos_host = C.addressof(pos_c)
+        desc.picks = picks.data_ptr()
+        desc.n_picks_host, desc.n_balancing_host = C.addressof(n_picks), C.addressof(n_bal)
+        self._check(self.lib.alq_balancing_select(self._h, C.byref(desc), self._stream()), "alq_balancing_select")
+        if n_picks.value < 0:
+            return None
+        np.random.set_state((name, key, int(pos_c.value), has_gauss, cached))
+        return picks[:n_picks.value].cpu().numpy().astype(np.int64), int(n_bal.value)
 
     # -- K4 / K5 ---------------------------------------------------------------------------------------
     def leaf_bounds(self, n: int) -> np.ndarray:

@@ -13,6 +13,11 @@ Rounding: the class centres here are running per-class sums divided by (count + 
 the last fp32 bits, so a balancing step whose two best ratios are closer than ~1e-6 relative may pick the other row
 than the reference does.  The golden fixtures (tests/golden/reference_golden_balancing.npz) are pick-for-pick
 identical; outside them the guarantee is "same pick unless the reference's own arg-min is decided by fp32 rounding".
+
+When the engine offers `balancing_select` (K11) the whole query is one persistent launch instead: same branch test,
+same tie rule, NumPy's RNG advanced draw for draw on the device, class sums in fp64 in a fixed order.  The engine
+declines (returns None) under option "balancing_loop" = 1 or beyond the loop's limits (centres in shared memory, counts
+plus budget below 2^24); the step loop below then runs unchanged.
 """
 from __future__ import annotations
 
@@ -53,6 +58,13 @@ class BalancingQuery(EngineMixin):
         budget = int(min(idxs_for_query.sum(), budget))
         if budget <= 0:
             return labeled_idxs_cur_rd, 0
+        if hasattr(eng, "balancing_select"):
+            got = eng.balancing_select(emb, eng.row_norm2(emb), ys.to(device=dev, dtype=torch.int32),
+                                       torch.from_numpy(idxs_for_query.astype(np.uint8)).to(dev),
+                                       torch.from_numpy(idxs_labeled.astype(np.uint8)).to(dev), C, budget)
+            if got is not None:
+                picks = list(got[0])
+                return picks, len(picks)
         # device state: per-class embedding sums, row norms, availability mask
         ys_dev = ys.to(dev)
         lab_rows = torch.from_numpy(np.flatnonzero(idxs_labeled)).to(dev)

@@ -59,7 +59,10 @@ const char* alq_last_error(const alq_ctx* ctx);
  *                    what a pool whose scores do not spread (tie groups) falls back to inside the launch
  *   "spin_timeout_ms" how long a kernel waits for a peer GPU's flag before giving up with ALQ_ERR_STATE (default 20000)
  *   "select_impl"    0 auto | 1 multi-kernel radix select   | 2 single cluster-resident launch
- *   "base_impl"      0 auto | 1 sequential class loop       | 2 per-class candidate lists + in-order resolve */
+ *   "base_impl"      0 auto | 1 sequential class loop       | 2 per-class candidate lists + in-order resolve
+ *   "balancing_loop" 0 auto (the persistent loop whenever its limits hold) | 1 per-step path: alq_balancing_select declines
+ *                    (n_picks_host = -1) and the caller runs its own step loop | 2 persistent loop, ALQ_ERR_INVALID naming
+ *                    the limit when the shape is beyond it */
 int alq_set_option(alq_ctx* ctx, const char* key, int64_t value);
 /* Number of kernels this context has launched since creation (bench.py's `gpu_launches`). */
 int64_t alq_launch_count(const alq_ctx* ctx);
@@ -356,6 +359,49 @@ int alq_class_counts(alq_ctx* ctx, const int32_t* labels, const uint8_t* avail, 
                      void* stream);
 int alq_class_pick(alq_ctx* ctx, const int32_t* labels, const uint8_t* avail, int64_t n, int32_t c, const int32_t* k,
                    const int32_t* perm, int64_t b, int32_t* out, void* stream);
+
+/* ---- K11: the whole query of BalancingSampler as one persistent launch -------------------------------------------
+ * balancing_sampler.py:58-134 picks one row per step: when the labeled class histogram is imbalanced relative to the
+ * remaining budget (:66-84, evaluated in fp32 exactly as torch does on the CPU) it takes the available row with the
+ * smallest d2(row, rarest centre) / max over the majority centres of d2(row, centre) (numerator 1 when the rarest class
+ * has no labeled row; lowest row on ties, NaN ranked as alq_ratio_argmin ranks it), otherwise one legacy
+ * `np.random.choice` over the available rows (MT19937, masked rejection draws).  After a pick the row is labeled, its
+ * class count rises and that class's centre is recomputed.
+ *
+ * Inputs (device unless _host): x[n, d] fp32 rows (d % 4 == 0, ldx % 4 == 0, 16-byte aligned), xn[n] = alq_row_norm2(x),
+ * labels[n] int32, avail[n] / labeled[n] uint8 masks (not modified), c classes, the budget, and NumPy's MT19937 state
+ * (np.random.get_state(): 624 key words and the position).  Class sums are fp64 in a fixed order (labeled rows in row
+ * order per chunk of 65 536 rows, the chunks in order, then the picks in pick order); a centre is
+ * fl32(sum / fl32(count + 1e-5)); a row's dot product with a centre is a fixed function of the row (lane-strided fmaf
+ * chains folded by a butterfly), whatever the grid, so the picks are bit-reproducible.
+ * Outputs: picks[0 .. *n_picks_host) int32 in pick order, *n_picks_host = min(budget, available rows),
+ * *n_balancing_host = the steps that balanced, and the MT19937 key / position after the last draw (in place).
+ * An available or labeled row whose label is outside [0, c) makes the call return ALQ_ERR_INVALID naming the row and
+ * its label, before any draw.
+ * Limits (option "balancing_loop"): every centre (4 c d bytes) plus the per-CTA tables fit the shared memory of one
+ * CTA, and 1 KB per class for the fp64 set-up pass; at most 65 535 rows per CTA segment (n < 65 536 * SMs); every class
+ * count plus the budget below 2^24 (the fp32 imbalance test is exact there).  Beyond them the call declines
+ * (*n_picks_host = -1, nothing drawn) under option 0 or 1 and fails with ALQ_ERR_INVALID under option 2.
+ * Launches: K10's table pass (2), one segment count, two fp64 set-up passes and the loop: six, whatever the budget.
+ * Synchronous (it reads the label check, the counts and the final RNG state back).                              */
+typedef struct alq_balancing_desc {
+    size_t struct_size;          /* sizeof(alq_balancing_desc) */
+    const float* x;  int64_t ldx; int32_t d;
+    const float* xn;             /* [n] |x_i|^2 */
+    const int32_t* labels;       /* [n] */
+    const uint8_t* avail;        /* [n] non-zero: the row may be picked */
+    const uint8_t* labeled;      /* [n] non-zero: the row is labeled (class histogram, centres) */
+    int64_t n;
+    int32_t c;
+    int64_t budget;
+    uint32_t* mt_key_host;       /* [624] in/out: np.random.get_state()[1] */
+    int32_t* mt_pos_host;        /* in/out: np.random.get_state()[2] */
+    int32_t* picks;              /* [budget] out */
+    int64_t* n_picks_host;       /* out: picks written, or -1 when the call declined (option / limits) */
+    int64_t* n_balancing_host;   /* out: balancing steps among them */
+} alq_balancing_desc;
+
+int alq_balancing_select(alq_ctx* ctx, const alq_balancing_desc* desc, void* stream);
 
 #ifdef __cplusplus
 }
