@@ -16,7 +16,7 @@ ALQ_OK = 0
 ERR_NAMES = {1: "ALQ_ERR_INVALID", 2: "ALQ_ERR_CUDA", 3: "ALQ_ERR_NOMEM", 4: "ALQ_ERR_STATE",
              5: "ALQ_ERR_NUMERIC"}
 MODE_MARGIN, MODE_LEAST_CONFIDENCE, MODE_ENTROPY = 0, 1, 2
-ABI_VERSION = 9
+ABI_VERSION = 10
 
 c_f32p = C.c_void_p
 c_i32p = C.c_void_p
@@ -124,6 +124,7 @@ SIGNATURES = {
     "alq_class_pick": (C.c_int, [C.c_void_p, c_i32p, C.c_void_p, C.c_int64, C.c_int32, c_i32p, c_i32p, C.c_int64, c_i32p,
                                  C.c_void_p]),
     "alq_balancing_select": (C.c_int, [C.c_void_p, C.POINTER(BalancingDesc), C.c_void_p]),
+    "alq_balancing_table_select": (C.c_int, [C.c_void_p, C.POINTER(BalancingDesc), C.c_void_p]),
 }
 
 

@@ -23,7 +23,7 @@
 // warp, nor the CTA, nor the grid size changes it, so the picks are bit-reproducible.
 #include <limits.h>
 
-#include "alq_greedy.cuh"
+#include "alq_balancing.cuh"
 
 namespace {
 
@@ -32,14 +32,6 @@ constexpr int kBalWarps = kBalThreads / 32;
 constexpr int kCentresPerPass = 8;               // dot products a lane accumulates at once
 constexpr int kSumChunk = 65536;                 // rows per fixed chunk of the fp64 class sums
 constexpr int kSumDims = 128;                    // dimensions per CTA of the class-sum pass (one per thread)
-constexpr int kMtN = 624;
-constexpr int kSegRowsMax = 65535;               // the key word carries a 16-bit row offset (0xffff: empty segment)
-constexpr unsigned int kEmptyOff = 0xffffu;
-
-__host__ __device__ __forceinline__ int seg_lo(int n, int grid, int b) {
-    return static_cast<int>(static_cast<long long>(n) * b / grid);
-}
-
 struct BalArgs {
     const float* x; long long ldx; int d;
     const float* xn;
@@ -61,7 +53,7 @@ struct BalArgs {
 };
 
 __device__ __forceinline__ float centre_of(double sum, int count) {
-    const float denom = __fadd_rn(static_cast<float>(count), 1e-5f);   // balancing_sampler.py:89 in fp32
+    const float denom = bal_den(count);
     return __double2float_rn(sum / static_cast<double>(denom));
 }
 
@@ -76,59 +68,6 @@ __device__ __forceinline__ float dot_fixed(const float4* x, const float4* q, int
         acc = fmaf(v.w, w.w, acc);
     }
     return warp_sum(acc);
-}
-
-// balancing_sampler.py:66-84 as torch evaluates it on the CPU: counts (< 2^24) against their fp32 mean, each average
-// fl32(sum) / fl32(n), spread = the difference (NaN when no class is above the mean), balance iff
-// remaining <= fl32(#rest) * spread.  Returns the number of selected classes (0: random step): sel[0] = the rarest class
-// (first index of the minimum), sel[1..] = the majority classes ascending.
-__device__ int imbalance_test(const int* cnt, int c, int remaining, int* sel) {
-    int total = 0, rare = 0;
-    for (int i = 0; i < c; ++i) {
-        total += cnt[i];
-        if (cnt[i] < cnt[rare]) rare = i;
-    }
-    const float mean = __fdiv_rn(static_cast<float>(total), static_cast<float>(c));
-    int na = 0, sa = 0, nr = 0, sr = 0;
-    for (int i = 0; i < c; ++i) {
-        if (static_cast<float>(cnt[i]) > mean) { ++na; sa += cnt[i]; }
-        else { ++nr; sr += cnt[i]; }
-    }
-    const float spread = __fsub_rn(__fdiv_rn(static_cast<float>(sa), static_cast<float>(na)),
-                                   __fdiv_rn(static_cast<float>(sr), static_cast<float>(nr)));
-    if (!(static_cast<float>(remaining) <= __fmul_rn(static_cast<float>(nr), spread))) return 0;
-    sel[0] = rare;
-    int m = 1;
-    for (int i = 0; i < c; ++i)
-        if (static_cast<float>(cnt[i]) > mean) sel[m++] = i;
-    return m;
-}
-
-// NumPy's mt19937_gen / mt19937_next32 (numpy/random/src/mt19937), one thread, state in shared memory
-__device__ void mt_twist(unsigned int* mt) {
-    for (int i = 0; i < kMtN; ++i) {
-        const unsigned int y = (mt[i] & 0x80000000u) | (mt[i + 1 < kMtN ? i + 1 : 0] & 0x7fffffffu);
-        const int j = i + 397 < kMtN ? i + 397 : i + 397 - kMtN;
-        mt[i] = mt[j] ^ (y >> 1) ^ ((y & 1u) ? 0x9908b0dfu : 0u);
-    }
-}
-__device__ __forceinline__ unsigned int mt_next32(unsigned int* mt, int& pos) {
-    if (pos >= kMtN) { mt_twist(mt); pos = 0; }
-    unsigned int y = mt[pos++];
-    y ^= y >> 11;
-    y ^= (y << 7) & 0x9d2c5680u;
-    y ^= (y << 15) & 0xefc60000u;
-    y ^= y >> 18;
-    return y;
-}
-// legacy RandomState.randint(0, rng + 1) for rng < 2^32 - 1 (random_bounded_uint64_fill, masked): rng == 0 draws nothing
-__device__ unsigned int mt_bounded(unsigned int* mt, int& pos, unsigned int rng) {
-    if (rng == 0) return 0;
-    unsigned int mask = rng;
-    mask |= mask >> 1; mask |= mask >> 2; mask |= mask >> 4; mask |= mask >> 8; mask |= mask >> 16;
-    unsigned int v;
-    while ((v = (mt_next32(mt, pos) & mask)) > rng) {}
-    return v;
 }
 
 // available rows per CTA segment; the smallest available row with a label outside [0, c) -> *bad
@@ -404,25 +343,55 @@ __global__ void __launch_bounds__(kBalThreads, 1) balancing_loop_kernel(const __
 
 }  // namespace
 
-extern "C" int alq_balancing_select(alq_ctx* ctx, const alq_balancing_desc* D, void* stream) {
-    if (!ctx) return ALQ_ERR_INVALID;
-    if (!D || D->struct_size < sizeof(alq_balancing_desc)) ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_balancing_select: bad descriptor");
+int alq_bal_check_desc(alq_ctx* ctx, const alq_balancing_desc* D, const char* fn) {
+    if (!D || D->struct_size < sizeof(alq_balancing_desc)) ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: bad descriptor", fn);
     const int64_t n64 = D->n;
     const int c = D->c, d = D->d;
-    if (n64 < 0 || n64 >= (1LL << 31)) ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_balancing_select: n=%lld outside [0, 2^31)", (long long)n64);
-    if (c < 1 || c > ALQ_CLASS_MAX) ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_balancing_select: C=%d outside [1, %d]", c, ALQ_CLASS_MAX);
+    if (n64 < 0 || n64 >= (1LL << 31)) ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: n=%lld outside [0, 2^31)", fn, (long long)n64);
+    if (c < 1 || c > ALQ_CLASS_MAX) ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: C=%d outside [1, %d]", fn, c, ALQ_CLASS_MAX);
     if (d <= 0 || D->ldx < d || D->budget < 0)
-        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_balancing_select: bad shape d=%d ldx=%lld budget=%lld", d, (long long)D->ldx, (long long)D->budget);
+        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: bad shape d=%d ldx=%lld budget=%lld", fn, d, (long long)D->ldx, (long long)D->budget);
     if (!D->mt_key_host || !D->mt_pos_host || !D->n_picks_host || !D->n_balancing_host ||
         (n64 > 0 && (!D->x || !D->xn || !D->labels || !D->avail || !D->labeled)) || (D->budget > 0 && !D->picks))
-        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_balancing_select: null pointer");
+        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: null pointer", fn);
     if ((d % 4) || (D->ldx % 4) || (n64 > 0 && !aligned16(D->x)))
-        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_balancing_select: d and ldx must be multiples of 4 and x 16-byte aligned");
+        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: d and ldx must be multiples of 4 and x 16-byte aligned", fn);
     if (*D->mt_pos_host < 0 || *D->mt_pos_host > kMtN)
-        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_balancing_select: MT19937 position %d outside [0, %d]", *D->mt_pos_host, kMtN);
+        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: MT19937 position %d outside [0, %d]", fn, *D->mt_pos_host, kMtN);
     *D->n_picks_host = -1;
     *D->n_balancing_host = 0;
-    if (ctx->balancing_loop == 1) return ALQ_OK;                      // the caller runs the per-step path
+    return ALQ_OK;
+}
+
+int alq_bal_counts(alq_ctx* ctx, const alq_balancing_desc* D, int n, int c, int grid, int32_t* tab, unsigned int* bad,
+                   int32_t* counts, int32_t* seg_avail, int32_t* counts_h, int32_t* seg_h, cudaStream_t st, const char* fn) {
+    ALQ_CUDA(ctx, cudaMemsetAsync(bad, 0xff, 2 * sizeof(unsigned int), st));
+    const int rc = alq_class_table_pass(ctx, D->labels, D->labeled, n, c, tab, bad, counts, st);
+    if (rc != ALQ_OK) return rc;
+    bal_seg_count_kernel<<<grid, 256, 0, st>>>(D->labels, D->avail, n, c, grid, seg_avail, bad + 1);
+    ALQ_LAUNCH_CHECK(ctx);
+    unsigned int bad_h[2] = {UINT_MAX, UINT_MAX};
+    ALQ_CUDA(ctx, cudaMemcpyAsync(bad_h, bad, sizeof(bad_h), cudaMemcpyDeviceToHost, st));
+    ALQ_CUDA(ctx, cudaMemcpyAsync(counts_h, counts, static_cast<size_t>(c) * 4, cudaMemcpyDeviceToHost, st));
+    ALQ_CUDA(ctx, cudaMemcpyAsync(seg_h, seg_avail, static_cast<size_t>(grid) * 4, cudaMemcpyDeviceToHost, st));
+    ALQ_CUDA(ctx, cudaStreamSynchronize(st));
+    for (int k = 1; k >= 0; --k)
+        if (bad_h[k] != UINT_MAX) {
+            int32_t y = 0;
+            ALQ_CUDA(ctx, cudaMemcpy(&y, D->labels + bad_h[k], sizeof(int32_t), cudaMemcpyDeviceToHost));
+            ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: %s row %u has label %d, outside [0, %d)", fn,
+                     k ? "available" : "labeled", bad_h[k], y, c);
+        }
+    return ALQ_OK;
+}
+
+extern "C" int alq_balancing_select(alq_ctx* ctx, const alq_balancing_desc* D, void* stream) {
+    if (!ctx) return ALQ_ERR_INVALID;
+    int rc = alq_bal_check_desc(ctx, D, "alq_balancing_select");
+    if (rc != ALQ_OK) return rc;
+    const int64_t n64 = D->n;
+    const int c = D->c, d = D->d;
+    if (ctx->balancing_loop == 1 || ctx->balancing_loop == 3) return ALQ_OK;   // the per-step path or K12 runs
     const int n = static_cast<int>(n64);
     const bool forced = ctx->balancing_loop == 2;
     if (n == 0 || D->budget == 0) {
@@ -456,7 +425,7 @@ extern "C" int alq_balancing_select(alq_ctx* ctx, const alq_balancing_desc* D, v
                                       static_cast<size_t>(nchunks) * cd * 8, cd * 8, static_cast<size_t>(grid) * cd * 8,
                                       static_cast<size_t>(n), (kMtN + 1) * 4 * 2, static_cast<size_t>(grid) * 16,
                                       static_cast<size_t>(std::min<int64_t>(budget_req, n)) * 8, 16});
-    int rc = alq_scratch_reserve(ctx, need);
+    rc = alq_scratch_reserve(ctx, need);
     if (rc != ALQ_OK) return rc;
     ScratchCursor cur(ctx->scratch);
     int32_t* tab = cur.take<int32_t>(entries);
@@ -472,24 +441,9 @@ extern "C" int alq_balancing_select(alq_ctx* ctx, const alq_balancing_desc* D, v
     unsigned long long* pickw = cur.take<unsigned long long>(static_cast<size_t>(std::min<int64_t>(budget_req, n)));
     int* small = cur.take<int>(4);                                     // [0] status, [1] balancing steps
 
-    ALQ_CUDA(ctx, cudaMemsetAsync(bad, 0xff, 2 * sizeof(unsigned int), st));
-    rc = alq_class_table_pass(ctx, D->labels, D->labeled, n, c, tab, bad, counts, st);
-    if (rc != ALQ_OK) return rc;
-    bal_seg_count_kernel<<<grid, 256, 0, st>>>(D->labels, D->avail, n, c, grid, seg_avail, bad + 1);
-    ALQ_LAUNCH_CHECK(ctx);
     std::vector<int32_t> counts_h(c), seg_h(grid);
-    unsigned int bad_h[2] = {UINT_MAX, UINT_MAX};
-    ALQ_CUDA(ctx, cudaMemcpyAsync(bad_h, bad, sizeof(bad_h), cudaMemcpyDeviceToHost, st));
-    ALQ_CUDA(ctx, cudaMemcpyAsync(counts_h.data(), counts, static_cast<size_t>(c) * 4, cudaMemcpyDeviceToHost, st));
-    ALQ_CUDA(ctx, cudaMemcpyAsync(seg_h.data(), seg_avail, static_cast<size_t>(grid) * 4, cudaMemcpyDeviceToHost, st));
-    ALQ_CUDA(ctx, cudaStreamSynchronize(st));
-    for (int k = 1; k >= 0; --k)
-        if (bad_h[k] != UINT_MAX) {
-            int32_t y = 0;
-            ALQ_CUDA(ctx, cudaMemcpy(&y, D->labels + bad_h[k], sizeof(int32_t), cudaMemcpyDeviceToHost));
-            ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_balancing_select: %s row %u has label %d, outside [0, %d)",
-                     k ? "available" : "labeled", bad_h[k], y, c);
-        }
+    rc = alq_bal_counts(ctx, D, n, c, grid, tab, bad, counts, seg_avail, counts_h.data(), seg_h.data(), st, "alq_balancing_select");
+    if (rc != ALQ_OK) return rc;
     int64_t n_avail = 0, labeled_total = 0;
     for (int b = 0; b < grid; ++b) n_avail += seg_h[b];
     for (int k = 0; k < c; ++k) labeled_total += counts_h[k];

@@ -93,7 +93,7 @@ struct alq_ctx {
                               // its candidates against the whole list -- the general route, also the fallback for tie groups)
     int spin_timeout_ms = 20000;   // bounded spins on peer flags (a dead peer must not hang the GPU)
     int base_impl = 0;        // 0 auto, 1 sequential class loop, 2 parallel candidate lists + in-order resolve
-    int balancing_loop = 0;   // 0 auto, 1 per-step path (alq_balancing_select declines), 2 persistent loop (error beyond its limits)
+    int balancing_loop = 0;   // 0 auto, 1 per-step path (K11 and K12 decline), 2 K11 (error beyond its limits), 3 K12 (the same)
     std::string err;
 };
 

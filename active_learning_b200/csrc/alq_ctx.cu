@@ -5,7 +5,7 @@
 
 #include "alq_common.cuh"
 
-extern "C" int alq_version(void) { return 9; }
+extern "C" int alq_version(void) { return 10; }
 
 extern "C" int alq_create(alq_ctx** out, int device) {
     if (!out) return ALQ_ERR_INVALID;
@@ -103,7 +103,7 @@ extern "C" int alq_set_option(alq_ctx* ctx, const char* key, int64_t value) {
     else if (k == "spin_timeout_ms" && value >= 1 && value <= 3600000) ctx->spin_timeout_ms = static_cast<int>(value);
     else if (k == "select_impl" && value >= 0 && value <= 2) ctx->select_impl = static_cast<int>(value);
     else if (k == "base_impl" && value >= 0 && value <= 2) ctx->base_impl = static_cast<int>(value);
-    else if (k == "balancing_loop" && value >= 0 && value <= 2) ctx->balancing_loop = static_cast<int>(value);
+    else if (k == "balancing_loop" && value >= 0 && value <= 3) ctx->balancing_loop = static_cast<int>(value);
     else ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_set_option: unknown option or value: %s=%lld", key, (long long)value);
     return ALQ_OK;
 }

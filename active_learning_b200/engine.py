@@ -110,7 +110,7 @@ class Engine:
     def set_option(self, key: str, value: int):
         """'k3_impl': 0 auto / 1 fp32 SIMT / 2 wgmma 3xTF32;  'greedy_variant' (selection loop only): 0 auto / 1 direct / 2 pipeline / 3 persistent;  'spin_timeout_ms'; 'l2_resident_mb'; 'd2_fast_path'; 'tail_buckets';
         'select_impl': 0 auto / 1 multi-kernel / 2 cluster;  'base_impl': 0 auto / 1 sequential / 2 parallel lists;
-        'balancing_loop': 0 auto / 1 per-step path / 2 persistent loop (AlqError beyond its limits)."""
+        'balancing_loop': 0 auto / 1 per-step path / 2 persistent loop K11 / 3 table loop K12 (2, 3: AlqError beyond the limits)."""
         self._check(self.lib.alq_set_option(self._h, key.encode(), int(value)), "alq_set_option")
 
     @property
@@ -509,35 +509,51 @@ class Engine:
         device.  The random steps draw from NumPy's global RandomState exactly as `np.random.choice` would: the state is
         taken from np.random.get_state() and the final one written back with set_state (has_gauss and cached_gaussian
         unchanged).  Returns (picks: host int64 array in pick order, balancing steps), or None when the per-step path
-        must run instead (option "balancing_loop" = 1, or auto beyond the loop's limits; nothing is drawn then).
+        must run instead (option "balancing_loop" = 1 or 3, or auto beyond the loop's limits; nothing is drawn then).
         AlqError for bad inputs, for a labeled or available row whose label is outside [0, num_classes), and, under
         balancing_loop = 2, for a shape beyond the limits (the message names the limit)."""
+        return self._balancing_call("balancing_select", self.lib.alq_balancing_select, emb, xn, labels, avail, labeled,
+                                    num_classes, budget)
+
+    def balancing_table_select(self, emb: torch.Tensor, xn: torch.Tensor, labels: torch.Tensor, avail: torch.Tensor,
+                               labeled: torch.Tensor, num_classes: int, budget: int):
+        """K12: the same query, arguments and contract as `balancing_select`, over an incremental row x class table of
+        fp64 dot products with the class sums instead of centres in shared memory, so it runs at ImageNet-LT's 1 000
+        classes of 2 048 dimensions.  Returns None under option "balancing_loop" = 1 or 2, or under auto beyond its
+        limits (shared memory for the per-class tables, rows per CTA segment, counts plus budget below 2^24, the table
+        and the per-CTA class sums in free device memory); AlqError naming the limit under balancing_loop = 3."""
+        return self._balancing_call("balancing_table_select", self.lib.alq_balancing_table_select, emb, xn, labels, avail,
+                                    labeled, num_classes, budget)
+
+    def _balancing_call(self, name, fn, emb, xn, labels, avail, labeled, num_classes, budget):
+        """Checks the arguments of K11 / K12 (messages start with `name`), runs `fn` with NumPy's MT19937 state and
+        writes the state back; None when the call declined."""
         emb = _f32c(emb, "emb")
         if emb.dim() != 2:
-            raise AlqError("balancing_select: emb must be [n, d]")
+            raise AlqError(f"{name}: emb must be [n, d]")
         n, d = emb.shape
         dev = emb.device
         if n >= 2 ** 31:
-            raise AlqError(f"balancing_select: n={n} rows, need n < 2^31")
+            raise AlqError(f"{name}: n={n} rows, need n < 2^31")
         if not isinstance(xn, torch.Tensor) or not xn.is_cuda or xn.dtype != torch.float32 or xn.numel() != n:
-            raise AlqError("balancing_select: xn must be a CUDA float32 tensor with one entry per row")
+            raise AlqError(f"{name}: xn must be a CUDA float32 tensor with one entry per row")
         if not isinstance(labels, torch.Tensor) or not labels.is_cuda or labels.dtype != torch.int32 or labels.numel() != n:
-            raise AlqError("balancing_select: labels must be a CUDA int32 tensor with one entry per row")
+            raise AlqError(f"{name}: labels must be a CUDA int32 tensor with one entry per row")
         masks = []
-        for name, m in (("avail", avail), ("labeled", labeled)):
+        for mname, m in (("avail", avail), ("labeled", labeled)):
             if (not isinstance(m, torch.Tensor) or not m.is_cuda or m.dtype not in (torch.uint8, torch.bool)
                     or m.numel() != n or m.device != dev):
-                raise AlqError(f"balancing_select: {name} must be a CUDA uint8 (or bool) tensor with one entry per row")
+                raise AlqError(f"{name}: {mname} must be a CUDA uint8 (or bool) tensor with one entry per row")
             masks.append(m.contiguous().view(torch.uint8).reshape(-1))
         c, budget = int(num_classes), int(budget)
         if not 1 <= c <= self.CLASS_MAX:
-            raise AlqError(f"balancing_select: num_classes={c} outside [1, {self.CLASS_MAX}]")
+            raise AlqError(f"{name}: num_classes={c} outside [1, {self.CLASS_MAX}]")
         if budget < 0:
-            raise AlqError(f"balancing_select: budget={budget} is negative")
+            raise AlqError(f"{name}: budget={budget} is negative")
         if emb.shape[1] % 4 or _ld(emb) % 4 or emb.data_ptr() % 16:
-            raise AlqError("balancing_select: emb needs d and its leading dimension multiples of 4 and a 16-byte aligned base")
+            raise AlqError(f"{name}: emb needs d and its leading dimension multiples of 4 and a 16-byte aligned base")
         xn, labels = xn.contiguous().reshape(-1), labels.contiguous()
-        name, key, pos, has_gauss, cached = np.random.get_state()
+        sname, key, pos, has_gauss, cached = np.random.get_state()
         key = np.array(key, dtype=np.uint32)
         pos_c, n_picks, n_bal = C.c_int32(int(pos)), C.c_int64(0), C.c_int64(0)
         picks = torch.empty(max(budget, 1), dtype=torch.int32, device=dev)
@@ -551,10 +567,10 @@ class Engine:
         desc.mt_pos_host = C.addressof(pos_c)
         desc.picks = picks.data_ptr()
         desc.n_picks_host, desc.n_balancing_host = C.addressof(n_picks), C.addressof(n_bal)
-        self._check(self.lib.alq_balancing_select(self._h, C.byref(desc), self._stream()), "alq_balancing_select")
+        self._check(fn(self._h, C.byref(desc), self._stream()), "alq_" + name)
         if n_picks.value < 0:
             return None
-        np.random.set_state((name, key, int(pos_c.value), has_gauss, cached))
+        np.random.set_state((sname, key, int(pos_c.value), has_gauss, cached))
         return picks[:n_picks.value].cpu().numpy().astype(np.int64), int(n_bal.value)
 
     # -- K4 / K5 ---------------------------------------------------------------------------------------

@@ -16,8 +16,11 @@ identical; outside them the guarantee is "same pick unless the reference's own a
 
 When the engine offers `balancing_select` (K11) the whole query is one persistent launch instead: same branch test,
 same tie rule, NumPy's RNG advanced draw for draw on the device, class sums in fp64 in a fixed order.  The engine
-declines (returns None) under option "balancing_loop" = 1 or beyond the loop's limits (centres in shared memory, counts
-plus budget below 2^24); the step loop below then runs unchanged.
+declines (returns None) under option "balancing_loop" = 1 or 3 or beyond the loop's limits (centres in shared memory,
+counts plus budget below 2^24).  Then, when the engine also offers `balancing_table_select` (K12: the same query over an
+incremental fp64 row x class table, for class counts like ImageNet-LT's 1 000), that runs; it declines under option 1
+or 2 or beyond its own limits (per-class tables in shared memory, the table in free device memory).  Only when both
+decline does the step loop below run, unchanged.
 """
 from __future__ import annotations
 
@@ -59,9 +62,12 @@ class BalancingQuery(EngineMixin):
         if budget <= 0:
             return labeled_idxs_cur_rd, 0
         if hasattr(eng, "balancing_select"):
-            got = eng.balancing_select(emb, eng.row_norm2(emb), ys.to(device=dev, dtype=torch.int32),
-                                       torch.from_numpy(idxs_for_query.astype(np.uint8)).to(dev),
-                                       torch.from_numpy(idxs_labeled.astype(np.uint8)).to(dev), C, budget)
+            args = (emb, eng.row_norm2(emb), ys.to(device=dev, dtype=torch.int32),
+                    torch.from_numpy(idxs_for_query.astype(np.uint8)).to(dev),
+                    torch.from_numpy(idxs_labeled.astype(np.uint8)).to(dev), C, budget)
+            got = eng.balancing_select(*args)
+            if got is None and hasattr(eng, "balancing_table_select"):
+                got = eng.balancing_table_select(*args)
             if got is not None:
                 picks = list(got[0])
                 return picks, len(picks)

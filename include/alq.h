@@ -60,9 +60,10 @@ const char* alq_last_error(const alq_ctx* ctx);
  *   "spin_timeout_ms" how long a kernel waits for a peer GPU's flag before giving up with ALQ_ERR_STATE (default 20000)
  *   "select_impl"    0 auto | 1 multi-kernel radix select   | 2 single cluster-resident launch
  *   "base_impl"      0 auto | 1 sequential class loop       | 2 per-class candidate lists + in-order resolve
- *   "balancing_loop" 0 auto (the persistent loop whenever its limits hold) | 1 per-step path: alq_balancing_select declines
- *                    (n_picks_host = -1) and the caller runs its own step loop | 2 persistent loop, ALQ_ERR_INVALID naming
- *                    the limit when the shape is beyond it */
+ *   "balancing_loop" 0 auto (K11 whenever its limits hold, otherwise K12 whenever its limits hold, otherwise the caller's
+ *                    per-step path) | 1 per-step path: alq_balancing_select and alq_balancing_table_select decline
+ *                    (n_picks_host = -1) and the caller runs its own step loop | 2 K11, ALQ_ERR_INVALID naming the limit
+ *                    when the shape is beyond it; K12 declines | 3 K12, the same; K11 declines */
 int alq_set_option(alq_ctx* ctx, const char* key, int64_t value);
 /* Number of kernels this context has launched since creation (bench.py's `gpu_launches`). */
 int64_t alq_launch_count(const alq_ctx* ctx);
@@ -381,7 +382,7 @@ int alq_class_pick(alq_ctx* ctx, const int32_t* labels, const uint8_t* avail, in
  * Limits (option "balancing_loop"): every centre (4 c d bytes) plus the per-CTA tables fit the shared memory of one
  * CTA, and 1 KB per class for the fp64 set-up pass; at most 65 535 rows per CTA segment (n < 65 536 * SMs); every class
  * count plus the budget below 2^24 (the fp32 imbalance test is exact there).  Beyond them the call declines
- * (*n_picks_host = -1, nothing drawn) under option 0 or 1 and fails with ALQ_ERR_INVALID under option 2.
+ * (*n_picks_host = -1, nothing drawn) under option 0, 1 or 3 and fails with ALQ_ERR_INVALID under option 2.
  * Launches: K10's table pass (2), one segment count, two fp64 set-up passes and the loop: six, whatever the budget.
  * Synchronous (it reads the label check, the counts and the final RNG state back).                              */
 typedef struct alq_balancing_desc {
@@ -402,6 +403,29 @@ typedef struct alq_balancing_desc {
 } alq_balancing_desc;
 
 int alq_balancing_select(alq_ctx* ctx, const alq_balancing_desc* desc, void* stream);
+
+/* ---- K12: the same query at large class counts, over an incremental row x class table ----------------------------
+ * Same descriptor, same semantics and same outputs as alq_balancing_select (the branch test, numerator 1, NumPy's
+ * draws and state, the lowest row on ties, NaN ranked as alq_ratio_argmin ranks it, the label check); only the
+ * distance arithmetic differs, so that it does not need the C x d centres in shared memory.
+ * At the first balancing step every available row i gets a table row T[i, c] = <x_i, S_c> (fp64; S_c the fp64 sum of
+ * class c's labeled rows, in row order) and xn64_i = <x_i, x_i> (fp64).  A balancing step scores
+ *     d2(i, c) = xn64_i - 2 T[i, c] / den_c + q_c / den_c^2,   den_c = fl32(n_c + 1e-5),  q_c = <S_c, S_c> (fp64),
+ * which is |x_i - m_c|^2 for the unrounded centre m_c = S_c / den_c (K11 rounds the centre to fp32), and ranks
+ * the rows by (fl32(near / far), row) with the ratio formed in fp64 and rounded once.  After a pick p of class y every
+ * table row gets T[i, y] += <x_i, x_p> (fp64 sums of exact fp32 products in a fixed order), applied while the next
+ * balancing step streams the rows; a query that never balances builds no table.  The picks are bit-reproducible and
+ * do not depend on the grid; they differ from K11's or the per-step path's only where fp32 rounding decides the
+ * arg-min (two best ratios within about 1e-6 relative).
+ * Limits (option "balancing_loop"): the per-class tables (20 c bytes), the per-segment counts, the MT state and at
+ * least one pending row (4 d bytes) fit one CTA's shared memory; at most 65 535 rows per CTA segment; the labeled count
+ * plus the budget below 2^24; the table (8 n_avail c bytes) plus one copy of the fp64 class sums per CTA (8 c d grid
+ * bytes) fit the device's free memory, checked before any of it is reserved (the context's grow-only scratch keeps it
+ * after the call).  Beyond them the call declines (*n_picks_host = -1, nothing drawn) under option 0 and fails with
+ * ALQ_ERR_INVALID naming the limit under option 3; options 1 and 2 always decline.
+ * Launches: K10's table pass (2), one segment count, one grouping of the labeled rows by class, one class-sum pass and
+ * the loop: six, whatever the budget.  Synchronous.                                                               */
+int alq_balancing_table_select(alq_ctx* ctx, const alq_balancing_desc* desc, void* stream);
 
 #ifdef __cplusplus
 }
