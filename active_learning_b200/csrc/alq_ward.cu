@@ -2,23 +2,31 @@
 // (margin_clustering_sampler.py:59 under active_learning/src/query_strategies runs
 // sklearn.cluster.AgglomerativeClustering(n_clusters=20), i.e. scipy.cluster.hierarchy.ward over the full tree).
 //
-// K7 alq_pdist_f64   the full symmetric n x n fp64 matrix of scipy's pdist(X, 'euclidean'): fp32 rows widened to
-//                    fp64 (exact), s summed k = 0, 1, ... as `d = a - b; s = s + d*d` with no FMA, then sqrt(s).
-//                    One CTA owns a 64 x 64 tile of pairs of the upper triangle (each pair computed once, written to
-//                    (i, j) and (j, i)); 256 threads x 4 x 4 pairs in registers; k-chunks of both row blocks arrive
+// K7 alq_pdist_f64   scipy's pdist(X, 'euclidean') in fp64: fp32 rows widened to fp64 (exact), s summed k = 0, 1, ...
+//                    as `d = a - b; s = s + d*d` with no FMA, then sqrt(s).  Two layouts of the result (below).
+//                    One CTA owns a 64 x 64 tile of pairs of the upper triangle (each pair computed once; written to
+//                    (i, j) and (j, i) of the square matrix, or once to the condensed vector);
+//                    256 threads x 4 x 4 pairs in registers; k-chunks of both row blocks arrive
 //                    with 4-byte cp.async (any ld, any alignment, zero-filled past d and past n) into a two-stage fp32
 //                    ring and are widened once into an fp64 tile that the inner loop reads.
 // K8 alq_ward_nn_chain  scipy's nn_chain (Ward update) as ONE launch of one thread-block cluster (16 CTAs when the GPU
 //                    can place them, else 8).  CTA r owns columns [lo_r, hi_r) with their cluster sizes in shared
 //                    memory.  A scan of row x: per-CTA (value, lowest index) -> DSMEM exchange -> every CTA resolves
-//                    the same winner -> one cluster barrier.  A merge updates the CTA's slice of row y and the
-//                    mirrored entries D[i, y] of its rows, then one cluster barrier.
+//                    the same winner -> one cluster barrier.  A merge updates the CTA's slice of row y (and, in the
+//                    square layout, the mirrored entries D[i, y] of its rows), then one cluster barrier.
+//
+// Layouts of D (both kernels are templated on it; nothing else depends on it):
+//   square     the full symmetric n x n matrix, row-major with leading dimension ldd (8 n^2 bytes);
+//   condensed  scipy's pdist vector: (i, j), i < j, at n i - i (i + 1) / 2 + (j - i - 1) (4 n (n - 1) bytes).  Row x
+//              of the symmetric matrix is then the entries (j, x), j < x, one per row j (strided), and (x, j), j > x,
+//              contiguous.
 //
 // Memory ordering of K8 (entries of D written by one SM and read by another): every write happens before a
 // `barrier.cluster.arrive.release` of its CTA and every read after a `barrier.cluster.wait.acquire` of the reader;
 // all reads of D go through ld.global.cg (L2, never a possibly stale L1 line) and all writes through st.global.cg.
 //
-// Offsets into `dist` are int64 (n^2 passes 2^31 at n = 46 341); row indices themselves are int32.
+// Offsets into `dist` are int64 (n^2 passes 2^31 at n = 46 341, n (n - 1) / 2 at n = 65 537); row indices themselves
+// are int32.
 #include <cooperative_groups.h>
 #include <math_constants.h>
 
@@ -31,6 +39,24 @@
 namespace cg = cooperative_groups;
 
 namespace ward {
+
+// offset of (i, j), i < j, in the condensed vector
+__device__ __forceinline__ int64_t cidx(int i, int j, int n) {
+    return static_cast<int64_t>(n) * i - static_cast<int64_t>(i) * (i + 1) / 2 + (j - i - 1);
+}
+// row x's base: (x, j) sits at row + j -- for every j in the square layout, for j > x in the condensed one (where the
+// base itself may lie before D: only row + j, j > x, is ever dereferenced)
+template <bool CONDENSED>
+__device__ __forceinline__ int64_t row_off(int x, int n, int64_t ldd) {
+    if constexpr (CONDENSED) return cidx(x, x + 1, n) - (x + 1);
+    else return static_cast<int64_t>(x) * ldd;
+}
+// address of the symmetric entry (x, j), j != x, given row x's base
+template <bool CONDENSED, typename T>
+__device__ __forceinline__ T* at(double* D, T* row, int x, int j, int n) {
+    if constexpr (CONDENSED) return j < x ? D + cidx(j, x, n) : row + j;
+    else return row + j;
+}
 
 // ---------------------------------------------------------------------------------------------------------------
 // K7
@@ -47,6 +73,7 @@ __device__ __forceinline__ void cp_async4(void* smem, const void* gmem, bool pre
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
+template <bool CONDENSED>
 __global__ void __launch_bounds__(PD_THREADS, 2)
 pdist_f64_kernel(const float* __restrict__ x, int n, int d, int64_t ldx, double* __restrict__ dist, int64_t ldd) {
     const int ti = blockIdx.y, tj = blockIdx.x;
@@ -111,7 +138,9 @@ pdist_f64_kernel(const float* __restrict__ x, int n, int d, int64_t ldx, double*
 #pragma unroll
         for (int b = 0; b < 4; ++b) {
             const int j = row_j + tx + 16 * b;
-            if (i < n && j < n && (ti != tj || i <= j)) {
+            if constexpr (CONDENSED) {                     // no diagonal; consecutive tx: consecutive j
+                if (i < j && j < n) dist[cidx(i, j, n)] = __dsqrt_rn(acc[a][b]);
+            } else if (i < n && j < n && (ti != tj || i <= j)) {
                 const double v = __dsqrt_rn(acc[a][b]);
                 dist[static_cast<int64_t>(i) * ldd + j] = v;
                 dist[static_cast<int64_t>(j) * ldd + i] = v;
@@ -154,9 +183,10 @@ __device__ __forceinline__ double ward_update(double dxi, double dyi, double dxy
     return __dsqrt_rn(__dsub_rn(__dadd_rn(a, b), c));
 }
 
-// dist: n x n (ldd), consumed.  chain_all: [cluster size][n] int2 (index, cluster size), one stack per CTA (every CTA
+// dist: n x n (ldd) or condensed, consumed.  chain_all: [cluster size][n] int2 (index, cluster size), one stack per CTA (every CTA
 // walks the same chain; private copies need no cross-CTA ordering).  status: 0, or ALQ_ERR_NUMERIC if a scan of a
 // one-element chain found no finite candidate (non-finite distances).
+template <bool CONDENSED>
 __global__ void __launch_bounds__(NC_THREADS, 1)
 ward_chain_kernel(double* __restrict__ D, int n, int64_t ldd, int2* __restrict__ chain_all, int32_t* __restrict__ merge_xy,
                   double* __restrict__ merge_dist, int* __restrict__ status) {
@@ -196,7 +226,7 @@ ward_chain_kernel(double* __restrict__ D, int n, int64_t ldd, int2* __restrict__
 #pragma unroll 1
         while (true) {
             // ---- scan row x over this CTA's live columns -------------------------------------------------------
-            const double* row = D + static_cast<int64_t>(x) * ldd;
+            const double* row = D + row_off<CONDENSED>(x, n, ldd);
             Cand c{CUDART_INF, INT_MAX, 0};
             int i = lo + tid;
 #pragma unroll 1
@@ -207,7 +237,7 @@ ward_chain_kernel(double* __restrict__ D, int n, int64_t ldd, int2* __restrict__
                 for (int u = 0; u < 4; ++u) {
                     const int j = i + u * NC_THREADS;
                     live[u] = sz[j - lo] > 0 && j != x;
-                    v[u] = live[u] ? __ldcg(row + j) : CUDART_INF;
+                    v[u] = live[u] ? __ldcg(at<CONDENSED>(D, row, x, j, n)) : CUDART_INF;
                 }
 #pragma unroll
                 for (int u = 0; u < 4; ++u)
@@ -216,7 +246,7 @@ ward_chain_kernel(double* __restrict__ D, int n, int64_t ldd, int2* __restrict__
             for (; i < hi; i += NC_THREADS) {
                 const int s = sz[i - lo];
                 if (s > 0 && i != x) {
-                    const double v = __ldcg(row + i);
+                    const double v = __ldcg(at<CONDENSED>(D, row, x, i, n));
                     if (v < c.v) { c.v = v; c.i = i; c.s = s; }
                 }
             }
@@ -234,7 +264,7 @@ ward_chain_kernel(double* __restrict__ D, int n, int64_t ldd, int2* __restrict__
             if (lane < cs) m = *cluster.map_shared_rank(&part[par], lane);
             warp_cand_min(m);
             par ^= 1;                                      // part[par] is rewritten only after one more barrier
-            cur = p >= 0 ? __ldcg(row + p) : CUDART_INF;   // scipy starts from D[x, prev]: ties go to prev
+            cur = p >= 0 ? __ldcg(at<CONDENSED>(D, row, x, p, n)) : CUDART_INF;   // scipy starts from D[x, prev]: ties go to prev
             int y, ys;
             if (m.v < cur) { y = m.i; ys = m.s; cur = m.v; }
             else { y = p; ys = ps; }
@@ -257,14 +287,19 @@ ward_chain_kernel(double* __restrict__ D, int n, int64_t ldd, int2* __restrict__
             merge_xy[2 * static_cast<int64_t>(k) + 1] = b;
             merge_dist[k] = cur;
         }
-        const double* rowa = D + static_cast<int64_t>(a) * ldd;
-        double* rowb = D + static_cast<int64_t>(b) * ldd;
+        const double* rowa = D + row_off<CONDENSED>(a, n, ldd);
+        double* rowb = D + row_off<CONDENSED>(b, n, ldd);
         for (int i = lo + tid; i < hi; i += NC_THREADS) {
             const int ni = sz[i - lo];
             if (ni > 0 && i != a && i != b) {
-                const double v = ward_update(__ldcg(rowa + i), __ldcg(rowb + i), cur, na, nb, ni);
-                __stcg(rowb + i, v);
-                __stcg(D + static_cast<int64_t>(i) * ldd + b, v);
+                if constexpr (CONDENSED) {                 // one store per (i, b)
+                    double* bi = at<CONDENSED>(D, rowb, b, i, n);
+                    __stcg(bi, ward_update(__ldcg(at<CONDENSED>(D, rowa, a, i, n)), __ldcg(bi), cur, na, nb, ni));
+                } else {                                   // row b and the mirrored column
+                    const double v = ward_update(__ldcg(rowa + i), __ldcg(rowb + i), cur, na, nb, ni);
+                    __stcg(rowb + i, v);
+                    __stcg(D + static_cast<int64_t>(i) * ldd + b, v);
+                }
             }
         }
         __syncthreads();
@@ -284,9 +319,11 @@ ward_chain_kernel(double* __restrict__ D, int n, int64_t ldd, int2* __restrict__
     }
 }
 
+template <bool CONDENSED>
 int ward_cluster_size(alq_ctx* ctx, size_t smem, int* out) {
-    ALQ_CUDA(ctx, cudaFuncSetAttribute(ward_chain_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
-    ALQ_CUDA(ctx, cudaFuncSetAttribute(ward_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+    auto* kern = ward_chain_kernel<CONDENSED>;
+    ALQ_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    ALQ_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
     for (int cs : {16, 8}) {
         cudaLaunchConfig_t cfg = {};
         cfg.gridDim = dim3(cs);
@@ -300,7 +337,7 @@ int ward_cluster_size(alq_ctx* ctx, size_t smem, int* out) {
         cfg.attrs = &attr;
         cfg.numAttrs = 1;
         int nclusters = 0;
-        if (cudaOccupancyMaxActiveClusters(&nclusters, ward_chain_kernel, &cfg) == cudaSuccess && nclusters > 0) {
+        if (cudaOccupancyMaxActiveClusters(&nclusters, kern, &cfg) == cudaSuccess && nclusters > 0) {
             *out = cs;
             return ALQ_OK;
         }
@@ -367,37 +404,29 @@ void heap_pushpop(std::vector<int64_t>& h, int64_t item) {
     }
 }
 
-}  // namespace ward
-
-using namespace ward;
-
-extern "C" int alq_pdist_f64(alq_ctx* ctx, const float* x, int64_t n, int32_t d, int64_t ldx, double* dist, int64_t ldd,
-                             void* stream) {
-    if (!ctx) return ALQ_ERR_INVALID;
-    if (!x || !dist || n < 1 || d < 1 || ldx < d || ldd < n)
-        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_pdist_f64: bad arguments (n=%lld d=%d ldx=%lld ldd=%lld)", (long long)n, d,
-                 (long long)ldx, (long long)ldd);
+// K7 / K8 launches for either layout; `name` is the entry point's, for its error messages
+template <bool CONDENSED>
+int pdist_run(alq_ctx* ctx, const char* name, const float* x, int64_t n, int32_t d, int64_t ldx, double* dist, int64_t ldd,
+              void* stream) {
     const int64_t nt = (n + PD_TILE - 1) / PD_TILE;
-    if (nt > 65535) ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_pdist_f64: n=%lld exceeds %d rows", (long long)n, 65535 * PD_TILE);
+    if (nt > 65535) ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: n=%lld exceeds %d rows", name, (long long)n, 65535 * PD_TILE);
     ALQ_CUDA(ctx, cudaSetDevice(ctx->device));
-    pdist_f64_kernel<<<dim3(static_cast<unsigned>(nt), static_cast<unsigned>(nt)), PD_THREADS, 0,
-                       static_cast<cudaStream_t>(stream)>>>(x, static_cast<int>(n), d, ldx, dist, ldd);
+    pdist_f64_kernel<CONDENSED><<<dim3(static_cast<unsigned>(nt), static_cast<unsigned>(nt)), PD_THREADS, 0,
+                                  static_cast<cudaStream_t>(stream)>>>(x, static_cast<int>(n), d, ldx, dist, ldd);
     ALQ_LAUNCH_CHECK(ctx);
     return ALQ_OK;
 }
 
-extern "C" int alq_ward_nn_chain(alq_ctx* ctx, double* dist, int64_t n, int64_t ldd, int32_t* merge_xy, double* merge_dist,
-                                 void* stream) {
-    if (!ctx) return ALQ_ERR_INVALID;
-    if (!dist || !merge_xy || !merge_dist || n < 2 || n >= (1LL << 31) - 1 || ldd < n)
-        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_ward_nn_chain: bad arguments (n=%lld ldd=%lld)", (long long)n, (long long)ldd);
+template <bool CONDENSED>
+int nn_chain_run(alq_ctx* ctx, const char* name, double* dist, int64_t n, int64_t ldd, int32_t* merge_xy,
+                 double* merge_dist, void* stream) {
     ALQ_CUDA(ctx, cudaSetDevice(ctx->device));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const size_t smem = static_cast<size_t>((n + 7) / 8) * sizeof(int) + 16;   // sized for the 8-CTA fallback
     if (smem + 4096 > ctx->smem_optin)
-        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_ward_nn_chain: n=%lld does not fit the shared memory of a cluster", (long long)n);
+        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: n=%lld does not fit the shared memory of a cluster", name, (long long)n);
     int cs = 0;
-    int rc = ward_cluster_size(ctx, smem, &cs);
+    int rc = ward_cluster_size<CONDENSED>(ctx, smem, &cs);
     if (rc) return rc;
     rc = alq_scratch_reserve(ctx, scratch_need({static_cast<size_t>(cs) * n * sizeof(int2), sizeof(int)}));
     if (rc) return rc;
@@ -418,13 +447,52 @@ extern "C" int alq_ward_nn_chain(alq_ctx* ctx, double* dist, int64_t n, int64_t 
     attr.val.clusterDim.z = 1;
     cfg.attrs = &attr;
     cfg.numAttrs = 1;
-    ALQ_CUDA(ctx, cudaLaunchKernelEx(&cfg, ward_chain_kernel, dist, static_cast<int>(n), ldd, chain, merge_xy, merge_dist, status));
+    ALQ_CUDA(ctx, cudaLaunchKernelEx(&cfg, ward_chain_kernel<CONDENSED>, dist, static_cast<int>(n), ldd, chain, merge_xy,
+                                     merge_dist, status));
     ALQ_LAUNCH_CHECK(ctx);
     int h_status = 0;
     ALQ_CUDA(ctx, cudaMemcpyAsync(&h_status, status, sizeof(int), cudaMemcpyDeviceToHost, st));
     ALQ_CUDA(ctx, cudaStreamSynchronize(st));
-    if (h_status) ALQ_FAIL(ctx, ALQ_ERR_NUMERIC, "alq_ward_nn_chain: a chain scan found no finite distance (non-finite input)");
+    if (h_status) ALQ_FAIL(ctx, ALQ_ERR_NUMERIC, "%s: a chain scan found no finite distance (non-finite input)", name);
     return ALQ_OK;
+}
+
+}  // namespace ward
+
+using namespace ward;
+
+extern "C" int alq_pdist_f64(alq_ctx* ctx, const float* x, int64_t n, int32_t d, int64_t ldx, double* dist, int64_t ldd,
+                             void* stream) {
+    if (!ctx) return ALQ_ERR_INVALID;
+    if (!x || !dist || n < 1 || d < 1 || ldx < d || ldd < n)
+        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_pdist_f64: bad arguments (n=%lld d=%d ldx=%lld ldd=%lld)", (long long)n, d,
+                 (long long)ldx, (long long)ldd);
+    return pdist_run<false>(ctx, "alq_pdist_f64", x, n, d, ldx, dist, ldd, stream);
+}
+
+extern "C" int alq_pdist_f64_condensed(alq_ctx* ctx, const float* x, int64_t n, int32_t d, int64_t ldx, double* dist,
+                                       void* stream) {
+    if (!ctx) return ALQ_ERR_INVALID;
+    if (!x || !dist || n < 1 || d < 1 || ldx < d)
+        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_pdist_f64_condensed: bad arguments (n=%lld d=%d ldx=%lld)", (long long)n, d,
+                 (long long)ldx);
+    return pdist_run<true>(ctx, "alq_pdist_f64_condensed", x, n, d, ldx, dist, 0, stream);
+}
+
+extern "C" int alq_ward_nn_chain(alq_ctx* ctx, double* dist, int64_t n, int64_t ldd, int32_t* merge_xy, double* merge_dist,
+                                 void* stream) {
+    if (!ctx) return ALQ_ERR_INVALID;
+    if (!dist || !merge_xy || !merge_dist || n < 2 || n >= (1LL << 31) - 1 || ldd < n)
+        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_ward_nn_chain: bad arguments (n=%lld ldd=%lld)", (long long)n, (long long)ldd);
+    return nn_chain_run<false>(ctx, "alq_ward_nn_chain", dist, n, ldd, merge_xy, merge_dist, stream);
+}
+
+extern "C" int alq_ward_nn_chain_condensed(alq_ctx* ctx, double* dist, int64_t n, int32_t* merge_xy, double* merge_dist,
+                                           void* stream) {
+    if (!ctx) return ALQ_ERR_INVALID;
+    if (!dist || !merge_xy || !merge_dist || n < 2 || n >= (1LL << 31) - 1)
+        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_ward_nn_chain_condensed: bad arguments (n=%lld)", (long long)n);
+    return nn_chain_run<true>(ctx, "alq_ward_nn_chain_condensed", dist, n, 0, merge_xy, merge_dist, stream);
 }
 
 extern "C" int alq_ward_labels(const int32_t* merge_xy_host, const double* merge_dist_host, int64_t n, int32_t n_clusters,

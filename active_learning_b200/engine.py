@@ -8,6 +8,7 @@ path here: constructing an Engine without a usable GPU + libalq.so raises.
 from __future__ import annotations
 
 import ctypes as C
+import math
 from typing import Optional, Sequence
 
 import numpy as np
@@ -324,10 +325,23 @@ class Engine:
     # -- K7 / K8: Ward clustering (MarginClusteringSampler) ---------------------------------------------
     WARD_HEADROOM_BYTES = 1 << 30     # the chain scratch, the merge list and whatever else the query holds
 
-    def pdist(self, x: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """K7: the n x n fp64 matrix of scipy's pdist(x, 'euclidean') (bit for bit; diagonal 0)."""
+    def pdist(self, x: torch.Tensor, out: Optional[torch.Tensor] = None, condensed: bool = False) -> torch.Tensor:
+        """K7: scipy's pdist(x, 'euclidean') bit for bit.  By default the n x n fp64 matrix (diagonal 0); with
+        condensed=True scipy's own 1-D layout, n (n - 1) / 2 entries with (i, j), i < j, at n i - i (i + 1) / 2 + j - i - 1
+        (half the memory; `out` may be longer, its tail is left untouched)."""
         x = _f32c(x, "x")
         n, d = x.shape
+        if condensed:
+            m = n * (n - 1) // 2
+            if out is None:
+                out = torch.empty(max(m, 1), dtype=torch.float64, device=x.device)[:m]
+            if not out.is_cuda or out.dtype != torch.float64 or out.dim() != 1 or out.shape[0] < m or out.stride(0) != 1:
+                raise AlqError(f"pdist: a condensed out must be a contiguous 1-D float64 CUDA tensor of at least {m} "
+                               f"entries")
+            if m:
+                self._check(self.lib.alq_pdist_f64_condensed(self._h, _ptr(x), n, d, _ld(x), _ptr(out), self._stream()),
+                            "alq_pdist_f64_condensed")
+            return out
         if out is None:
             out = torch.empty((n, n), dtype=torch.float64, device=x.device)
         if out.dtype != torch.float64 or out.dim() != 2 or out.shape[0] < n or out.shape[1] < n or out.stride(1) != 1:
@@ -336,49 +350,91 @@ class Engine:
                     "alq_pdist_f64")
         return out
 
+    @staticmethod
+    def condensed_rows(length: int) -> int:
+        """n such that n (n - 1) / 2 == length; AlqError if there is none."""
+        length = int(length)
+        n = (1 + math.isqrt(1 + 8 * length)) // 2 if length >= 0 else 0
+        if n < 2 or n * (n - 1) // 2 != length:
+            raise AlqError(f"nn_chain: a condensed distance vector has n (n - 1) / 2 entries for some n >= 2, got {length}")
+        return n
+
     def nn_chain(self, dist: torch.Tensor, n: Optional[int] = None):
         """K8: scipy's Ward nn_chain over `dist` (consumed).  (merge_xy [n-1, 2] int32 with x < y, merge_dist [n-1]
-        fp64) on the device, in the chain's discovery order.  `dist` is a row-major float64 CUDA matrix of at least
-        n x n (n defaults to its row count).  Synchronous; AlqError (ALQ_ERR_NUMERIC) if a scan meets no finite
-        distance."""
-        if not dist.is_cuda or dist.dtype != torch.float64 or dist.dim() != 2 or dist.stride(1) != 1:
-            raise AlqError("nn_chain: dist must be a row-major float64 CUDA matrix")
-        n = dist.shape[0] if n is None else int(n)
-        if n < 2 or dist.shape[0] < n or dist.shape[1] < n or dist.stride(0) < n:
-            raise AlqError(f"nn_chain: need n >= 2 and a matrix of at least n x n, got n={n} for {tuple(dist.shape)} "
-                           f"with row stride {dist.stride(0)}")
+        fp64) on the device, in the chain's discovery order.  `dist` is either a row-major float64 CUDA matrix of at
+        least n x n (n defaults to its row count) or scipy's condensed vector, a contiguous 1-D float64 CUDA tensor of
+        exactly n (n - 1) / 2 entries (n is inferred from its length).  Synchronous; AlqError (ALQ_ERR_NUMERIC) if a scan
+        meets no finite distance."""
+        if dist.dim() == 1:
+            if not dist.is_cuda or dist.dtype != torch.float64 or dist.stride(0) != 1:
+                raise AlqError("nn_chain: a condensed dist must be a contiguous 1-D float64 CUDA tensor")
+            m = self.condensed_rows(dist.shape[0])
+            if n is not None and int(n) != m:
+                raise AlqError(f"nn_chain: n={n} does not match a condensed vector of {dist.shape[0]} entries (n={m})")
+            n = m
+        else:
+            if not dist.is_cuda or dist.dtype != torch.float64 or dist.dim() != 2 or dist.stride(1) != 1:
+                raise AlqError("nn_chain: dist must be a row-major float64 CUDA matrix")
+            n = dist.shape[0] if n is None else int(n)
+            if n < 2 or dist.shape[0] < n or dist.shape[1] < n or dist.stride(0) < n:
+                raise AlqError(f"nn_chain: need n >= 2 and a matrix of at least n x n, got n={n} for {tuple(dist.shape)} "
+                               f"with row stride {dist.stride(0)}")
         xy = torch.empty((max(n - 1, 1), 2), dtype=torch.int32, device=dist.device)
         md = torch.empty(max(n - 1, 1), dtype=torch.float64, device=dist.device)
-        self._check(self.lib.alq_ward_nn_chain(self._h, _ptr(dist), n, dist.stride(0), _ptr(xy), _ptr(md), self._stream()),
-                    "alq_ward_nn_chain")
+        if dist.dim() == 1:
+            self._check(self.lib.alq_ward_nn_chain_condensed(self._h, _ptr(dist), n, _ptr(xy), _ptr(md), self._stream()),
+                        "alq_ward_nn_chain_condensed")
+        else:
+            self._check(self.lib.alq_ward_nn_chain(self._h, _ptr(dist), n, dist.stride(0), _ptr(xy), _ptr(md),
+                                                   self._stream()), "alq_ward_nn_chain")
         return xy[:n - 1], md[:n - 1]
 
-    def ward_bytes(self, n: int) -> int:
-        """Device memory a Ward tree over n rows needs: the 8 n^2 distance matrix plus headroom."""
-        return 8 * int(n) * int(n) + self.WARD_HEADROOM_BYTES
+    @classmethod
+    def ward_bytes(cls, n: int) -> int:
+        """Device memory a Ward tree over n rows needs in the square layout: the 8 n^2 distance matrix plus headroom."""
+        return 8 * int(n) * int(n) + cls.WARD_HEADROOM_BYTES
 
-    def _ward_guard(self, n: int):
+    @classmethod
+    def ward_condensed_bytes(cls, n: int) -> int:
+        """The same in the condensed layout: scipy's 4 n (n - 1) byte distance vector plus headroom."""
+        return 4 * int(n) * (int(n) - 1) + cls.WARD_HEADROOM_BYTES
+
+    @classmethod
+    def ward_layout(cls, n: int, free_bytes: int) -> str:
+        """'square' whenever the n x n matrix fits `free_bytes` (it is the faster layout where both fit; see DESIGN),
+        else 'condensed' when the vector does, else AlqError naming n and both byte counts."""
+        if cls.ward_bytes(n) <= free_bytes:
+            return "square"
+        if cls.ward_condensed_bytes(n) <= free_bytes:
+            return "condensed"
+        raise AlqError(f"ward: n={n} rows need {cls.ward_bytes(n)} bytes of device memory as the n x n matrix (8 n^2) "
+                       f"or {cls.ward_condensed_bytes(n)} as scipy's condensed vector (4 n (n - 1)), each with "
+                       f"{cls.WARD_HEADROOM_BYTES} headroom; {free_bytes} are free; use a smaller subset_unlabeled")
+
+    def _ward_free_bytes(self) -> int:
+        """Device memory a Ward query can take: free on the device plus what torch's allocator caches unused."""
         free, _total = torch.cuda.mem_get_info(self.device)
-        cached = torch.cuda.memory_reserved(self.device) - torch.cuda.memory_allocated(self.device)
-        need = self.ward_bytes(n)
-        if need > free + cached:
-            raise AlqError(f"ward: n={n} rows need {need} bytes of device memory (8 * n^2 for the distance matrix plus "
-                           f"{self.WARD_HEADROOM_BYTES} headroom), {free + cached} are free; use a smaller subset_unlabeled")
+        return free + torch.cuda.memory_reserved(self.device) - torch.cuda.memory_allocated(self.device)
+
+    def _ward_guard(self, n: int) -> str:
+        return self.ward_layout(n, self._ward_free_bytes())
 
     def ward_tree(self, x: torch.Tensor):
         """scipy.cluster.hierarchy.ward(x)'s merges before its sort: (merge_xy [n-1, 2] int32, merge_dist [n-1] fp64) as
         host arrays, in discovery order.  Checks the device memory first and never attempts an allocation that cannot
-        fit; there is no CPU fallback.  ValueError for fewer than 2 rows or non-finite rows.  The 8 n^2 matrix is
-        returned to the device before this returns (torch.cuda.empty_cache, which also releases the process's other
-        unused cached blocks): at 80 000 rows it is 51.2 GB that the caching allocator would otherwise keep."""
+        fit; there is no CPU fallback.  The distances are the n x n matrix when it fits and scipy's condensed vector
+        (half the bytes) when only that fits; the merges are the same either way.  ValueError for fewer than 2 rows or
+        non-finite rows.  The distances are returned to the device before this returns (torch.cuda.empty_cache, which
+        also releases the process's other unused cached blocks): at 80 000 rows the matrix is 51.2 GB that the caching
+        allocator would otherwise keep."""
         x = _f32c(x, "x")
         n = x.shape[0]
         if n < 2:
             raise ValueError(f"ward needs at least 2 rows, got {n}")
-        self._ward_guard(n)
+        layout = self._ward_guard(n)
         if not bool(torch.isfinite(x).all()):
             raise ValueError("ward: the embeddings contain NaN or infinity")
-        dist = self.pdist(x)
+        dist = self.pdist(x, condensed=layout == "condensed")
         try:
             xy, md = self.nn_chain(dist, n)
             xy, md = xy.cpu().numpy(), md.cpu().numpy()

@@ -4,9 +4,12 @@ active_learning/src/query_strategies (https://arxiv.org/abs/2107.14263).
 The reference clusters the pool embeddings with sklearn's AgglomerativeClustering(n_clusters=20) -- Ward linkage over
 the full tree: scipy's single-threaded pdist (a 25.6 GB condensed matrix at 80 000 rows) and nn_chain on the host --
 then picks round-robin over the clusters, smallest cluster first, the smallest-margin row left in each.  Here one
-pool forward yields logits and embeddings, K1 scores the margins, K7 builds the fp64 distance matrix in HBM and K8
-walks the nearest-neighbour chain in one launch; the merge tree is scipy's bit for bit, so the labels are sklearn's
-(include/alq.h).  The round robin is O(n log n) host NumPy over n margins.
+pool forward yields logits and embeddings, K1 scores the margins, K7 builds the fp64 distances in HBM and K8 walks the
+nearest-neighbour chain in one launch; the merge tree is scipy's bit for bit, so the labels are sklearn's
+(include/alq.h).  The distances are the n x n matrix (8 n^2 bytes) when it fits the free device memory and scipy's
+condensed vector (4 n (n - 1) bytes) otherwise, so on an 80 GB card the limit is about 140 000 rows (computed from the
+card's memory, not measured), enough for ImageNet-LT's whole train set with subset_unlabeled unset; beyond it the query
+raises AlqError.  The round robin is O(n log n) host NumPy over n margins.
 """
 from __future__ import annotations
 

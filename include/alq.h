@@ -10,7 +10,7 @@
  *   - Return value: ALQ_OK (0) or an ALQ_ERR_* code; `alq_last_error(ctx)` describes the failure.
  *   - All arithmetic is IEEE fp32 (fp64 only for the inverse-CDF search and the Ward clustering, K7/K8; K3 and K9
  *     contract on the tensor cores as 3xTF32, fp32 to about 2^-21 per product); index math is int32 on the device
- *     (n < 2^31), except the int64 offsets into K7/K8's n x n matrix.  There is no CPU fallback anywhere in this library.
+ *     (n < 2^31), except the int64 offsets into K7/K8's distances.  There is no CPU fallback anywhere in this library.
  *   - Matrices are row-major with an explicit leading dimension (`ld*`, in elements).  The fast
  *     paths need the base pointer 16-byte aligned and ld % 4 == 0.
  */
@@ -306,10 +306,18 @@ int alq_base_select(alq_ctx* ctx, const float* min_margin, const float* radius, 
  *   n = 80 000), so the caller frees it when the query ends (Engine.ward_tree hands it back to the device) and it
  *   never sits in the grow-only arena.  Offsets into `dist` are
  *   int64 -- the one exception to the int32 index rule above (n^2 passes 2^31 at n = 46 341).
+ * alq_pdist_f64_condensed (K7, condensed layout): the same distances, bit for bit, written only once each into
+ *   scipy's condensed vector -- pdist's own output: (i, j), i < j, at dist[n*i - i*(i+1)/2 + (j - i - 1)], n (n - 1) / 2
+ *   entries (4 n (n - 1) bytes, half the square matrix: 25.6 GB at n = 80 000, 53.7 GB at n = 115 846).  Nothing past
+ *   them is written.  Same arguments, limits and caller-owned buffer as alq_pdist_f64, without ldd.  Offsets are
+ *   int64 (the vector passes 2^31 entries at n = 65 537).
  * alq_ward_nn_chain (K8): scipy's nn_chain with the Ward update, in ONE launch of one thread-block cluster, consuming
  *   `dist` in place (its contents are unspecified afterwards).  merge_xy[k] = (x, y) with x < y and merge_dist[k], for
  *   k < n - 1, in the chain's discovery order (before scipy's sort).  n >= 2.  Synchronous; ALQ_ERR_NUMERIC if a scan
  *   found no finite distance (non-finite input).
+ * alq_ward_nn_chain_condensed (K8, condensed layout): the same walk and the same merge list, bit for bit, over a
+ *   condensed vector of n (n - 1) / 2 entries (as alq_pdist_f64_condensed writes it), consumed in place.  Same
+ *   arguments and contract as alq_ward_nn_chain, without ldd.
  * alq_ward_labels: host-only, needs no GPU.  From K8's merge list: the stable sort by distance and scipy's union-find
  *   relabelling (hierarchy.ward's Z), then sklearn's _hc_cut(n_clusters): labels_host[0..n) in [0, n_clusters),
  *   numbered in the order of the cut's final heap.  ALQ_ERR_INVALID if n_clusters > n, or if the list is not a merge
@@ -319,6 +327,9 @@ int alq_pdist_f64(alq_ctx* ctx, const float* x, int64_t n, int32_t d, int64_t ld
                   void* stream);
 int alq_ward_nn_chain(alq_ctx* ctx, double* dist, int64_t n, int64_t ldd, int32_t* merge_xy, double* merge_dist,
                       void* stream);
+int alq_pdist_f64_condensed(alq_ctx* ctx, const float* x, int64_t n, int32_t d, int64_t ldx, double* dist, void* stream);
+int alq_ward_nn_chain_condensed(alq_ctx* ctx, double* dist, int64_t n, int32_t* merge_xy, double* merge_dist,
+                                void* stream);
 int alq_ward_labels(const int32_t* merge_xy_host, const double* merge_dist_host, int64_t n, int32_t n_clusters,
                     int32_t* labels_host);
 

@@ -1,16 +1,21 @@
-"""Ward clustering of MarginClusteringSampler on the H100: K7 (fp64 distance matrix), K8 (nearest-neighbour chain) and
-the host cut (alq_ward_labels), timed separately, and sklearn on the host for comparison.
+"""Ward clustering of MarginClusteringSampler on the H100: K7 (fp64 distances), K8 (nearest-neighbour chain) and the
+host cut (alq_ward_labels), timed separately, in either distance layout, and sklearn on the host for comparison.
 
-    python tools/hac_time.py [--sizes 20000 40000 80000] [--sklearn 10000 20000] [--d 2048] [--out FILE]
+    python tools/hac_time.py [--sizes 20000 40000 80000 104262 115846] [--layout square|condensed|both]
+                             [--sklearn 10000 20000] [--d 2048] [--out FILE]
 
-Rows are post-ReLU Gaussians (what a ResNet's pooled features look like).  After a warm-up at a small size, each size
-runs K7 + K8 `--repeats` times into one n x n matrix allocated outside the timed windows; CUDA events around each call
-give min / median / max.  The K8 window also holds the entry point's host-side set-up before the launch and its 4-byte
-status read-back after it (microseconds), so one more repetition under torch.profiler reports both kernels' device
-time alone.  The host cut is timed with a wall clock.  K7's rate counts 3 fp64 operations (sub, mul, add) per
-pair and dimension, n (n - 1) / 2 * d pairs-dimensions, against the H100 SXM data sheet's FP64 (non-tensor) peak of
-34 TFLOP/s -- which counts an FMA as two operations; K7 may not fuse, so its instruction-bound ceiling is half of that.
-K8 is reported per merge (n - 1 of them) and per chain push (2 (n - 1)).  For the sklearn sizes the GPU labels must equal
+Rows are post-ReLU Gaussians (what a ResNet's pooled features look like).  After a warm-up at a small size in every
+layout, each size runs K7 + K8 `--repeats` times per layout; `both` alternates the square n x n matrix and scipy's
+condensed vector within each repetition, in one process.  A layout whose buffer (plus Engine.WARD_HEADROOM_BYTES) does
+not fit the free device memory is left out at that size: on an 80 GB card 104 262 and 115 846 rows (ImageNet-LT's
+available rows at 10 % labeled, and its whole train set) run condensed only.  The buffer is allocated before each
+repetition and freed after it, outside the timed windows; CUDA events around each call give min / median / max.  The K8
+window also holds the entry point's host-side set-up before the launch and its 4-byte status read-back after it
+(microseconds), so one more repetition per layout under torch.profiler reports both kernels' device time alone.  The
+host cut is timed with a wall clock.  K7's rate counts 3 fp64 operations (sub, mul, add) per pair and dimension,
+n (n - 1) / 2 * d pairs-dimensions, against the H100 SXM data sheet's FP64 (non-tensor) peak of 34 TFLOP/s -- which
+counts an FMA as two operations; K7 may not fuse, so its instruction-bound ceiling is half of that.  K8 is reported per
+merge (n - 1 of them) and per chain push (2 (n - 1)).  For the sklearn sizes the GPU labels must equal
 AgglomerativeClustering(n_clusters=20).fit(x).labels_.  Prints one JSON line per measurement and the card's name and
 power limit first.
 """
@@ -62,7 +67,8 @@ def kernel_ms(prof, name):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--sizes", type=int, nargs="*", default=[20000, 40000, 80000])
+    ap.add_argument("--sizes", type=int, nargs="*", default=[20000, 40000, 80000, 104262, 115846])
+    ap.add_argument("--layout", choices=["square", "condensed", "both"], default="both")
     ap.add_argument("--sklearn", type=int, nargs="*", default=[10000, 20000])
     ap.add_argument("--d", type=int, default=2048)
     ap.add_argument("--repeats", type=int, default=3)
@@ -72,47 +78,67 @@ def main():
     eng = Engine()
     results = [{"card": card(), "torch_device": torch.cuda.get_device_name()}]
     print(json.dumps(results[0]), flush=True)
+    layouts = ["square", "condensed"] if args.layout == "both" else [args.layout]
 
-    def tree(x, dist):
+    def alloc(n, layout):
+        shape = (n, n) if layout == "square" else (n * (n - 1) // 2,)
+        return torch.empty(shape, dtype=torch.float64, device="cuda")
+
+    def tree(x, layout):
         n = x.shape[0]
-        _, k7_ms = timed(lambda: eng.pdist(x, out=dist))
+        dist = alloc(n, layout)
+        _, k7_ms = timed(lambda: eng.pdist(x, out=dist, condensed=layout == "condensed"))
         (xy, md), k8_ms = timed(lambda: eng.nn_chain(dist, n))
+        del dist
+        torch.cuda.empty_cache()
         return xy, md, k7_ms, k8_ms
 
     x = rows(2000, args.d, 1)                              # warm-up: module load, cluster attributes, scratch
-    tree(x, torch.empty((2000, 2000), dtype=torch.float64, device="cuda"))
+    for layout in layouts:
+        tree(x, layout)
+    from torch.profiler import ProfilerActivity, profile
     for n in args.sizes:
-        eng._ward_guard(n)
         x = rows(n, args.d, n)
-        dist = torch.empty((n, n), dtype=torch.float64, device="cuda")
-        k7, k8 = [], []
+        free = eng._ward_free_bytes()
+        fits = [lay for lay in layouts
+                if (eng.ward_bytes(n) if lay == "square" else eng.ward_condensed_bytes(n)) <= free]
+        if not fits:
+            eng.ward_layout(n, free)                       # raises, naming n and both byte counts
+        k7 = {lay: [] for lay in fits}
+        k8 = {lay: [] for lay in fits}
+        merges = {}
         for _ in range(args.repeats):
-            xy, md, k7_ms, k8_ms = tree(x, dist)
-            k7.append(k7_ms)
-            k8.append(k8_ms)
-        xy, md = xy.cpu().numpy(), md.cpu().numpy()
-        t0 = time.perf_counter()
-        ward_labels_host(xy, md, n, 20)
-        cut_ms = (time.perf_counter() - t0) * 1e3
-        from torch.profiler import ProfilerActivity, profile
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            tree(x, dist)
-            torch.cuda.synchronize()
-        del dist
-        torch.cuda.empty_cache()
-        k7_med, k8_med = float(np.median(k7)), float(np.median(k8))
-        ops = 3.0 * n * (n - 1) / 2 * args.d
-        k7_kernel, k8_kernel = kernel_ms(prof, "pdist_f64_kernel"), kernel_ms(prof, "ward_chain_kernel")
-        rec = {"n": n, "d": args.d, "repeats": args.repeats,
-               "k7_ms_min_med_max": [round(min(k7), 2), round(k7_med, 2), round(max(k7), 2)],
-               "k7_kernel_ms_profiler": k7_kernel,
-               "k7_tflops": round(ops / k7_med / 1e9, 2), "k7_share_of_fp64_peak": round(ops / k7_med / 1e9 / FP64_PEAK_TFLOPS, 3),
-               "k8_ms_min_med_max": [round(min(k8), 2), round(k8_med, 2), round(max(k8), 2)],
-               "k8_kernel_ms_profiler": k8_kernel,
-               "k8_us_per_merge": round(k8_med * 1e3 / (n - 1), 3), "k8_us_per_push": round(k8_med * 1e3 / (2 * (n - 1)), 3),
-               "cut_ms": round(cut_ms, 2)}
-        results.append(rec)
-        print(json.dumps(rec), flush=True)
+            for lay in fits:
+                xy, md, k7_ms, k8_ms = tree(x, lay)
+                k7[lay].append(k7_ms)
+                k8[lay].append(k8_ms)
+                merges[lay] = (xy.cpu().numpy(), md.cpu().numpy())
+        for lay in fits:
+            xy, md = merges[lay]
+            t0 = time.perf_counter()
+            ward_labels_host(xy, md, n, 20)
+            cut_ms = (time.perf_counter() - t0) * 1e3
+            with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                tree(x, lay)
+                torch.cuda.synchronize()
+            k7_med, k8_med = float(np.median(k7[lay])), float(np.median(k8[lay]))
+            ops = 3.0 * n * (n - 1) / 2 * args.d
+            rec = {"n": n, "d": args.d, "layout": lay, "repeats": args.repeats,
+                   "k7_ms_min_med_max": [round(min(k7[lay]), 2), round(k7_med, 2), round(max(k7[lay]), 2)],
+                   "k7_kernel_ms_profiler": kernel_ms(prof, "pdist_f64_kernel"),
+                   "k7_tflops": round(ops / k7_med / 1e9, 2),
+                   "k7_share_of_fp64_peak": round(ops / k7_med / 1e9 / FP64_PEAK_TFLOPS, 3),
+                   "k8_ms_min_med_max": [round(min(k8[lay]), 2), round(k8_med, 2), round(max(k8[lay]), 2)],
+                   "k8_kernel_ms_profiler": kernel_ms(prof, "ward_chain_kernel"),
+                   "k8_us_per_merge": round(k8_med * 1e3 / (n - 1), 3),
+                   "k8_us_per_push": round(k8_med * 1e3 / (2 * (n - 1)), 3),
+                   "cut_ms": round(cut_ms, 2)}
+            if len(fits) == 2 and lay == "condensed":      # the two layouts walked the same tree
+                rec["merges_identical_to_square"] = bool(np.array_equal(xy, merges["square"][0])
+                                                         and np.array_equal(md, merges["square"][1]))
+            results.append(rec)
+            print(json.dumps(rec), flush=True)
+        del x
     if args.sklearn:
         from sklearn.cluster import AgglomerativeClustering
     for n in args.sklearn:
