@@ -64,6 +64,8 @@ class BalancingDesc(C.Structure):
         ("picks", C.c_void_p),
         ("n_picks_host", C.c_void_p),
         ("n_balancing_host", C.c_void_p),
+        ("shard_off_host", C.c_void_p),
+        ("group_free_bytes", C.c_int64),
     ]
 
 

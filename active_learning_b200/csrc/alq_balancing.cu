@@ -21,6 +21,9 @@
 // A row's dot product with a centre is a fixed function of that row: lane l accumulates the float4 chunks l, l + 32, ..
 // with fmaf in x, y, z, w order, and a butterfly folds the 32 partials (every lane ends with the same value).  Neither the
 // warp, nor the CTA, nor the grid size changes it, so the picks are bit-reproducible.
+// Sharded over a group (shard_off_host), the segments above are every rank's CTA segments (BalShard): every CTA of every
+// rank keeps all of their counts, the key words go into every rank's window and the owner of a random pick stores its
+// word there too; K12 shares the layout and the host steps below.
 #include <limits.h>
 
 #include "alq_balancing.cuh"
@@ -40,15 +43,15 @@ struct BalArgs {
     const double* sums0;         // [c][d] fp64 class sums of the labeled rows
     double* sums;                // [grid][c][d] every CTA's running copy
     const int* counts0;          // [c]
-    const int* seg_avail0;       // [grid]
+    const int* seg_avail0;       // [world * grid]
     const unsigned int* mt_in;   // [kMtN + 1]: key, pos
     unsigned int* mt_out;        // [kMtN + 1]
     int* picks;
     int* n_bal;
     int* status;
-    unsigned long long* keyw;    // [2][grid] LL words of the balancing steps (two parities)
-    unsigned long long* pickw;   // [budget]  LL word of each random step
-    int n, c, budget, grid, n_avail;
+    BalShard S;
+    BalWords W;                  // key words of the balancing steps (two parities), one pick word per random step
+    int n, c, budget, n_avail;
     long long timeout_cycles;
 };
 
@@ -70,12 +73,12 @@ __device__ __forceinline__ float dot_fixed(const float4* x, const float4* q, int
     return warp_sum(acc);
 }
 
-// available rows per CTA segment; the smallest available row with a label outside [0, c) -> *bad
+// available rows per global segment (one block each); the smallest available row with a label outside [0, c) -> *bad
 __global__ void __launch_bounds__(256) bal_seg_count_kernel(const int* __restrict__ labels, const uint8_t* __restrict__ avail,
-                                                            int n, int c, int grid, int* __restrict__ seg_avail,
+                                                            int c, const __grid_constant__ BalShard S, int* __restrict__ seg_avail,
                                                             unsigned int* __restrict__ bad) {
     __shared__ int wsum[8];
-    const int lo = seg_lo(n, grid, blockIdx.x), hi = seg_lo(n, grid, blockIdx.x + 1);
+    const int lo = gseg_lo(S, blockIdx.x), hi = gseg_lo(S, blockIdx.x + 1);
     int cnt = 0;
     for (int i = lo + threadIdx.x; i < hi; i += blockDim.x) {
         if (!avail[i]) continue;
@@ -140,30 +143,31 @@ __global__ void bal_class_sum_reduce_kernel(const double* __restrict__ partial, 
     sums0[i] = s;
 }
 
-__host__ __device__ __forceinline__ size_t bal_loop_smem(int c, int d, int grid) {
-    return static_cast<size_t>(c) * d * 4 + static_cast<size_t>(c) * 12 + static_cast<size_t>(grid) * 4 + kMtN * 4 + 64;
+__host__ __device__ __forceinline__ size_t bal_loop_smem(int c, int d, int nseg) {
+    return static_cast<size_t>(c) * d * 4 + static_cast<size_t>(c) * 12 + static_cast<size_t>(nseg) * 4 + kMtN * 4 + 64;
 }
 
 __global__ void __launch_bounds__(kBalThreads, 1) balancing_loop_kernel(const __grid_constant__ BalArgs A) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    const int c = A.c, d = A.d, dv = d >> 2, grid = A.grid;
+    const int c = A.c, d = A.d, dv = d >> 2, nseg = A.S.world * A.S.grid;
     float* cent = reinterpret_cast<float*>(smem_raw);                 // [c][d]
     float* cn = cent + static_cast<size_t>(c) * d;                    // [c]
     int* cnt = reinterpret_cast<int*>(cn + c);                        // [c]
     int* sel = cnt + c;                                               // [c]
-    int* seg_av = sel + c;                                            // [grid]
-    unsigned int* mt = reinterpret_cast<unsigned int*>(seg_av + grid);   // [kMtN]
+    int* seg_av = sel + c;                                            // [nseg]
+    unsigned int* mt = reinterpret_cast<unsigned int*>(seg_av + nseg);   // [kMtN]
     __shared__ unsigned long long s_key[kBalWarps];
     __shared__ int s_wc[kBalWarps];
     __shared__ int s_nsel, s_pick, s_owner, s_rank, s_found, s_mtpos, s_navail;
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int b = blockIdx.x;
-    const int row_lo = seg_lo(A.n, grid, b), row_hi = seg_lo(A.n, grid, b + 1);
+    const int gb = A.S.rank * A.S.grid + b;                           // my global segment
+    const int row_lo = gseg_lo(A.S, gb), row_hi = gseg_lo(A.S, gb + 1);
     double* my_sums = A.sums + static_cast<size_t>(b) * c * d;
 
     for (int i = tid; i < c; i += kBalThreads) cnt[i] = A.counts0[i];
-    for (int i = tid; i < grid; i += kBalThreads) seg_av[i] = A.seg_avail0[i];
+    for (int i = tid; i < nseg; i += kBalThreads) seg_av[i] = A.seg_avail0[i];
     for (int i = tid; i < kMtN; i += kBalThreads) mt[i] = A.mt_in[i];
     if (tid == 0) { s_mtpos = static_cast<int>(A.mt_in[kMtN]); s_navail = A.n_avail; }
     __syncthreads();
@@ -178,7 +182,7 @@ __global__ void __launch_bounds__(kBalThreads, 1) balancing_loop_kernel(const __
         const float v = dot_fixed(q, q, dv, lane);
         if (lane == 0) cn[k] = v;
     }
-    __syncthreads();
+    bal_ready_wait(A, tid);
 
     unsigned int rnd_key = 0;
     int n_bal = 0;
@@ -232,49 +236,21 @@ __global__ void __launch_bounds__(kBalThreads, 1) balancing_loop_kernel(const __
             }
             if (lane == 0) s_key[warp] = best;
             __syncthreads();
-            const unsigned int tag16 = 0x8000u | (++rnd_key & 0x7fffu);
-            char* const keyw = reinterpret_cast<char*>(A.keyw + static_cast<size_t>(rnd_key & 1u) * grid);
-            if (tid == 0) {
-                unsigned long long m = s_key[0];
-                for (int w = 1; w < kBalWarps; ++w) m = s_key[w] < m ? s_key[w] : m;
-                const unsigned long long off = m == ~0ull ? kEmptyOff : static_cast<unsigned long long>(static_cast<uint32_t>(m) - row_lo);
-                ll_store_raw(keyw + static_cast<size_t>(b) * 8, (static_cast<unsigned long long>(tag16) << 48) | (off << 32) | (m >> 32));
-            }
-            unsigned long long mine = ~0ull;
-            ll_gather(keyw, grid, 8, tag16, 48, A, tid, [&](int i, unsigned long long w) {
-                const unsigned int off = static_cast<unsigned int>(w >> 32) & 0xffffu;
-                if (off == kEmptyOff) return;
-                const unsigned long long key = ((w & 0xffffffffull) << 32) | static_cast<uint32_t>(seg_lo(A.n, grid, i) + static_cast<int>(off));
-                mine = key < mine ? key : mine;
-            });
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) {
-                const unsigned long long w = __shfl_xor_sync(0xffffffffu, mine, o);
-                mine = w < mine ? w : mine;
-            }
-            __syncthreads();                                              // s_key is reused
-            if (lane == 0) s_key[warp] = mine;
-            __syncthreads();
-            if (tid == 0) {
-                unsigned long long m = s_key[0];
-                for (int w = 1; w < kBalWarps; ++w) m = s_key[w] < m ? s_key[w] : m;
-                s_pick = m == ~0ull ? -1 : static_cast<int>(static_cast<uint32_t>(m));
-            }
-            __syncthreads();
+            bal_agree<kBalWarps>(A, s_key, &s_pick, ++rnd_key, row_lo, tid);
         } else {
             // ===== random step (balancing_sampler.py:128): np.random.choice over the available rows =====
             if (tid == 0) {
                 int k = static_cast<int>(mt_bounded(mt, s_mtpos, static_cast<unsigned int>(s_navail - 1)));
                 int o = 0;
-                while (o + 1 < grid && k >= seg_av[o]) { k -= seg_av[o]; ++o; }
+                while (o + 1 < nseg && k >= seg_av[o]) { k -= seg_av[o]; ++o; }
                 s_owner = o;
                 s_rank = k;
                 s_found = -1;
             }
             __syncthreads();
-            unsigned long long* const pw = A.pickw + t;
-            const unsigned int ptag = 0x80000000u | static_cast<unsigned int>(t);
-            if (s_owner == b) {                                           // the rank-th available row of this segment
+            const size_t pw = A.W.pickw + static_cast<size_t>(t) * 8;
+            const unsigned int ptag = bal_pick_tag(A.W, t);
+            if (s_owner == gb) {                                          // the rank-th available row of this segment
                 const int rank = s_rank;
                 int base = 0;
                 for (int r0 = row_lo; r0 < row_hi; r0 += kBalThreads) {
@@ -295,9 +271,9 @@ __global__ void __launch_bounds__(kBalThreads, 1) balancing_loop_kernel(const __
                     if (here) break;
                     base += tot;
                 }
-                if (tid == 0) ll_store(pw, ptag, static_cast<unsigned int>(s_found));
+                if (tid < A.S.world) ll_store(A.W.peer[tid] + pw, ptag, static_cast<unsigned int>(s_found));
             }
-            if (tid == 0) s_pick = static_cast<int>(ll_wait(pw, ptag, A));
+            if (tid == 0) s_pick = static_cast<int>(ll_wait(A.W.peer[A.S.rank] + pw, ptag, A));
             __syncthreads();
         }
 
@@ -309,15 +285,13 @@ __global__ void __launch_bounds__(kBalThreads, 1) balancing_loop_kernel(const __
         }
         const int cls = __ldg(A.labels + pick);
         const int newc = cnt[cls] + 1;
-        int o = static_cast<int>(static_cast<long long>(pick) * grid / A.n);
-        while (o + 1 < grid && seg_lo(A.n, grid, o + 1) <= pick) ++o;
-        while (o > 0 && seg_lo(A.n, grid, o) > pick) --o;
+        const int o = gseg_of(A.S, pick);
         __syncthreads();                                                 // cnt[cls] read by every thread
         if (tid == 0) {
             cnt[cls] = newc;
             seg_av[o] -= 1;
             s_navail -= 1;
-            if (o == b) A.avail[pick] = 0;
+            if (o == gb) A.avail[pick] = 0;
             if (b == 0) A.picks[t] = pick;
         }
         float* cc = cent + static_cast<size_t>(cls) * d;
@@ -341,10 +315,73 @@ __global__ void __launch_bounds__(kBalThreads, 1) balancing_loop_kernel(const __
     }
 }
 
+constexpr size_t kWordsHead = 128;               // u64 ready[ALQ_MAX_WORLD] in front of a window's words (greedy's layout)
+
+size_t up128(size_t v) { return (v + 127) & ~size_t(127); }
+
 }  // namespace
 
+// descriptors of the shorter, single-GPU layout end here
+constexpr size_t kBalDescV1 = offsetof(alq_balancing_desc, shard_off_host);
+
+int alq_bal_shard(alq_ctx* ctx, const alq_balancing_desc* D, int n, BalShard* S, bool* sharded, const char* fn) {
+    const int32_t* so = D->struct_size >= sizeof(alq_balancing_desc) ? D->shard_off_host : nullptr;
+    *sharded = so != nullptr;
+    S->world = 1;
+    S->rank = 0;
+    S->off[0] = 0;
+    S->off[1] = n;
+    if (so) {
+        const AlqComm& G = ctx->comm;
+        if (!G.window || !G.connected)
+            ALQ_FAIL(ctx, ALQ_ERR_STATE, "%s: a sharded call (shard_off_host) needs the group of alq_comm_create/connect", fn);
+        if (so[0] != 0 || so[G.world] != n)
+            ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: shard_off must run from 0 to n=%d, got %d .. %d", fn, n, so[0], so[G.world]);
+        for (int r = 0; r < G.world; ++r)
+            if (so[r + 1] < so[r]) ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: shard_off[%d] = %d < shard_off[%d] = %d", fn, r + 1, so[r + 1], r, so[r]);
+        S->world = G.world;
+        S->rank = G.rank;
+        std::copy(so, so + G.world + 1, S->off);
+    }
+    int rows_min = n;
+    for (int r = 0; r < S->world; ++r) rows_min = std::min(rows_min, S->off[r + 1] - S->off[r]);
+    S->grid = std::max(1, std::min(ctx->sm_count, (rows_min + 127) / 128));
+    return ALQ_OK;
+}
+
+int alq_bal_seg_rows_max(const BalShard& S) {
+    int m = 0;
+    for (int g = 0; g < S.world * S.grid; ++g) m = std::max(m, gseg_lo(S, g + 1) - gseg_lo(S, g));
+    return m;
+}
+
+size_t alq_bal_words_bytes(const BalShard& S, int64_t budget, bool sharded) {
+    const size_t keyw = sharded ? kWordsHead : 0;
+    return up128(keyw + static_cast<size_t>(2) * S.world * S.grid * 8) + static_cast<size_t>(budget) * 8;
+}
+
+int alq_bal_words_begin(alq_ctx* ctx, const BalShard& S, bool sharded, int budget, char* scratch, BalWords* W, cudaStream_t st) {
+    *W = BalWords{};
+    W->keyw = static_cast<unsigned int>(sharded ? kWordsHead : 0);
+    W->pickw = static_cast<unsigned int>(up128(W->keyw + static_cast<size_t>(2) * S.world * S.grid * 8));
+    const size_t end = alq_bal_words_bytes(S, budget, sharded);
+    W->tag_base = 0x80000000u;
+    if (!sharded) {
+        W->peer[0] = scratch;
+        ALQ_CUDA(ctx, cudaMemsetAsync(scratch, 0, end, st));
+        return ALQ_OK;
+    }
+    // the words start without a valid tag; peers write them only after our ready word, which follows the clear
+    ALQ_CUDA(ctx, cudaMemsetAsync(ctx->comm.window + kWordsHead, 0, end - kWordsHead, st));
+    for (int r = 0; r < S.world; ++r) W->peer[r] = ctx->comm.peer[r];
+    ctx->comm.epoch += 1;
+    W->ready_tag = ctx->comm.epoch << 32;
+    W->tag_base |= static_cast<unsigned int>(ctx->comm.epoch & 0x7fu) << 24;
+    return alq_comm_ready(ctx, W->ready_tag, st);
+}
+
 int alq_bal_check_desc(alq_ctx* ctx, const alq_balancing_desc* D, const char* fn) {
-    if (!D || D->struct_size < sizeof(alq_balancing_desc)) ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: bad descriptor", fn);
+    if (!D || D->struct_size < kBalDescV1) ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: bad descriptor", fn);
     const int64_t n64 = D->n;
     const int c = D->c, d = D->d;
     if (n64 < 0 || n64 >= (1LL << 31)) ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: n=%lld outside [0, 2^31)", fn, (long long)n64);
@@ -363,17 +400,18 @@ int alq_bal_check_desc(alq_ctx* ctx, const alq_balancing_desc* D, const char* fn
     return ALQ_OK;
 }
 
-int alq_bal_counts(alq_ctx* ctx, const alq_balancing_desc* D, int n, int c, int grid, int32_t* tab, unsigned int* bad,
+int alq_bal_counts(alq_ctx* ctx, const alq_balancing_desc* D, int n, int c, const BalShard& S, int32_t* tab, unsigned int* bad,
                    int32_t* counts, int32_t* seg_avail, int32_t* counts_h, int32_t* seg_h, cudaStream_t st, const char* fn) {
+    const int nseg = S.world * S.grid;
     ALQ_CUDA(ctx, cudaMemsetAsync(bad, 0xff, 2 * sizeof(unsigned int), st));
     const int rc = alq_class_table_pass(ctx, D->labels, D->labeled, n, c, tab, bad, counts, st);
     if (rc != ALQ_OK) return rc;
-    bal_seg_count_kernel<<<grid, 256, 0, st>>>(D->labels, D->avail, n, c, grid, seg_avail, bad + 1);
+    bal_seg_count_kernel<<<nseg, 256, 0, st>>>(D->labels, D->avail, c, S, seg_avail, bad + 1);
     ALQ_LAUNCH_CHECK(ctx);
     unsigned int bad_h[2] = {UINT_MAX, UINT_MAX};
     ALQ_CUDA(ctx, cudaMemcpyAsync(bad_h, bad, sizeof(bad_h), cudaMemcpyDeviceToHost, st));
     ALQ_CUDA(ctx, cudaMemcpyAsync(counts_h, counts, static_cast<size_t>(c) * 4, cudaMemcpyDeviceToHost, st));
-    ALQ_CUDA(ctx, cudaMemcpyAsync(seg_h, seg_avail, static_cast<size_t>(grid) * 4, cudaMemcpyDeviceToHost, st));
+    ALQ_CUDA(ctx, cudaMemcpyAsync(seg_h, seg_avail, static_cast<size_t>(nseg) * 4, cudaMemcpyDeviceToHost, st));
     ALQ_CUDA(ctx, cudaStreamSynchronize(st));
     for (int k = 1; k >= 0; --k)
         if (bad_h[k] != UINT_MAX) {
@@ -400,9 +438,13 @@ extern "C" int alq_balancing_select(alq_ctx* ctx, const alq_balancing_desc* D, v
     }
     const cudaStream_t st = static_cast<cudaStream_t>(stream);
 
-    // ---- limits that the shape decides --------------------------------------------------------------------------
-    const int grid = std::max(1, std::min(ctx->sm_count, (n + 127) / 128));
-    const size_t smem = bal_loop_smem(c, d, grid);
+    // ---- limits that the shape decides (the same on every rank of a sharded call) -------------------------------------
+    BalShard S;
+    bool sharded = false;
+    rc = alq_bal_shard(ctx, D, n, &S, &sharded, "alq_balancing_select");
+    if (rc != ALQ_OK) return rc;
+    const int grid = S.grid, nseg = S.world * grid;
+    const size_t smem = bal_loop_smem(c, d, nseg);
     const size_t sum_smem = static_cast<size_t>(c) * kSumDims * sizeof(double);
     const size_t smem_cap = ctx->smem_optin > 4096 ? ctx->smem_optin - 1024 : 0;   // the kernels' static shared memory
     if (smem > smem_cap || sum_smem > smem_cap) {
@@ -410,42 +452,46 @@ extern "C" int alq_balancing_select(alq_ctx* ctx, const alq_balancing_desc* D, v
         ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_balancing_select: the %d centres of %d floats need %zu bytes of shared memory, "
                  "%zu are available (limit: centres in shared memory)", c, d, std::max(smem, sum_smem), smem_cap);
     }
-    if (n - seg_lo(n, grid, grid - 1) > kSegRowsMax) {
+    if (alq_bal_seg_rows_max(S) > kSegRowsMax) {
         if (!forced) return ALQ_OK;
         ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_balancing_select: n=%d rows over %d CTAs exceed %d rows per CTA segment "
-                 "(limit: rows per segment)", n, grid, kSegRowsMax);
+                 "(limit: rows per segment)", n, nseg, kSegRowsMax);
+    }
+    const int64_t budget_req = D->budget;
+    const size_t words = alq_bal_words_bytes(S, std::min<int64_t>(budget_req, n), sharded);
+    if (sharded && words > ctx->comm.greedy_bytes()) {
+        if (!forced) return ALQ_OK;
+        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_balancing_select: a budget of %lld needs %zu bytes of the peer window, %zu are "
+                 "usable (limit: words in the peer window)", (long long)budget_req, words, ctx->comm.greedy_bytes());
     }
 
     // ---- set-up: counts, segment counts, label checks -----------------------------------------------------------
     const int nchunks = (n + kSumChunk - 1) / kSumChunk;
     const size_t cd = static_cast<size_t>(c) * d;
     const size_t entries = alq_class_table_entries(n, c);
-    const int64_t budget_req = D->budget;
-    const size_t need = scratch_need({entries * 4, static_cast<size_t>(c) * 4, 8, static_cast<size_t>(grid) * 4,
+    const size_t need = scratch_need({entries * 4, static_cast<size_t>(c) * 4, 8, static_cast<size_t>(nseg) * 4,
                                       static_cast<size_t>(nchunks) * cd * 8, cd * 8, static_cast<size_t>(grid) * cd * 8,
-                                      static_cast<size_t>(n), (kMtN + 1) * 4 * 2, static_cast<size_t>(grid) * 16,
-                                      static_cast<size_t>(std::min<int64_t>(budget_req, n)) * 8, 16});
+                                      static_cast<size_t>(n), (kMtN + 1) * 4 * 2, sharded ? 0 : words, 16});
     rc = alq_scratch_reserve(ctx, need);
     if (rc != ALQ_OK) return rc;
     ScratchCursor cur(ctx->scratch);
     int32_t* tab = cur.take<int32_t>(entries);
     int32_t* counts = cur.take<int32_t>(c);
     unsigned int* bad = cur.take<unsigned int>(2);
-    int32_t* seg_avail = cur.take<int32_t>(grid);
+    int32_t* seg_avail = cur.take<int32_t>(nseg);
     double* partial = cur.take<double>(static_cast<size_t>(nchunks) * cd);
     double* sums0 = cur.take<double>(cd);
     double* sums = cur.take<double>(static_cast<size_t>(grid) * cd);
     uint8_t* avail = cur.take<uint8_t>(n);
     unsigned int* mt = cur.take<unsigned int>(2 * (kMtN + 1));
-    unsigned long long* keyw = cur.take<unsigned long long>(static_cast<size_t>(grid) * 2);
-    unsigned long long* pickw = cur.take<unsigned long long>(static_cast<size_t>(std::min<int64_t>(budget_req, n)));
+    char* word_scratch = cur.take<char>(sharded ? 0 : words);
     int* small = cur.take<int>(4);                                     // [0] status, [1] balancing steps
 
-    std::vector<int32_t> counts_h(c), seg_h(grid);
-    rc = alq_bal_counts(ctx, D, n, c, grid, tab, bad, counts, seg_avail, counts_h.data(), seg_h.data(), st, "alq_balancing_select");
+    std::vector<int32_t> counts_h(c), seg_h(nseg);
+    rc = alq_bal_counts(ctx, D, n, c, S, tab, bad, counts, seg_avail, counts_h.data(), seg_h.data(), st, "alq_balancing_select");
     if (rc != ALQ_OK) return rc;
     int64_t n_avail = 0, labeled_total = 0;
-    for (int b = 0; b < grid; ++b) n_avail += seg_h[b];
+    for (int g = 0; g < nseg; ++g) n_avail += seg_h[g];
     for (int k = 0; k < c; ++k) labeled_total += counts_h[k];
     const int budget = static_cast<int>(std::min<int64_t>(budget_req, n_avail));
     if (labeled_total + budget >= (1LL << 24)) {
@@ -471,19 +517,19 @@ extern "C" int alq_balancing_select(alq_ctx* ctx, const alq_balancing_desc* D, v
     mt_h[kMtN] = static_cast<unsigned int>(*D->mt_pos_host);
     ALQ_CUDA(ctx, cudaMemcpyAsync(mt, mt_h.data(), (kMtN + 1) * 4, cudaMemcpyHostToDevice, st));
     ALQ_CUDA(ctx, cudaMemcpyAsync(avail, D->avail, static_cast<size_t>(n), cudaMemcpyDeviceToDevice, st));
-    ALQ_CUDA(ctx, cudaMemsetAsync(keyw, 0, static_cast<size_t>(grid) * 16, st));
-    ALQ_CUDA(ctx, cudaMemsetAsync(pickw, 0, static_cast<size_t>(budget) * 8, st));
     ALQ_CUDA(ctx, cudaMemsetAsync(small, 0, 4 * sizeof(int), st));
 
     // ---- the loop ---------------------------------------------------------------------------------------------------
     BalArgs A{};
+    rc = alq_bal_words_begin(ctx, S, sharded, budget, word_scratch, &A.W, st);
+    if (rc != ALQ_OK) return rc;
     A.x = D->x; A.ldx = D->ldx; A.d = d;
     A.xn = D->xn; A.labels = D->labels; A.avail = avail;
     A.sums0 = sums0; A.sums = sums; A.counts0 = counts; A.seg_avail0 = seg_avail;
     A.mt_in = mt; A.mt_out = mt + kMtN + 1;
     A.picks = D->picks; A.n_bal = small + 1; A.status = small;
-    A.keyw = keyw; A.pickw = pickw;
-    A.n = n; A.c = c; A.budget = budget; A.grid = grid; A.n_avail = static_cast<int>(n_avail);
+    A.S = S;
+    A.n = n; A.c = c; A.budget = budget; A.n_avail = static_cast<int>(n_avail);
     A.timeout_cycles = static_cast<long long>(ctx->spin_timeout_ms) * ctx->clock_khz;
     ALQ_CUDA(ctx, cudaFuncSetAttribute(balancing_loop_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
     // every CTA spins on the others' words, so all of them must be resident: grid <= SMs, one CTA per SM at most
@@ -499,7 +545,7 @@ extern "C" int alq_balancing_select(alq_ctx* ctx, const alq_balancing_desc* D, v
     ALQ_CUDA(ctx, cudaMemcpyAsync(small_h, small, sizeof(small_h), cudaMemcpyDeviceToHost, st));
     ALQ_CUDA(ctx, cudaMemcpyAsync(mt_h.data(), A.mt_out, (kMtN + 1) * 4, cudaMemcpyDeviceToHost, st));
     ALQ_CUDA(ctx, cudaStreamSynchronize(st));
-    if (small_h[0] != 0) ALQ_FAIL(ctx, small_h[0], "alq_balancing_select: timed out waiting for a CTA of the grid");
+    if (small_h[0] != 0) ALQ_FAIL(ctx, small_h[0], "alq_balancing_select: timed out waiting for a peer GPU or a CTA of the grid");
     std::copy(mt_h.begin(), mt_h.begin() + kMtN, D->mt_key_host);
     *D->mt_pos_host = static_cast<int32_t>(mt_h[kMtN]);
     *D->n_picks_host = budget;

@@ -53,15 +53,15 @@ struct TabArgs {
     int* slot_row;               // [n_slots] the row of every table slot
     const int* slot_lo;          // [grid]: CTA b owns the slots slot_lo[b] ..
     const int* counts0;          // [c]
-    const int* seg_avail0;       // [grid]
+    const int* seg_avail0;       // [world * grid]
     const unsigned int* mt_in;   // [kMtN + 1]: key, pos
     unsigned int* mt_out;        // [kMtN + 1]
     int* picks;
     int* n_bal;
     int* status;
-    unsigned long long* keyw;    // [2][grid] LL words of the balancing steps (two parities)
-    unsigned long long* pickw;   // [budget]  LL word of each random step
-    int n, c, budget, grid, n_avail, pend_cap;
+    BalShard S;
+    BalWords W;                  // key words of the balancing steps (two parities), one pick word per random step
+    int n, c, budget, n_avail, pend_cap;
     long long timeout_cycles;
 };
 
@@ -144,22 +144,22 @@ __host__ __device__ __forceinline__ size_t bal_table_region(int pend_cap, int d)
     const size_t pend = static_cast<size_t>(pend_cap) * d * 4;
     return pend > kBuildBytes ? pend : kBuildBytes;
 }
-__host__ __device__ __forceinline__ size_t bal_table_smem(int c, int d, int grid, int pend_cap) {
-    return bal_table_region(pend_cap, d) + static_cast<size_t>(c) * 20 + static_cast<size_t>(grid) * 4 +
+__host__ __device__ __forceinline__ size_t bal_table_smem(int c, int d, int nseg, int pend_cap) {
+    return bal_table_region(pend_cap, d) + static_cast<size_t>(c) * 20 + static_cast<size_t>(nseg) * 4 +
            static_cast<size_t>(pend_cap) * 4 + kMtN * 4 + 64;
 }
 
 __global__ void __launch_bounds__(kTabThreads, 1) balancing_table_kernel(const __grid_constant__ TabArgs A) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    const int c = A.c, d = A.d, dv = d >> 2, grid = A.grid, pend_cap = A.pend_cap;
+    const int c = A.c, d = A.d, dv = d >> 2, nseg = A.S.world * A.S.grid, pend_cap = A.pend_cap;
     float* pend_x = reinterpret_cast<float*>(smem_raw);                               // [pend_cap][d] (the build's stage)
     double* stage = reinterpret_cast<double*>(smem_raw);                              // [kBuildDims][kBuildLd]
     double* q = reinterpret_cast<double*>(smem_raw + bal_table_region(pend_cap, d));  // [c]
     int* cnt = reinterpret_cast<int*>(q + c);                                         // [c]
     float* den = reinterpret_cast<float*>(cnt + c);                                   // [c]
     int* sel = reinterpret_cast<int*>(den + c);                                       // [c]
-    int* seg_av = sel + c;                                                            // [grid]
-    int* pend_y = seg_av + grid;                                                      // [pend_cap]
+    int* seg_av = sel + c;                                                            // [nseg]
+    int* pend_y = seg_av + nseg;                                                      // [pend_cap]
     unsigned int* mt = reinterpret_cast<unsigned int*>(pend_y + pend_cap);            // [kMtN]
     __shared__ unsigned long long s_key[kTabWarps];
     __shared__ int s_wc[kTabWarps], s_red[5 * kTabWarps];
@@ -168,7 +168,8 @@ __global__ void __launch_bounds__(kTabThreads, 1) balancing_table_kernel(const _
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int b = blockIdx.x;
-    const int row_lo = seg_lo(A.n, grid, b), row_hi = seg_lo(A.n, grid, b + 1);
+    const int gb = A.S.rank * A.S.grid + b;                                           // my global segment
+    const int row_lo = gseg_lo(A.S, gb), row_hi = gseg_lo(A.S, gb + 1);
     const int slo = A.slot_lo[b];
     double* my_sums = A.sums + static_cast<size_t>(b) * c * d;
 
@@ -178,11 +179,11 @@ __global__ void __launch_bounds__(kTabThreads, 1) balancing_table_kernel(const _
         den[i] = bal_den(k);
         q[i] = A.q0[i];
     }
-    for (int i = tid; i < grid; i += kTabThreads) seg_av[i] = A.seg_avail0[i];
+    for (int i = tid; i < nseg; i += kTabThreads) seg_av[i] = A.seg_avail0[i];
     for (int i = tid; i < kMtN; i += kTabThreads) mt[i] = A.mt_in[i];
     if (tid == 0) { s_mtpos = static_cast<int>(A.mt_in[kMtN]); s_navail = A.n_avail; }
     for (size_t i = tid; i < static_cast<size_t>(c) * d; i += kTabThreads) my_sums[i] = A.sums0[i];
-    __syncthreads();
+    bal_ready_wait(A, tid);
 
     // the table rows of my slots, streamed once per balancing step: apply the pending picks (in pick order) and,
     // when `score`, return the warp's smallest key (ord(fl32(near / far) + 0) << 32 | row)
@@ -375,49 +376,21 @@ __global__ void __launch_bounds__(kTabThreads, 1) balancing_table_kernel(const _
             npend = 0;
             if (lane == 0) s_key[warp] = best;
             __syncthreads();
-            const unsigned int tag16 = 0x8000u | (++rnd_key & 0x7fffu);
-            char* const keyw = reinterpret_cast<char*>(A.keyw + static_cast<size_t>(rnd_key & 1u) * grid);
-            if (tid == 0) {
-                unsigned long long m = s_key[0];
-                for (int w = 1; w < kTabWarps; ++w) m = s_key[w] < m ? s_key[w] : m;
-                const unsigned long long off = m == ~0ull ? kEmptyOff : static_cast<unsigned long long>(static_cast<uint32_t>(m) - row_lo);
-                ll_store_raw(keyw + static_cast<size_t>(b) * 8, (static_cast<unsigned long long>(tag16) << 48) | (off << 32) | (m >> 32));
-            }
-            unsigned long long mine = ~0ull;
-            ll_gather(keyw, grid, 8, tag16, 48, A, tid, [&](int i, unsigned long long w) {
-                const unsigned int off = static_cast<unsigned int>(w >> 32) & 0xffffu;
-                if (off == kEmptyOff) return;
-                const unsigned long long key = ((w & 0xffffffffull) << 32) | static_cast<uint32_t>(seg_lo(A.n, grid, i) + static_cast<int>(off));
-                mine = key < mine ? key : mine;
-            });
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) {
-                const unsigned long long w = __shfl_xor_sync(0xffffffffu, mine, o);
-                mine = w < mine ? w : mine;
-            }
-            __syncthreads();                                              // s_key is reused
-            if (lane == 0) s_key[warp] = mine;
-            __syncthreads();
-            if (tid == 0) {
-                unsigned long long m = s_key[0];
-                for (int w = 1; w < kTabWarps; ++w) m = s_key[w] < m ? s_key[w] : m;
-                s_pick = m == ~0ull ? -1 : static_cast<int>(static_cast<uint32_t>(m));
-            }
-            __syncthreads();
+            bal_agree<kTabWarps>(A, s_key, &s_pick, ++rnd_key, row_lo, tid);
         } else {
             // ===== random step (balancing_sampler.py:128): np.random.choice over the available rows =====
             if (tid == 0) {
                 int k = static_cast<int>(mt_bounded(mt, s_mtpos, static_cast<unsigned int>(s_navail - 1)));
                 int o = 0;
-                while (o + 1 < grid && k >= seg_av[o]) { k -= seg_av[o]; ++o; }
+                while (o + 1 < nseg && k >= seg_av[o]) { k -= seg_av[o]; ++o; }
                 s_owner = o;
                 s_rank = k;
                 s_found = -1;
             }
             __syncthreads();
-            unsigned long long* const pw = A.pickw + t;
-            const unsigned int ptag = 0x80000000u | static_cast<unsigned int>(t);
-            if (s_owner == b) {                                           // the rank-th available row of this segment
+            const size_t pw = A.W.pickw + static_cast<size_t>(t) * 8;
+            const unsigned int ptag = bal_pick_tag(A.W, t);
+            if (s_owner == gb) {                                          // the rank-th available row of this segment
                 const int rank = s_rank;
                 int base = 0;
                 for (int r0 = row_lo; r0 < row_hi; r0 += kTabThreads) {
@@ -438,9 +411,9 @@ __global__ void __launch_bounds__(kTabThreads, 1) balancing_table_kernel(const _
                     if (here) break;
                     base += tot;
                 }
-                if (tid == 0) ll_store(pw, ptag, static_cast<unsigned int>(s_found));
+                if (tid < A.S.world) ll_store(A.W.peer[tid] + pw, ptag, static_cast<unsigned int>(s_found));
             }
-            if (tid == 0) s_pick = static_cast<int>(ll_wait(pw, ptag, A));
+            if (tid == 0) s_pick = static_cast<int>(ll_wait(A.W.peer[A.S.rank] + pw, ptag, A));
             __syncthreads();
         }
 
@@ -457,16 +430,14 @@ __global__ void __launch_bounds__(kTabThreads, 1) balancing_table_kernel(const _
         }
         const int cls = __ldg(A.labels + pick);
         const int newc = cnt[cls] + 1;
-        int o = static_cast<int>(static_cast<long long>(pick) * grid / A.n);
-        while (o + 1 < grid && seg_lo(A.n, grid, o + 1) <= pick) ++o;
-        while (o > 0 && seg_lo(A.n, grid, o) > pick) --o;
+        const int o = gseg_of(A.S, pick);
         __syncthreads();                                                 // cnt[cls] read by every thread
         if (tid == 0) {
             cnt[cls] = newc;
             den[cls] = bal_den(newc);
             seg_av[o] -= 1;
             s_navail -= 1;
-            if (o == b) A.avail[pick] = 0;
+            if (o == gb) A.avail[pick] = 0;
             if (b == 0) A.picks[t] = pick;
             if (built) pend_y[npend] = cls;
         }
@@ -509,42 +480,56 @@ extern "C" int alq_balancing_table_select(alq_ctx* ctx, const alq_balancing_desc
     }
     const cudaStream_t st = static_cast<cudaStream_t>(stream);
 
-    // ---- limits that the shape decides --------------------------------------------------------------------------
-    const int grid = std::max(1, std::min(ctx->sm_count, (n + 127) / 128));
+    // ---- limits that the shape decides (the same on every rank of a sharded call) -------------------------------------
+    BalShard S;
+    bool sharded = false;
+    rc = alq_bal_shard(ctx, D, n, &S, &sharded, fn);
+    if (rc != ALQ_OK) return rc;
+    const int grid = S.grid, nseg = S.world * grid;
     const size_t smem_cap = ctx->smem_optin > 4096 ? ctx->smem_optin - 1024 : 0;   // the kernel's static shared memory
-    const size_t fixed = bal_table_smem(c, d, grid, 0) - kBuildBytes;
+    const size_t fixed = bal_table_smem(c, d, nseg, 0) - kBuildBytes;
     int pend_cap = fixed < smem_cap ? static_cast<int>(std::min<size_t>(kPendMax, (smem_cap - fixed) / (static_cast<size_t>(d) * 4 + 4))) : 0;
-    while (pend_cap > 0 && bal_table_smem(c, d, grid, pend_cap) > smem_cap) --pend_cap;
+    while (pend_cap > 0 && bal_table_smem(c, d, nseg, pend_cap) > smem_cap) --pend_cap;
     const size_t group_smem = static_cast<size_t>(c) * 4;
     if (pend_cap < 1 || group_smem > smem_cap) {
         if (!forced) return ALQ_OK;
         ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: the tables of %d classes and one pending row of %d floats need %zu bytes of shared "
                  "memory, %zu are available (limit: class tables in shared memory)", fn, c, d,
-                 bal_table_smem(c, d, grid, 1), smem_cap);
+                 bal_table_smem(c, d, nseg, 1), smem_cap);
     }
-    const size_t smem = bal_table_smem(c, d, grid, pend_cap);
-    if (n - seg_lo(n, grid, grid - 1) > kSegRowsMax) {
+    const size_t smem = bal_table_smem(c, d, nseg, pend_cap);
+    if (alq_bal_seg_rows_max(S) > kSegRowsMax) {
         if (!forced) return ALQ_OK;
         ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: n=%d rows over %d CTAs exceed %d rows per CTA segment (limit: rows per segment)",
-                 fn, n, grid, kSegRowsMax);
+                 fn, n, nseg, kSegRowsMax);
+    }
+    const size_t words = alq_bal_words_bytes(S, std::min<int64_t>(D->budget, n), sharded);
+    if (sharded && words > ctx->comm.greedy_bytes()) {
+        if (!forced) return ALQ_OK;
+        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: a budget of %lld needs %zu bytes of the peer window, %zu are usable (limit: words "
+                 "in the peer window)", fn, (long long)D->budget, words, ctx->comm.greedy_bytes());
     }
 
     // ---- set-up: counts, segment counts, label checks -----------------------------------------------------------
     const size_t entries = alq_class_table_entries(n, c);
-    rc = alq_scratch_reserve(ctx, scratch_need({entries * 4, static_cast<size_t>(c) * 4, 8, static_cast<size_t>(grid) * 4}));
+    rc = alq_scratch_reserve(ctx, scratch_need({entries * 4, static_cast<size_t>(c) * 4, 8, static_cast<size_t>(nseg) * 4}));
     if (rc != ALQ_OK) return rc;
-    std::vector<int32_t> counts_h(c), seg_h(grid);
+    std::vector<int32_t> counts_h(c), seg_h(nseg);
     {
         ScratchCursor cur(ctx->scratch);
         int32_t* tab = cur.take<int32_t>(entries);
         int32_t* counts = cur.take<int32_t>(c);
         unsigned int* bad = cur.take<unsigned int>(2);
-        int32_t* seg_avail = cur.take<int32_t>(grid);
-        rc = alq_bal_counts(ctx, D, n, c, grid, tab, bad, counts, seg_avail, counts_h.data(), seg_h.data(), st, fn);
+        int32_t* seg_avail = cur.take<int32_t>(nseg);
+        rc = alq_bal_counts(ctx, D, n, c, S, tab, bad, counts, seg_avail, counts_h.data(), seg_h.data(), st, fn);
         if (rc != ALQ_OK) return rc;
     }
     int64_t n_avail = 0, labeled_total = 0;
-    for (int b = 0; b < grid; ++b) n_avail += seg_h[b];
+    std::vector<int64_t> avail_of(S.world, 0);                        // available rows per rank: its table rows
+    for (int g = 0; g < nseg; ++g) {
+        n_avail += seg_h[g];
+        avail_of[g / grid] += seg_h[g];
+    }
     for (int k = 0; k < c; ++k) labeled_total += counts_h[k];
     const int budget = static_cast<int>(std::min<int64_t>(D->budget, n_avail));
     if (labeled_total + budget >= (1LL << 24)) {
@@ -559,13 +544,30 @@ extern "C" int alq_balancing_table_select(alq_ctx* ctx, const alq_balancing_desc
 
     // ---- the table and the per-CTA sums must fit the device's free memory: checked before anything is reserved ----
     const size_t cd = static_cast<size_t>(c) * d;
-    const size_t na = static_cast<size_t>(n_avail);
-    const size_t need = scratch_need({static_cast<size_t>(c) * 4, static_cast<size_t>(grid) * 4, static_cast<size_t>(c + 1) * 4,
-                                      static_cast<size_t>(grid) * 4, static_cast<size_t>(std::max<int64_t>(labeled_total, 1)) * 4,
-                                      cd * 8, static_cast<size_t>(c) * 8, static_cast<size_t>(grid) * cd * 8, na * c * 8,
-                                      na * 8, na * 4, static_cast<size_t>(n), (kMtN + 1) * 4 * 2,
-                                      static_cast<size_t>(grid) * 16, static_cast<size_t>(budget) * 8, 16});
-    if (need > ctx->scratch_bytes) {
+    const size_t words_b = alq_bal_words_bytes(S, budget, sharded);
+    auto need_for = [&](size_t na) {
+        return scratch_need({static_cast<size_t>(c) * 4, static_cast<size_t>(nseg) * 4, static_cast<size_t>(c + 1) * 4,
+                             static_cast<size_t>(grid) * 4, static_cast<size_t>(std::max<int64_t>(labeled_total, 1)) * 4,
+                             cd * 8, static_cast<size_t>(c) * 8, static_cast<size_t>(grid) * cd * 8, na * c * 8,
+                             na * 8, na * 4, static_cast<size_t>(n), (kMtN + 1) * 4 * 2, sharded ? 0 : words_b, 16});
+    };
+    const size_t na = static_cast<size_t>(avail_of[S.rank]);
+    const size_t need = need_for(na);
+    if (sharded) {
+        // the same decision on every rank: every rank's share against the group's least free memory (the caller's
+        // gather; this context's scratch is not counted, so the check is conservative)
+        for (int r = 0; r < S.world; ++r) {
+            const size_t nr = need_for(static_cast<size_t>(avail_of[r]));
+            const size_t want = nr + (nr >> 2) + (1u << 20);            // what alq_scratch_reserve allocates
+            if (D->group_free_bytes < 0 || want > static_cast<size_t>(D->group_free_bytes)) {
+                if (!forced) return ALQ_OK;
+                ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: rank %d's %lld x %d table (%zu bytes) and %d copies of the class sums (%zu "
+                         "bytes) need %zu bytes of device memory, the group has %lld free (limit: table in device memory)", fn,
+                         r, (long long)avail_of[r], c, static_cast<size_t>(avail_of[r]) * c * 8, grid,
+                         static_cast<size_t>(grid) * cd * 8, want, (long long)D->group_free_bytes);
+            }
+        }
+    } else if (need > ctx->scratch_bytes) {
         size_t free_b = 0, total_b = 0;
         ALQ_CUDA(ctx, cudaMemGetInfo(&free_b, &total_b));
         const size_t want = need + (need >> 2) + (1u << 20);           // what alq_scratch_reserve allocates
@@ -580,7 +582,7 @@ extern "C" int alq_balancing_table_select(alq_ctx* ctx, const alq_balancing_desc
     if (rc != ALQ_OK) return rc;
     ScratchCursor cur(ctx->scratch);
     int32_t* counts = cur.take<int32_t>(c);
-    int32_t* seg_avail = cur.take<int32_t>(grid);
+    int32_t* seg_avail = cur.take<int32_t>(nseg);
     int32_t* off = cur.take<int32_t>(c + 1);
     int32_t* slot_lo = cur.take<int32_t>(grid);
     int32_t* grp = cur.take<int32_t>(static_cast<size_t>(std::max<int64_t>(labeled_total, 1)));
@@ -592,16 +594,16 @@ extern "C" int alq_balancing_table_select(alq_ctx* ctx, const alq_balancing_desc
     int32_t* slot_row = cur.take<int32_t>(na);
     uint8_t* avail = cur.take<uint8_t>(n);
     unsigned int* mt = cur.take<unsigned int>(2 * (kMtN + 1));
-    unsigned long long* keyw = cur.take<unsigned long long>(static_cast<size_t>(grid) * 2);
-    unsigned long long* pickw = cur.take<unsigned long long>(static_cast<size_t>(budget));
+    char* word_scratch = cur.take<char>(sharded ? 0 : words_b);
     int* small = cur.take<int>(4);                                     // [0] status, [1] balancing steps
 
+    // table slots: the available rows of this rank's segments only
     std::vector<int32_t> off_h(c + 1), slot_lo_h(grid);
     off_h[0] = 0;
     for (int k = 0; k < c; ++k) off_h[k + 1] = off_h[k] + counts_h[k];
-    for (int b = 0, s = 0; b < grid; ++b) { slot_lo_h[b] = s; s += seg_h[b]; }
+    for (int b = 0, s = 0; b < grid; ++b) { slot_lo_h[b] = s; s += seg_h[S.rank * grid + b]; }
     ALQ_CUDA(ctx, cudaMemcpyAsync(counts, counts_h.data(), static_cast<size_t>(c) * 4, cudaMemcpyHostToDevice, st));
-    ALQ_CUDA(ctx, cudaMemcpyAsync(seg_avail, seg_h.data(), static_cast<size_t>(grid) * 4, cudaMemcpyHostToDevice, st));
+    ALQ_CUDA(ctx, cudaMemcpyAsync(seg_avail, seg_h.data(), static_cast<size_t>(nseg) * 4, cudaMemcpyHostToDevice, st));
     ALQ_CUDA(ctx, cudaMemcpyAsync(off, off_h.data(), static_cast<size_t>(c + 1) * 4, cudaMemcpyHostToDevice, st));
     ALQ_CUDA(ctx, cudaMemcpyAsync(slot_lo, slot_lo_h.data(), static_cast<size_t>(grid) * 4, cudaMemcpyHostToDevice, st));
 
@@ -617,12 +619,12 @@ extern "C" int alq_balancing_table_select(alq_ctx* ctx, const alq_balancing_desc
     mt_h[kMtN] = static_cast<unsigned int>(*D->mt_pos_host);
     ALQ_CUDA(ctx, cudaMemcpyAsync(mt, mt_h.data(), (kMtN + 1) * 4, cudaMemcpyHostToDevice, st));
     ALQ_CUDA(ctx, cudaMemcpyAsync(avail, D->avail, static_cast<size_t>(n), cudaMemcpyDeviceToDevice, st));
-    ALQ_CUDA(ctx, cudaMemsetAsync(keyw, 0, static_cast<size_t>(grid) * 16, st));
-    ALQ_CUDA(ctx, cudaMemsetAsync(pickw, 0, static_cast<size_t>(budget) * 8, st));
     ALQ_CUDA(ctx, cudaMemsetAsync(small, 0, 4 * sizeof(int), st));
 
     // ---- the loop ---------------------------------------------------------------------------------------------------
     TabArgs A{};
+    rc = alq_bal_words_begin(ctx, S, sharded, budget, word_scratch, &A.W, st);
+    if (rc != ALQ_OK) return rc;
     A.x = D->x; A.ldx = D->ldx; A.d = d;
     A.labels = D->labels; A.avail = avail;
     A.sums0 = sums0; A.q0 = q0; A.sums = sums;
@@ -630,8 +632,8 @@ extern "C" int alq_balancing_table_select(alq_ctx* ctx, const alq_balancing_desc
     A.counts0 = counts; A.seg_avail0 = seg_avail;
     A.mt_in = mt; A.mt_out = mt + kMtN + 1;
     A.picks = D->picks; A.n_bal = small + 1; A.status = small;
-    A.keyw = keyw; A.pickw = pickw;
-    A.n = n; A.c = c; A.budget = budget; A.grid = grid; A.n_avail = static_cast<int>(n_avail); A.pend_cap = pend_cap;
+    A.S = S;
+    A.n = n; A.c = c; A.budget = budget; A.n_avail = static_cast<int>(n_avail); A.pend_cap = pend_cap;
     A.timeout_cycles = static_cast<long long>(ctx->spin_timeout_ms) * ctx->clock_khz;
     ALQ_CUDA(ctx, cudaFuncSetAttribute(balancing_table_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
     // every CTA spins on the others' words, so all of them must be resident: grid <= SMs, one CTA per SM at most
@@ -647,7 +649,7 @@ extern "C" int alq_balancing_table_select(alq_ctx* ctx, const alq_balancing_desc
     ALQ_CUDA(ctx, cudaMemcpyAsync(small_h, small, sizeof(small_h), cudaMemcpyDeviceToHost, st));
     ALQ_CUDA(ctx, cudaMemcpyAsync(mt_h.data(), A.mt_out, (kMtN + 1) * 4, cudaMemcpyDeviceToHost, st));
     ALQ_CUDA(ctx, cudaStreamSynchronize(st));
-    if (small_h[0] != 0) ALQ_FAIL(ctx, small_h[0], "%s: timed out waiting for a CTA of the grid", fn);
+    if (small_h[0] != 0) ALQ_FAIL(ctx, small_h[0], "%s: timed out waiting for a peer GPU or a CTA of the grid", fn);
     std::copy(mt_h.begin(), mt_h.begin() + kMtN, D->mt_key_host);
     *D->mt_pos_host = static_cast<int32_t>(mt_h[kMtN]);
     *D->n_picks_host = budget;

@@ -6,6 +6,29 @@
 // P2P) and system-scope flags -- no host round trip and no collective library inside the 10 000-step loop.
 #include "alq_common.cuh"
 
+namespace {
+
+struct PeerWindows {
+    char* p[ALQ_MAX_WORLD];
+};
+
+__global__ void comm_ready_kernel(const __grid_constant__ PeerWindows W, int world, int rank, unsigned long long tag) {
+    if (threadIdx.x < world) {
+        __threadfence_system();
+        st_release_sys(reinterpret_cast<unsigned long long*>(W.p[threadIdx.x]) + rank, tag);
+    }
+}
+
+}  // namespace
+
+int alq_comm_ready(alq_ctx* ctx, unsigned long long tag, cudaStream_t st) {
+    PeerWindows W{};
+    for (int r = 0; r < ctx->comm.world; ++r) W.p[r] = ctx->comm.peer[r];
+    comm_ready_kernel<<<1, 32, 0, st>>>(W, ctx->comm.world, ctx->comm.rank, tag);
+    ALQ_LAUNCH_CHECK(ctx);
+    return ALQ_OK;
+}
+
 extern "C" int alq_comm_create(alq_ctx* ctx, int32_t world, int32_t rank, size_t window_bytes, void* handle_out) {
     if (!ctx) return ALQ_ERR_INVALID;
     if (world < 1 || world > ALQ_MAX_WORLD || rank < 0 || rank >= world || !handle_out || window_bytes < (1u << 16))

@@ -131,6 +131,10 @@ void alq_gridsync_begin(alq_ctx* ctx, cudaStream_t st);
 void alq_gridsync_end(alq_ctx* ctx, cudaStream_t st);
 
 int alq_scratch_reserve(alq_ctx* ctx, size_t bytes);
+// The start-of-call handshake of a collective call over the group's windows (alq_comm.cu): once this rank has cleared
+// its window for the call (earlier on `st`), store `tag` into ready[rank] of every rank's window, the u64
+// ready[ALQ_MAX_WORLD] at its head.  Peers write into this window only after they have seen it.
+int alq_comm_ready(alq_ctx* ctx, unsigned long long tag, cudaStream_t st);
 // K10's tile histogram + per-class scan (alq_classes.cu): counts[k] = rows with avail != 0 and labels == k; an available
 // row with a label outside [0, c) is not counted and, with `bad` given, the smallest such row is atomicMin'ed there.
 // `tab` holds alq_class_table_entries(n, c) int32 entries of scratch.

@@ -105,6 +105,7 @@ class Engine:
         blob = b"".join(handles)
         self._check(self.lib.alq_comm_connect(self._h, blob), "alq_comm_connect")
         self.world, self.rank = world, rank
+        self.comm_group = process_group
         self.comm_ready = True
         return self
 
@@ -559,7 +560,7 @@ class Engine:
 
     # -- K11: BalancingSampler's whole query -----------------------------------------------------------
     def balancing_select(self, emb: torch.Tensor, xn: torch.Tensor, labels: torch.Tensor, avail: torch.Tensor,
-                         labeled: torch.Tensor, num_classes: int, budget: int):
+                         labeled: torch.Tensor, num_classes: int, budget: int, shard_off: Optional[Sequence[int]] = None):
         """K11: balancing_sampler.py:58-134 in one persistent launch.  `emb` [n, d] float32 (d and the leading dimension
         multiples of 4), `xn` = row_norm2(emb), `labels` int32 [n], `avail` / `labeled` uint8 (or bool) [n], all on this
         device.  The random steps draw from NumPy's global RandomState exactly as `np.random.choice` would: the state is
@@ -567,21 +568,29 @@ class Engine:
         unchanged).  Returns (picks: host int64 array in pick order, balancing steps), or None when the per-step path
         must run instead (option "balancing_loop" = 1 or 3, or auto beyond the loop's limits; nothing is drawn then).
         AlqError for bad inputs, for a labeled or available row whose label is outside [0, num_classes), and, under
-        balancing_loop = 2, for a shape beyond the limits (the message names the limit)."""
+        balancing_loop = 2, for a shape beyond the limits (the message names the limit).
+
+        Sharded (comm_init): every tensor is the GLOBAL array, replicated on every rank, and `shard_off` [world + 1] says
+        which rows each rank streams (e.g. ShardGroup.row_range's bounds).  Collective: every rank calls it with the same
+        inputs, which one small all_gather_object checks first (sharding.balancing_agreement: AlqError on every rank on a
+        mismatch, before any launch).  Every rank returns the same picks, steps and MT19937 state as one GPU would."""
         return self._balancing_call("balancing_select", self.lib.alq_balancing_select, emb, xn, labels, avail, labeled,
-                                    num_classes, budget)
+                                    num_classes, budget, shard_off)
 
     def balancing_table_select(self, emb: torch.Tensor, xn: torch.Tensor, labels: torch.Tensor, avail: torch.Tensor,
-                               labeled: torch.Tensor, num_classes: int, budget: int):
+                               labeled: torch.Tensor, num_classes: int, budget: int,
+                               shard_off: Optional[Sequence[int]] = None):
         """K12: the same query, arguments and contract as `balancing_select`, over an incremental row x class table of
         fp64 dot products with the class sums instead of centres in shared memory, so it runs at ImageNet-LT's 1 000
         classes of 2 048 dimensions.  Returns None under option "balancing_loop" = 1 or 2, or under auto beyond its
         limits (shared memory for the per-class tables, rows per CTA segment, counts plus budget below 2^24, the table
-        and the per-CTA class sums in free device memory); AlqError naming the limit under balancing_loop = 3."""
+        and the per-CTA class sums in free device memory); AlqError naming the limit under balancing_loop = 3.  Sharded
+        as `balancing_select`; each rank then holds the table rows of its own shard only, and the memory limit is
+        checked against the least free device memory of the group, gathered with the input check."""
         return self._balancing_call("balancing_table_select", self.lib.alq_balancing_table_select, emb, xn, labels, avail,
-                                    labeled, num_classes, budget)
+                                    labeled, num_classes, budget, shard_off)
 
-    def _balancing_call(self, name, fn, emb, xn, labels, avail, labeled, num_classes, budget):
+    def _balancing_call(self, name, fn, emb, xn, labels, avail, labeled, num_classes, budget, shard_off=None):
         """Checks the arguments of K11 / K12 (messages start with `name`), runs `fn` with NumPy's MT19937 state and
         writes the state back; None when the call declined."""
         emb = _f32c(emb, "emb")
@@ -609,6 +618,17 @@ class Engine:
         if emb.shape[1] % 4 or _ld(emb) % 4 or emb.data_ptr() % 16:
             raise AlqError(f"{name}: emb needs d and its leading dimension multiples of 4 and a 16-byte aligned base")
         xn, labels = xn.contiguous().reshape(-1), labels.contiguous()
+        so, free_min = None, 0
+        if shard_off is not None:
+            from .sharding import balancing_agreement
+            if not getattr(self, "comm_ready", False):
+                raise AlqError(f"{name}: a sharded call (shard_off) needs comm_init first")
+            so = np.ascontiguousarray(shard_off, dtype=np.int32).reshape(-1)
+            if so.size != self.world + 1:
+                raise AlqError(f"{name}: shard_off needs {self.world + 1} offsets for a group of {self.world}, got {so.size}")
+            free = torch.cuda.mem_get_info(self.device)[0] if name == "balancing_table_select" else 0
+            free_min = balancing_agreement("alq_" + name, (n, d), c, budget, so, labels, masks[0], masks[1], free,
+                                           self.comm_group)
         sname, key, pos, has_gauss, cached = np.random.get_state()
         key = np.array(key, dtype=np.uint32)
         pos_c, n_picks, n_bal = C.c_int32(int(pos)), C.c_int64(0), C.c_int64(0)
@@ -623,6 +643,8 @@ class Engine:
         desc.mt_pos_host = C.addressof(pos_c)
         desc.picks = picks.data_ptr()
         desc.n_picks_host, desc.n_balancing_host = C.addressof(n_picks), C.addressof(n_bal)
+        if so is not None:
+            desc.shard_off_host, desc.group_free_bytes = so.ctypes.data, int(free_min)
         self._check(fn(self._h, C.byref(desc), self._stream()), "alq_" + name)
         if n_picks.value < 0:
             return None

@@ -21,6 +21,11 @@ counts plus budget below 2^24).  Then, when the engine also offers `balancing_ta
 incremental fp64 row x class table, for class counts like ImageNet-LT's 1 000), that runs; it declines under option 1
 or 2 or beyond its own limits (per-class tables in shared memory, the table in free device memory).  Only when both
 decline does the step loop below run, unchanged.
+
+In a ShardGroup of G > 1 ranks each rank forwards 1/G of the pool, the embeddings and labels are replicated with one
+all-gather, and K11 / K12 run sharded by row (each rank streams its row_range, the ranks agree on every pick through the
+engine's peer-memory windows).  The host bookkeeping and NumPy's RNG are replicated, so every rank returns the one-GPU
+picks, and the step loop, if both decline, runs identically on every rank.
 """
 from __future__ import annotations
 
@@ -36,15 +41,21 @@ class BalancingQuery(EngineMixin):
         self.freeze_feature = kwargs["freeze_feature"]          # required, like balancing_sampler.py:24
         self._bal_cache = None
 
-    def _pool_embeddings(self):
+    def _pool_embeddings(self, group=None):
         """Embeddings [n_pool, D padded to x4] on the device and the pool's labels (:39-58); kept across rounds under
-        --freeze_feature like the reference's saved_embeddings / saved_ys."""
+        --freeze_feature like the reference's saved_embeddings / saved_ys.  With a ShardGroup each rank forwards its
+        row_range of the pool and one all_gather_rows replicates the embeddings and the labels on every rank."""
         if self.freeze_feature and getattr(self, "_bal_cache", None) is not None:
             return self._bal_cache
+        lo, hi = (0, self.n_pool) if group is None else group.row_range(self.n_pool)
         labels = []
         self.feature_net.eval()
-        _, emb = self._forward_pool(list(range(self.n_pool)), self.feature_net, want_features=True, labels_out=labels)
+        _, emb = self._forward_pool(list(range(lo, hi)), self.feature_net, want_features=True, labels_out=labels)
         ys = torch.cat([torch.as_tensor(b).reshape(-1) for b in labels], dim=0).to(torch.int64)
+        if group is not None:
+            counts = [b - a for a, b in (group.row_range(self.n_pool, r) for r in range(group.world_size))]
+            emb = group.all_gather_rows(emb, counts)
+            ys = group.all_gather_rows(ys.to(emb.device), counts).cpu()
         if self.freeze_feature:
             self._bal_cache = (emb, ys)
         return emb, ys
@@ -54,7 +65,10 @@ class BalancingQuery(EngineMixin):
         idxs_for_query = self.available_query_idxs(boolean=True)
         idxs_labeled = self.already_labeled_idxs(boolean=True)
         labeled_idxs_cur_rd = []
-        emb, ys = self._pool_embeddings()
+        group = getattr(self, "_shard_group", None)
+        if group is not None and group.world_size < 2:
+            group = None
+        emb, ys = self._pool_embeddings(group)
         eng = self.get_engine()
         dev = emb.device
         C = self.num_classes
@@ -65,9 +79,12 @@ class BalancingQuery(EngineMixin):
             args = (emb, eng.row_norm2(emb), ys.to(device=dev, dtype=torch.int32),
                     torch.from_numpy(idxs_for_query.astype(np.uint8)).to(dev),
                     torch.from_numpy(idxs_labeled.astype(np.uint8)).to(dev), C, budget)
-            got = eng.balancing_select(*args)
+            # a group streams row_range's blocks of the replicated pool: every rank gets the one-GPU picks
+            kw = {} if group is None else {
+                "shard_off": [group.row_range(self.n_pool, r)[0] for r in range(group.world_size)] + [self.n_pool]}
+            got = eng.balancing_select(*args, **kw)
             if got is None and hasattr(eng, "balancing_table_select"):
-                got = eng.balancing_table_select(*args)
+                got = eng.balancing_table_select(*args, **kw)
             if got is not None:
                 picks = list(got[0])
                 return picks, len(picks)

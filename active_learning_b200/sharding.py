@@ -59,6 +59,48 @@ def plan_shards(cand_pos: np.ndarray, full_n: int, world: int, leaf_aligned: boo
     return shard_off, shard_pos
 
 
+def check_replicated(what: str, record: dict, local=None, process_group=None) -> list:
+    """A collective call over replicated inputs must see the same inputs on every rank: one all_gather_object of this
+    rank's `record` (small host values and digests) together with a rank-local value `local`, and an AlqError naming the
+    first field of `record` that differs -- raised on every rank, since every rank compares the same gathered records.
+    Returns every rank's `local`, in rank order."""
+    from ._lib import AlqError
+    out = [None] * dist.get_world_size(process_group)
+    dist.all_gather_object(out, (record, local), group=process_group)
+    for key in record:
+        vals = [r[0].get(key) for r in out]
+        if any(v != vals[0] for v in vals[1:]):
+            raise AlqError(f"{what}: the ranks disagree on {key} ({vals}); a sharded call needs the same replicated "
+                           f"inputs on every rank")
+    return [r[1] for r in out]
+
+
+def digest(*arrays) -> str:
+    """sha1 over the bytes of host arrays / tensors (the replicated masks and labels of a collective call)."""
+    import hashlib
+    h = hashlib.sha1()
+    for a in arrays:
+        if isinstance(a, torch.Tensor):
+            a = a.detach().cpu().contiguous().numpy()
+        a = np.ascontiguousarray(a)
+        h.update(str(a.dtype).encode() + str(a.shape).encode())
+        h.update(a.tobytes())
+    return h.hexdigest()
+
+
+def balancing_agreement(what: str, shape, num_classes: int, budget: int, shard_off, labels, avail, labeled,
+                        free_bytes: int = 0, process_group=None) -> int:
+    """The host check in front of a sharded BalancingSampler call (K11 / K12): every rank must hold the same n, d, C,
+    budget, shard offsets, labels, masks and NumPy MT19937 state, or the ranks would stream different problems and wait
+    on each other's words until the timeout.  AlqError on every rank otherwise, before anything runs on the device.
+    Returns the least of the ranks' `free_bytes` (K12's table check must decide the same way everywhere)."""
+    _, key, pos, _, _ = np.random.get_state()
+    record = {"n, d": tuple(int(v) for v in shape), "num_classes": int(num_classes), "budget": int(budget),
+              "shard_off": [int(v) for v in shard_off], "labels": digest(labels), "masks": digest(avail, labeled),
+              "MT19937 state": digest(np.asarray(key, dtype=np.uint32), np.int64(pos))}
+    return min(check_replicated(what, record, int(free_bytes), process_group))
+
+
 class ShardGroup:
     def __init__(self, process_group=None):
         if not dist.is_initialized():

@@ -71,8 +71,9 @@ int64_t alq_launch_count(const alq_ctx* ctx);
 /* ---- multi-GPU group: one process per GPU, peer-memory windows over NVLink ---------------------
  * alq_comm_create allocates this rank's window and returns its 64-byte CUDA IPC handle; the caller
  * exchanges the handles (e.g. torch.distributed.all_gather) and passes all of them, in rank order, to
- * alq_comm_connect.  The global (non-partitioned) CoreSet / k-means++ loops then exchange their
- * per-step winner through these windows from inside the kernels (alq_greedy_desc.shard_off_host).   */
+ * alq_comm_connect.  The global (non-partitioned) CoreSet / k-means++ loops and BalancingSampler's loops then exchange
+ * their per-step winner through these windows from inside the kernels (alq_greedy_desc.shard_off_host,
+ * alq_balancing_desc.shard_off_host).                                                             */
 #define ALQ_IPC_HANDLE_BYTES 64
 int alq_comm_create(alq_ctx* ctx, int32_t world, int32_t rank, size_t window_bytes, void* handle_out);
 int alq_comm_connect(alq_ctx* ctx, const void* all_handles);
@@ -395,7 +396,22 @@ int alq_class_pick(alq_ctx* ctx, const int32_t* labels, const uint8_t* avail, in
  * count plus the budget below 2^24 (the fp32 imbalance test is exact there).  Beyond them the call declines
  * (*n_picks_host = -1, nothing drawn) under option 0, 1 or 3 and fails with ALQ_ERR_INVALID under option 2.
  * Launches: K10's table pass (2), one segment count, two fp64 set-up passes and the loop: six, whatever the budget.
- * Synchronous (it reads the label check, the counts and the final RNG state back).                              */
+ * Synchronous (it reads the label check, the counts and the final RNG state back).
+ *
+ * Rows sharded over a group (K11 and K12; shard_off_host non-NULL; needs alq_comm_create/connect).  Every array stays
+ * GLOBAL and REPLICATED on every rank (x, xn, labels, avail, labeled: n rows each); rank r streams rows
+ * [shard_off[r], shard_off[r + 1]) only, so a pick is announced as a row id and read from the local replica.  Every rank
+ * runs the same number of CTAs (from the smallest shard), counts the available rows of every rank's CTA segments and
+ * keeps the same counts, centres or class sums and MT19937 state; a balancing step exchanges one 8-byte key word per CTA
+ * through the peer-memory windows, a random step the owner's pick word.  The words share the window region of the
+ * persistent selection loop (alq_greedy_select) and its start-of-call ready handshake, and their tags carry the call's
+ * epoch.  Picks, the balancing steps and the written-back MT19937 state are identical on every rank and bit-identical to
+ * the single-GPU call on the same inputs; with one rank and shard_off = {0, n} the CTA segments are exactly the
+ * single-GPU ones.  Collective: every rank makes the call with the same inputs (the caller checks that; Engine does),
+ * in the same order relative to its other group calls, and the ranks take the same run-or-decline decision (the shape
+ * limits, the window's room for one word per pick, and K12's memory check on group_free_bytes).  Every wait is bounded
+ * by "spin_timeout_ms": a rank that fails after the decision ends the call with ALQ_ERR_STATE on its peers, never with a
+ * hang.  A descriptor whose struct_size ends before shard_off_host is a single-GPU call.                          */
 typedef struct alq_balancing_desc {
     size_t struct_size;          /* sizeof(alq_balancing_desc) */
     const float* x;  int64_t ldx; int32_t d;
@@ -411,6 +427,9 @@ typedef struct alq_balancing_desc {
     int32_t* picks;              /* [budget] out */
     int64_t* n_picks_host;       /* out: picks written, or -1 when the call declined (option / limits) */
     int64_t* n_balancing_host;   /* out: balancing steps among them */
+    const int32_t* shard_off_host;   /* [world + 1] rows per rank of a sharded call, or NULL: one GPU */
+    int64_t group_free_bytes;    /* sharded K12: the least free device memory (bytes) over the group's ranks, gathered by
+                                    the caller before the call; the table check tests every rank's share against it */
 } alq_balancing_desc;
 
 int alq_balancing_select(alq_ctx* ctx, const alq_balancing_desc* desc, void* stream);
