@@ -1284,6 +1284,12 @@ static int uncertainty_tail_impl(alq_ctx* ctx, const float* logits, int64_t n, i
     }
     if (!fused) {                                   // separate launches: K1, K1b (and the window exchange of the local winners)
         ctx->sel_last_ctr = nullptr;
+        // the window exchange takes at most kTopbWords words per rank: a larger budget is declined before anything runs,
+        // and on every rank alike (the decision only uses c, b, rows_min and rows_max)
+        if (sharded && b > static_cast<int64_t>(AlqComm::kTopbWords))
+            ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_uncertainty_tail_sharded: the launch does not fuse and b = %lld exceeds the %zu "
+                     "words of the window exchange (gather the local winners with alq_topb_pack / alq_topb_merge)", (long long)b,
+                     AlqComm::kTopbWords);
         int rc = alq_score_softmax(ctx, logits, n, c, ld, mode, scores, stream);
         if (rc) return rc;
         if (!sharded) return alq_select_smallest(ctx, scores, n, b, out_pos, stream);

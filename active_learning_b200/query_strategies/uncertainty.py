@@ -11,7 +11,7 @@ from __future__ import annotations
 import numpy as np
 import torch
 
-from .._lib import MODE_ENTROPY, MODE_LEAST_CONFIDENCE, MODE_MARGIN  # noqa: F401
+from .._lib import MODE_ENTROPY, MODE_LEAST_CONFIDENCE, MODE_MARGIN, AlqError  # noqa: F401
 from .strategy import EngineMixin
 
 
@@ -62,13 +62,13 @@ class UncertaintyQuery(EngineMixin):
             import torch.distributed as dist
             sizes = [b_ - a_ for a_, b_ in (group.row_range(n, q) for q in range(group.world_size))]
             dist.barrier(group=group.pg)
-            _, gpos = eng.uncertainty_tail_sharded(logits, self.MODE, budget, lo, min(sizes), max(sizes))
-            host = gpos.cpu().numpy()
             try:
+                _, gpos = eng.uncertainty_tail_sharded(logits, self.MODE, budget, lo, min(sizes), max(sizes))
+                host = gpos.cpu().numpy()
                 eng.comm_check()
                 return host.astype(np.int64) & 0xFFFFFFFF
-            except Exception:                       # a peer never showed up: the collective path below
-                pass
+            except AlqError:                        # a peer never showed up, or a budget above 16 384 that does not
+                pass                                # fuse (declined on every rank alike): the collective path below
         b_loc = min(budget, hi - lo)
         scores, pos_loc = self._tail(eng, logits, b_loc)
         return group.merge_smallest(scores, pos_loc, lo, budget, eng, rendezvous=True)

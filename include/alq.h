@@ -115,8 +115,10 @@ int alq_uncertainty_tail_timing(alq_ctx* ctx, float* out_ms_host);
  * the ranks and the b + few candidate words gathered through the windows from inside the kernel (8-byte {tag, value} words
  * and plain stores over NVLink; no collective library, nothing on the host).  Collective: every rank calls it with the same
  * c, mode, b, rows_min / rows_max (the smallest / largest shard; they decide, identically on every rank, whether the fused
- * kernel applies -- otherwise K1, K1b and alq_topb_exchange run back to back, same result).  Asynchronous; a peer that never
- * shows up is reported through alq_comm_check like alq_topb_exchange.                                              */
+ * kernel applies -- otherwise K1, K1b and alq_topb_exchange run back to back, same result).  The separate launches serve
+ * b <= 16384 only (alq_topb_exchange's limit): a larger b that does not fuse returns ALQ_ERR_INVALID on every rank before
+ * anything runs, and the caller exchanges the local winners itself (alq_topb_pack + alq_topb_merge).  Asynchronous; a
+ * peer that never shows up is reported through alq_comm_check like alq_topb_exchange.                              */
 int alq_uncertainty_tail_sharded(alq_ctx* ctx, const float* logits, int64_t n, int32_t c, int64_t ld, int32_t mode,
                                  int64_t b, int64_t row_lo, int64_t rows_min, int64_t rows_max, float* scores,
                                  int32_t* out_gpos, void* stream);

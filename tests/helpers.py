@@ -3,6 +3,7 @@ embeddings of every pool index, and OracleEngine -- an implementation of the Eng
 CPU tensors built from oracle/al_oracle.py.  OracleEngine exists ONLY so the CPU test tier can
 exercise the samplers' host logic (index bookkeeping, RNG order, partition batching, sharding);
 it is never importable from the product package."""
+import contextlib
 import hashlib
 import tempfile
 
@@ -81,6 +82,36 @@ def tied_tail_pools():
     rng = np.random.default_rng(5)
     for n, c, b in ((60000, 8, 9000), (150000, 4, 12000)):
         yield torch.from_numpy(rng.integers(-2, 3, size=(n, c)).astype(np.float32)).cuda(), b
+
+
+@contextlib.contextmanager
+def one_rank_engine(tmp_dir):
+    """An Engine connected to a gloo group of world size 1 (file rendezvous under `tmp_dir`).  The peer-memory window is
+    then this GPU's own memory, and the sharded calls run the same stores, waits, fences and tags as on a real group."""
+    import torch.distributed as dist
+    from active_learning_b200.engine import Engine
+    dist.init_process_group("gloo", init_method=f"file://{tmp_dir}/init", world_size=1, rank=0)
+    try:
+        e = Engine().comm_init()
+        yield e
+        e.close()
+    finally:
+        dist.destroy_process_group()
+
+
+def tail_rows_per_tile(c):
+    """Rows per tile of the row-pipe plan of the fused tail (alq_score.cu: plan_row_pipe)."""
+    return min(32, max(1, 16384 // (4 * c)))
+
+
+def fuses(n, c):
+    """Whether alq_uncertainty_tail_sharded takes the fused launch for a shard of n rows of width c (rows_min = rows_max =
+    n): the one-GPU rule (c % 4 == 0, c <= 2048, 4096 <= n, 5 n <= sm * 2048 * 4), and at least as many row tiles as SMs
+    (every CTA must stream rows).  On a 132-SM H100 the 4100-row pool of width 12 has 129 tiles and does not fuse."""
+    sm = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
+    if c % 4 or c > 2048 or n < 4096 or n * 5 > sm * 2048 * 4:
+        return False
+    return -(-n // tail_rows_per_tile(c)) >= sm
 
 
 class IndexDataset(torch.utils.data.Dataset):

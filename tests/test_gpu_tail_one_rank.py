@@ -6,7 +6,7 @@ with positions shifted by the shard's row offset."""
 import pytest
 import torch
 
-from helpers import FUSED_TAIL_SHAPES, fused_tail_logits, skewed_tail_pools, tied_tail_pools
+from helpers import FUSED_TAIL_SHAPES, fused_tail_logits, fuses, one_rank_engine, skewed_tail_pools, tied_tail_pools
 
 pytestmark = pytest.mark.gpu
 
@@ -15,27 +15,8 @@ ROW_LO_BIG = (1 << 30) + 7      # global positions stay below 2^31 for every poo
 
 @pytest.fixture(scope="module")
 def eng(tmp_path_factory):
-    import torch.distributed as dist
-    from active_learning_b200.engine import Engine
-    init = tmp_path_factory.mktemp("one_rank_group") / "init"
-    dist.init_process_group("gloo", init_method=f"file://{init}", world_size=1, rank=0)
-    try:
-        e = Engine().comm_init()
+    with one_rank_engine(tmp_path_factory.mktemp("one_rank_group")) as e:
         yield e
-        e.close()
-    finally:
-        dist.destroy_process_group()
-
-
-def fuses(n, c):
-    """Whether alq_uncertainty_tail_sharded takes the fused launch for a shard of n rows of width c (rows_min = rows_max =
-    n): the row-pipe plan's rows per tile, and at least as many row tiles as SMs (every CTA must stream rows).  On a
-    132-SM H100 the 4100-row pool of width 12 has 129 tiles and does not fuse."""
-    sm = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
-    if c % 4 or c > 2048 or n < 4096 or n * 5 > sm * 2048 * 4:
-        return False
-    rows_per_tile = min(32, max(1, 16384 // (4 * c)))
-    return -(-n // rows_per_tile) >= sm
 
 
 def check_one_rank(eng, logits, mode, b):

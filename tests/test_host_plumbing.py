@@ -303,3 +303,37 @@ def test_update_is_vectorised_with_the_reference_assertion(gold):
     with pytest.raises(AssertionError):
         s.update(np.array([other[0], other[1], other[0]]), 3)   # repeated inside one call
     s.update(np.array([], dtype=np.int64), 0)                   # empty round
+
+
+class _DecliningTailEngine(OracleEngine):
+    """A peer-memory engine whose sharded tail declines the way libalq does when the launch does not fuse and the budget
+    exceeds the 16 384 words of the window exchange."""
+    comm_ready = True
+    declined = 0
+
+    def uncertainty_tail_sharded(self, logits, mode, b, row_lo, rows_min, rows_max, scores_out=None):
+        from active_learning_b200._lib import AlqError
+        self.declined += 1
+        raise AlqError(f"alq_uncertainty_tail_sharded: ALQ_ERR_INVALID: the launch does not fuse and b = {b} exceeds the "
+                       f"16384 words of the window exchange")
+
+
+def test_sharded_uncertainty_query_falls_back_when_the_tail_declines(tmp_path):
+    """UncertaintyQuery._query_sharded on a pool whose width never fuses (c = 10) with a budget above 16 384: the sharded
+    tail declines, and the query gathers the local winners through ShardGroup.merge_smallest's collective path instead of
+    raising.  The picks are the single-process stable selection."""
+    import torch.distributed as dist
+    from active_learning_b200.sharding import ShardGroup
+    n, c, budget = 20000, 10, 17000
+    logits = torch.from_numpy(np.random.default_rng(3).integers(-2, 3, size=(n, c)).astype(np.float32))
+    eng = _DecliningTailEngine()
+    dist.init_process_group("gloo", init_method=f"file://{tmp_path}/init", world_size=1, rank=0)
+    try:
+        s = make_strategy("MarginSampler", logits, torch.zeros(n, 4), [], [], 4096, engine=eng)
+        s._shard_group = ShardGroup()
+        idxs = s.available_query_idxs(boolean=False, shuffle=False)
+        pos = s._query_sharded(idxs, budget, s._shard_group)
+    finally:
+        dist.destroy_process_group()
+    assert eng.declined == 1
+    assert np.array_equal(pos, O.select_smallest(O.softmax_scores(logits, O.MODE_MARGIN, batch_size=4096), budget))
