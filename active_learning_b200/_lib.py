@@ -122,6 +122,10 @@ SIGNATURES = {
     "alq_pdist_f64_condensed": (C.c_int, [C.c_void_p, c_f32p, C.c_int64, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p]),
     "alq_ward_nn_chain_condensed": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, c_i32p, C.c_void_p, C.c_void_p]),
     "alq_ward_labels": (C.c_int, [c_i32p, C.c_void_p, C.c_int64, C.c_int32, c_i32p]),
+    "alq_pdist_f64_condensed_rows": (C.c_int, [C.c_void_p, c_f32p, C.c_int64, C.c_int32, C.c_int64, C.c_int64, C.c_int64,
+                                               C.c_void_p, C.c_void_p]),
+    "alq_pdist_f64_expand": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_int64,
+                                       C.c_void_p]),
     "alq_vaal_scores": (C.c_int, [C.c_void_p, c_f32p, C.c_int64, C.c_int32, C.c_int64, c_f32p, C.c_int64, c_f32p,
                                   c_f32p, C.c_int64, c_f32p, c_f32p, c_f32p, C.c_int32, c_f32p, c_f32p, C.c_void_p]),
     "alq_class_counts": (C.c_int, [C.c_void_p, c_i32p, C.c_void_p, C.c_int64, C.c_int32, c_i32p, C.c_void_p]),

@@ -73,10 +73,20 @@ __device__ __forceinline__ void cp_async4(void* smem, const void* gmem, bool pre
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
+// The band of rows [b.row_lo, b.row_hi): the grid's tile rows start at b.tile_lo = row_lo / PD_TILE, and in the
+// condensed layout (i, j) lands at cidx(i, j) - b.base, base = cidx(row_lo, row_lo + 1), so a band is one contiguous
+// slice of scipy's vector.  The square layout always takes the whole matrix and reads no field of b.
+struct Band {
+    int row_lo, row_hi, tile_lo;
+    int64_t base;
+};
+
 template <bool CONDENSED>
 __global__ void __launch_bounds__(PD_THREADS, 2)
-pdist_f64_kernel(const float* __restrict__ x, int n, int d, int64_t ldx, double* __restrict__ dist, int64_t ldd) {
-    const int ti = blockIdx.y, tj = blockIdx.x;
+pdist_f64_kernel(const float* __restrict__ x, int n, int d, int64_t ldx, double* __restrict__ dist, int64_t ldd,
+                 const Band band) {
+    const int ti = CONDENSED ? band.tile_lo + static_cast<int>(blockIdx.y) : static_cast<int>(blockIdx.y);
+    const int tj = blockIdx.x;
     if (ti > tj) return;                                   // upper triangle of tiles only
     __shared__ float s32[2][2][PD_KC][PD_PAD];             // [stage][operand][k][row]
     __shared__ double s64[2][PD_KC][PD_TILE];              // [operand][k][row]
@@ -139,13 +149,51 @@ pdist_f64_kernel(const float* __restrict__ x, int n, int d, int64_t ldx, double*
         for (int b = 0; b < 4; ++b) {
             const int j = row_j + tx + 16 * b;
             if constexpr (CONDENSED) {                     // no diagonal; consecutive tx: consecutive j
-                if (i < j && j < n) dist[cidx(i, j, n)] = __dsqrt_rn(acc[a][b]);
+                if (band.row_lo <= i && i < band.row_hi && i < j && j < n)
+                    dist[cidx(i, j, n) - band.base] = __dsqrt_rn(acc[a][b]);
             } else if (i < n && j < n && (ti != tj || i <= j)) {
                 const double v = __dsqrt_rn(acc[a][b]);
                 dist[static_cast<int64_t>(i) * ldd + j] = v;
                 dist[static_cast<int64_t>(j) * ldd + i] = v;
             }
         }
+    }
+}
+
+// The square matrix from condensed bands: for i in [row_lo, row_hi), j > i, dist[i, j] = dist[j, i] = the band's entry
+// and dist[i, i] = 0.0.  HBM-bound; one CTA per 64 x 64 tile of the upper triangle, staged in shared memory so that the
+// row-wise stores (consecutive threads: consecutive j) and the transposed ones (consecutive i) are both coalesced.
+constexpr int EX_TILE = 64;
+constexpr int EX_THREADS = 256;
+constexpr int EX_ROWS = EX_THREADS / EX_TILE;              // tile rows per pass
+
+__global__ void __launch_bounds__(EX_THREADS)
+pdist_expand_kernel(const double* __restrict__ rows, int n, int row_lo, int row_hi, double* __restrict__ dist,
+                    int64_t ldd) {
+    const int ti = blockIdx.y + row_lo / EX_TILE, tj = blockIdx.x;
+    if (ti > tj) return;
+    __shared__ double t[EX_TILE][EX_TILE + 1];             // odd pitch: the transposed reads are conflict-free
+    const int c = threadIdx.x % EX_TILE, r0 = threadIdx.x / EX_TILE;
+    const int64_t base = cidx(row_lo, row_lo + 1, n);
+    const int j = tj * EX_TILE + c;
+#pragma unroll 4
+    for (int r = r0; r < EX_TILE; r += EX_ROWS) {
+        const int i = ti * EX_TILE + r;
+        if (i < row_lo || i >= row_hi || j >= n || j < i) continue;
+        if (j == i) {
+            dist[static_cast<int64_t>(i) * ldd + i] = 0.0;
+            continue;
+        }
+        const double v = rows[cidx(i, j, n) - base];
+        dist[static_cast<int64_t>(i) * ldd + j] = v;
+        t[r][c] = v;
+    }
+    __syncthreads();
+#pragma unroll 4
+    for (int r = r0; r < EX_TILE; r += EX_ROWS) {          // row jj of the tile's mirror, consecutive threads: consecutive i
+        const int jj = tj * EX_TILE + r, i = ti * EX_TILE + c;
+        if (i < row_lo || i >= row_hi || jj >= n || jj <= i) continue;
+        dist[static_cast<int64_t>(jj) * ldd + i] = t[c][r];
     }
 }
 
@@ -404,15 +452,20 @@ void heap_pushpop(std::vector<int64_t>& h, int64_t item) {
     }
 }
 
-// K7 / K8 launches for either layout; `name` is the entry point's, for its error messages
+// K7 launches for either layout over the rows [row_lo, row_hi) (the square layout always takes [0, n)); `name` is the
+// entry point's, for its error messages
 template <bool CONDENSED>
 int pdist_run(alq_ctx* ctx, const char* name, const float* x, int64_t n, int32_t d, int64_t ldx, double* dist, int64_t ldd,
-              void* stream) {
+              int64_t row_lo, int64_t row_hi, void* stream) {
     const int64_t nt = (n + PD_TILE - 1) / PD_TILE;
     if (nt > 65535) ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: n=%lld exceeds %d rows", name, (long long)n, 65535 * PD_TILE);
+    const int64_t t0 = row_lo / PD_TILE, t1 = (row_hi + PD_TILE - 1) / PD_TILE;
+    if (t1 <= t0) return ALQ_OK;                           // an empty band writes nothing
     ALQ_CUDA(ctx, cudaSetDevice(ctx->device));
-    pdist_f64_kernel<CONDENSED><<<dim3(static_cast<unsigned>(nt), static_cast<unsigned>(nt)), PD_THREADS, 0,
-                                  static_cast<cudaStream_t>(stream)>>>(x, static_cast<int>(n), d, ldx, dist, ldd);
+    pdist_f64_kernel<CONDENSED><<<dim3(static_cast<unsigned>(nt), static_cast<unsigned>(t1 - t0)), PD_THREADS, 0,
+                                  static_cast<cudaStream_t>(stream)>>>(
+        x, static_cast<int>(n), d, ldx, dist, ldd,
+        Band{static_cast<int>(row_lo), static_cast<int>(row_hi), static_cast<int>(t0), row_lo * n - row_lo * (row_lo + 1) / 2});
     ALQ_LAUNCH_CHECK(ctx);
     return ALQ_OK;
 }
@@ -467,7 +520,7 @@ extern "C" int alq_pdist_f64(alq_ctx* ctx, const float* x, int64_t n, int32_t d,
     if (!x || !dist || n < 1 || d < 1 || ldx < d || ldd < n)
         ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_pdist_f64: bad arguments (n=%lld d=%d ldx=%lld ldd=%lld)", (long long)n, d,
                  (long long)ldx, (long long)ldd);
-    return pdist_run<false>(ctx, "alq_pdist_f64", x, n, d, ldx, dist, ldd, stream);
+    return pdist_run<false>(ctx, "alq_pdist_f64", x, n, d, ldx, dist, ldd, 0, n, stream);
 }
 
 extern "C" int alq_pdist_f64_condensed(alq_ctx* ctx, const float* x, int64_t n, int32_t d, int64_t ldx, double* dist,
@@ -476,7 +529,35 @@ extern "C" int alq_pdist_f64_condensed(alq_ctx* ctx, const float* x, int64_t n, 
     if (!x || !dist || n < 1 || d < 1 || ldx < d)
         ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_pdist_f64_condensed: bad arguments (n=%lld d=%d ldx=%lld)", (long long)n, d,
                  (long long)ldx);
-    return pdist_run<true>(ctx, "alq_pdist_f64_condensed", x, n, d, ldx, dist, 0, stream);
+    return pdist_run<true>(ctx, "alq_pdist_f64_condensed", x, n, d, ldx, dist, 0, 0, n, stream);
+}
+
+extern "C" int alq_pdist_f64_condensed_rows(alq_ctx* ctx, const float* x, int64_t n, int32_t d, int64_t ldx,
+                                            int64_t row_lo, int64_t row_hi, double* dist, void* stream) {
+    if (!ctx) return ALQ_ERR_INVALID;
+    if (!x || !dist || n < 1 || d < 1 || ldx < d || row_lo < 0 || row_hi > n || row_lo > row_hi)
+        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_pdist_f64_condensed_rows: bad arguments (n=%lld d=%d ldx=%lld rows [%lld, %lld))",
+                 (long long)n, d, (long long)ldx, (long long)row_lo, (long long)row_hi);
+    return pdist_run<true>(ctx, "alq_pdist_f64_condensed_rows", x, n, d, ldx, dist, 0, row_lo, row_hi, stream);
+}
+
+extern "C" int alq_pdist_f64_expand(alq_ctx* ctx, const double* rows, int64_t n, int64_t row_lo, int64_t row_hi,
+                                    double* dist, int64_t ldd, void* stream) {
+    if (!ctx) return ALQ_ERR_INVALID;
+    if (!rows || !dist || n < 1 || ldd < n || row_lo < 0 || row_hi > n || row_lo > row_hi)
+        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_pdist_f64_expand: bad arguments (n=%lld ldd=%lld rows [%lld, %lld))",
+                 (long long)n, (long long)ldd, (long long)row_lo, (long long)row_hi);
+    const int64_t nt = (n + EX_TILE - 1) / EX_TILE;
+    if (nt > 65535)
+        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_pdist_f64_expand: n=%lld exceeds %d rows", (long long)n, 65535 * EX_TILE);
+    const int64_t t0 = row_lo / EX_TILE, t1 = (row_hi + EX_TILE - 1) / EX_TILE;
+    if (t1 <= t0) return ALQ_OK;
+    ALQ_CUDA(ctx, cudaSetDevice(ctx->device));
+    pdist_expand_kernel<<<dim3(static_cast<unsigned>(nt), static_cast<unsigned>(t1 - t0)), EX_THREADS, 0,
+                          static_cast<cudaStream_t>(stream)>>>(rows, static_cast<int>(n), static_cast<int>(row_lo),
+                                                               static_cast<int>(row_hi), dist, ldd);
+    ALQ_LAUNCH_CHECK(ctx);
+    return ALQ_OK;
 }
 
 extern "C" int alq_ward_nn_chain(alq_ctx* ctx, double* dist, int64_t n, int64_t ldd, int32_t* merge_xy, double* merge_dist,

@@ -16,6 +16,7 @@ import torch
 
 from . import _lib
 from ._lib import AlqError, GreedyDesc, MODE_ENTROPY, MODE_LEAST_CONFIDENCE, MODE_MARGIN  # noqa: F401
+from .sharding import band_pairs
 
 
 def _ptr(t: Optional[torch.Tensor]):
@@ -350,6 +351,46 @@ class Engine:
         self._check(self.lib.alq_pdist_f64(self._h, _ptr(x), n, d, _ld(x), _ptr(out), out.stride(0), self._stream()),
                     "alq_pdist_f64")
         return out
+
+    def pdist_rows(self, x: torch.Tensor, row_lo: int, row_hi: int, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """K7 over a band of rows: the entries (i, j), row_lo <= i < row_hi, j > i, of pdist(x, condensed=True), bit for
+        bit, as one contiguous fp64 vector (the band's slice of scipy's vector).  `out` may be longer; its tail is left
+        untouched.  An empty band returns an empty vector."""
+        x = _f32c(x, "x")
+        n, d = x.shape
+        lo, hi = int(row_lo), int(row_hi)
+        if not 0 <= lo <= hi <= n:
+            raise AlqError(f"pdist_rows: rows [{lo}, {hi}) are not a band of {n} rows")
+        m = band_pairs(n, lo, hi)
+        if out is None:
+            out = torch.empty(max(m, 1), dtype=torch.float64, device=x.device)[:m]
+        if not out.is_cuda or out.dtype != torch.float64 or out.dim() != 1 or out.shape[0] < m or out.stride(0) != 1:
+            raise AlqError(f"pdist_rows: out must be a contiguous 1-D float64 CUDA tensor of at least {m} entries")
+        if m:
+            self._check(self.lib.alq_pdist_f64_condensed_rows(self._h, _ptr(x), n, d, _ld(x), lo, hi, _ptr(out),
+                                                              self._stream()), "alq_pdist_f64_condensed_rows")
+        return out
+
+    def pdist_expand(self, rows: torch.Tensor, n: int, row_lo: int, row_hi: int, dist: torch.Tensor) -> torch.Tensor:
+        """A band from pdist_rows (rows [row_lo, row_hi) of n) into the square matrix `dist` (row-major fp64, at least
+        n x n): both (i, j) and (j, i) of every pair of the band, and 0.0 on the band's diagonal.  Bands covering [0, n)
+        give exactly pdist(x).  Returns `dist`."""
+        n, lo, hi = int(n), int(row_lo), int(row_hi)
+        if not 0 <= lo <= hi <= n:
+            raise AlqError(f"pdist_expand: rows [{lo}, {hi}) are not a band of {n} rows")
+        m = band_pairs(n, lo, hi)
+        if not rows.is_cuda or rows.dtype != torch.float64 or rows.dim() != 1 or rows.shape[0] < m or rows.stride(0) != 1:
+            raise AlqError(f"pdist_expand: rows must be a contiguous 1-D float64 CUDA tensor of at least {m} entries")
+        if (not dist.is_cuda or dist.dtype != torch.float64 or dist.dim() != 2 or dist.shape[0] < n or dist.shape[1] < n
+                or dist.stride(1) != 1 or dist.stride(0) < n):
+            raise AlqError("pdist_expand: dist must be a row-major float64 CUDA tensor of at least n x n")
+        if hi > lo:
+            # the band [n - 1, n) holds no pair, only a diagonal entry: its rows are never read, and an empty tensor's
+            # data_ptr is null, which the library refuses -- any device address stands in
+            src = _ptr(rows) if m else _ptr(dist)
+            self._check(self.lib.alq_pdist_f64_expand(self._h, src, n, lo, hi, _ptr(dist), dist.stride(0),
+                                                      self._stream()), "alq_pdist_f64_expand")
+        return dist
 
     @staticmethod
     def condensed_rows(length: int) -> int:

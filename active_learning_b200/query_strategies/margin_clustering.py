@@ -10,6 +10,11 @@ nearest-neighbour chain in one launch; the merge tree is scipy's bit for bit, so
 condensed vector (4 n (n - 1) bytes) otherwise, so on an 80 GB card the limit is about 140 000 rows (computed from the
 card's memory, not measured), enough for ImageNet-LT's whole train set with subset_unlabeled unset; beyond it the query
 raises AlqError.  The round robin is O(n log n) host NumPy over n margins.
+
+In a ShardGroup of G > 1 ranks (with an engine that has the band kernel, `pdist_rows`) each rank forwards and scores its
+row_range of the HAC rows, one all_gather_rows replicates the margins (and, in a round that clusters, the embeddings),
+and ShardGroup.ward_labels splits K7 by pair-balanced bands of rows, sends the bands to rank 0 for K8 and broadcasts the
+labels; every rank then runs the same round robin and returns the one-GPU picks.
 """
 from __future__ import annotations
 
@@ -60,15 +65,20 @@ class MarginClusteringQuery(EngineMixin):
         self.cluster_assignment = None
 
     # ---- margin_clustering_sampler.py:47-90 --------------------------------------------------------------
+    def _hac_rows(self):
+        if self.subset_unlabeled is None:
+            return self.available_query_idxs(boolean=False, shuffle=False)
+        return sorted(self.available_query_idxs(boolean=False, shuffle=True)[:self.subset_unlabeled])
+
     def query(self, budget):
         group = getattr(self, "_shard_group", None)
         if group is not None and group.world_size > 1:
-            raise AlqError("MarginClusteringSampler runs on one GPU: the nearest-neighbour chain of Ward clustering is "
-                           "sequential over the whole pool; query it from a single rank")
-        if self.subset_unlabeled is None:
-            idxs_for_hac = self.available_query_idxs(boolean=False, shuffle=False)
-        else:
-            idxs_for_hac = sorted(self.available_query_idxs(boolean=False, shuffle=True)[:self.subset_unlabeled])
+            if not hasattr(self.get_engine(), "pdist_rows"):
+                raise AlqError("MarginClusteringSampler runs on one GPU with this engine: it has no band kernel "
+                               "(pdist_rows) to split Ward clustering's distances over a group; query it from a single "
+                               "rank")
+            return self._query_sharded(budget, group)
+        idxs_for_hac = self._hac_rows()
         eng = self.get_engine()
         self.feature_net.eval()
         logits, emb = self._forward_pool(idxs_for_hac, self.feature_net, want_features=True)
@@ -82,3 +92,25 @@ class MarginClusteringQuery(EngineMixin):
         picks, self.cluster_assignment = round_robin(cluster_assignment, margins, budget)
         query_idxs = list(np.asarray(idxs_for_hac, dtype=np.int64)[picks])
         return query_idxs, budget
+
+    # -- row-sharded variant: each rank forwards and scores n/G rows, K7 by bands, K8 on rank 0 ---------------
+    def _query_sharded(self, budget, group):
+        from ..sharding import digest
+        idxs_for_hac = self._hac_rows()            # the same NumPy draws on every rank; ward_labels checks the digest
+        n = len(idxs_for_hac)
+        lo, hi = group.row_range(n)
+        counts = [b - a for a, b in (group.row_range(n, r) for r in range(group.world_size))]
+        clusters = self.cluster_assignment is None or bool(self.subset_unlabeled)
+        eng = self.get_engine()
+        self.feature_net.eval()
+        logits, emb = self._forward_pool(idxs_for_hac[lo:hi], self.feature_net, want_features=True)
+        margins = group.all_gather_rows(eng.score_softmax(logits, MODE_MARGIN), counts).cpu().numpy()
+        if clusters:
+            x = group.all_gather_rows(emb, counts)
+            cluster_assignment = group.ward_labels(x, N_CLUSTERS, eng,
+                                                   rows_digest=digest(np.asarray(idxs_for_hac, dtype=np.int64)))
+        else:
+            cluster_assignment = self.cluster_assignment
+        budget = int(min(n, budget))
+        picks, self.cluster_assignment = round_robin(cluster_assignment, margins, budget)
+        return list(np.asarray(idxs_for_hac, dtype=np.int64)[picks]), budget

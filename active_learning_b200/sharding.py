@@ -4,7 +4,9 @@ independent, so the data path needs no collective; what is exchanged is
 
   * uncertainty samplers : each rank's local top-B (score, global position) -> one all-gather of
                            G*B 12-byte records -> the same stable merge on every rank;
-  * partitioned samplers : partition i runs on rank i % G; the picked row lists are gathered once.
+  * partitioned samplers : partition i runs on rank i % G; the picked row lists are gathered once;
+  * Ward clustering      : K7 by pair-balanced bands of rows (ward_bands), each band sent to rank 0 in chunks, K8 on
+                           rank 0, the n labels broadcast back (ShardGroup.ward_labels).
 
 Works with backend "nccl" (GPU) and "gloo" (the CPU tests of this host logic).
 """
@@ -101,6 +103,77 @@ def balancing_agreement(what: str, shape, num_classes: int, budget: int, shard_o
     return min(check_replicated(what, record, int(free_bytes), process_group))
 
 
+WARD_CHUNK_BYTES = 1 << 30      # largest piece of a K7 band in flight between two ranks (two such buffers per peer)
+
+
+def band_pairs(n: int, lo: int, hi: int) -> int:
+    """Pairs (i, j), lo <= i < hi, j > i, of n rows: the entries rows [lo, hi) occupy in scipy's condensed vector."""
+    n, lo, hi = int(n), int(lo), int(hi)
+    return (hi - lo) * (n - 1) - (hi * (hi - 1) - lo * (lo - 1)) // 2
+
+
+def ward_bands(n: int, world: int) -> list:
+    """[world + 1] row offsets splitting K7's n (n - 1) / 2 pairs over `world` ranks: from 0 to n, never decreasing,
+    interior cuts on multiples of 64 (K7's tile rows stay whole), each band within one tile row (64 n pairs) of an equal
+    share.  Row i carries n - 1 - i pairs, so the early bands hold fewer rows.  Bands may be empty for small n."""
+    n, world = int(n), int(world)
+    total = n * (n - 1) // 2
+    cuts = np.arange(0, n + 1, 64, dtype=np.int64)                     # candidate interior cuts
+    before = cuts * (n - 1) - cuts * (cuts - 1) // 2                   # pairs above each candidate, increasing
+    out = [0]
+    for r in range(1, world):
+        want = r * total                                               # world * (pairs before the cut), exactly
+        k = int(np.searchsorted(before * world, want))
+        if k == len(cuts) or (k > 0 and want - before[k - 1] * world <= before[k] * world - want):
+            k -= 1
+        out.append(max(int(cuts[k]), out[-1]))
+    out.append(n)
+    return out
+
+
+def ward_chunks(n: int, lo: int, hi: int, max_bytes: int) -> list:
+    """Rows [lo, hi) of a K7 band cut into consecutive (a, b) pieces of at most max_bytes of fp64 pairs each (at least
+    one row per piece), cut on multiples of 64 where that keeps a piece non-empty.  Sender and receiver derive the same
+    pieces from (n, lo, hi, max_bytes)."""
+    out, a = [], int(lo)
+    cap = max(1, int(max_bytes) // 8)
+    while a < hi:
+        b, top = a + 1, int(hi)                                        # largest b with band_pairs(a, b) <= cap
+        while b < top:
+            mid = (b + top + 1) // 2
+            if band_pairs(n, a, mid) <= cap:
+                b = mid
+            else:
+                top = mid - 1
+        if b < hi and b - b % 64 > a:
+            b -= b % 64
+        out.append((a, b))
+        a = b
+    return out
+
+
+def ward_receive_order(plan: list) -> list:
+    """The order in which rank 0 takes in the peers' chunks: (rank, a, b), round robin over the ranks -- chunk k of every
+    rank r >= 1 before chunk k + 1 of any -- so that all peers, each sending its chunks in order from two buffers, make
+    progress at the same time.  `plan[r]` is rank r's ward_chunks list."""
+    out = []
+    for k in range(max((len(p) for p in plan[1:]), default=0)):
+        out.extend((r, *plan[r][k]) for r in range(1, len(plan)) if k < len(plan[r]))
+    return out
+
+
+def ward_group_layout(n: int, free_bytes: int, staging_bytes: int) -> str:
+    """Rank 0's layout in ShardGroup.ward_labels: the n x n matrix when it fits `free_bytes` together with the staging
+    buffers it needs (`staging_bytes`), else scipy's condensed vector (which needs none) when that fits, else the
+    AlqError of Engine.ward_layout naming n and both byte counts."""
+    from .engine import Engine
+    if Engine.ward_bytes(n) + staging_bytes <= free_bytes:
+        return "square"
+    if Engine.ward_condensed_bytes(n) <= free_bytes:
+        return "condensed"
+    return Engine.ward_layout(n, free_bytes)          # raises: neither fits
+
+
 class ShardGroup:
     def __init__(self, process_group=None):
         if not dist.is_initialized():
@@ -191,3 +264,166 @@ class ShardGroup:
             for k, v in d.items():
                 merged[int(k)] = np.asarray(v, dtype=np.int64)
         return merged
+
+    # ---- Ward clustering (MarginClusteringSampler) ---------------------------------------------------
+    def ward_labels(self, x, n_clusters, engine, rows_digest=""):
+        """sklearn's AgglomerativeClustering(n_clusters) labels of the replicated rows x [n, D], on every rank, with K7
+        split over the ranks: rank r computes the pairs of its ward_bands(n, G) band (engine.pdist_rows) in chunks of
+        at most WARD_CHUNK_BYTES and sends them to rank 0, which assembles the distances (the n x n matrix through
+        engine.pdist_expand when it fits, else scipy's condensed vector), runs K8 (engine.nn_chain) and the labelling,
+        and broadcasts the labels.  The labels are those of Engine.ward_labels on one GPU.
+
+        Transfer: every peer computes its chunks in order into two buffers and sends each to rank 0 as it is done
+        (it waits on the send of two chunks earlier before reusing a buffer).  Rank 0 computes its own band on a side
+        stream, so that no receive waits behind it, and takes in the peers' chunks round robin (ward_receive_order):
+        condensed, all receives are posted at once, each into its slice of the vector; square, they go through two
+        staging buffers, the next chunk received while the previous one is expanded.  An unexpected runtime error in
+        the middle of the transfer (the arguments and buffers are checked before it) leaves the other side waiting on
+        its send or receive until the process group's timeout; errors before the transfer and in K8 reach every rank.
+
+        `rows_digest` names the pool rows of x (the caller's digest of their positions): the ranks must agree on it.
+        ValueError on every rank for fewer than max(2, n_clusters) rows or non-finite rows (sklearn's errors); AlqError on
+        every rank, before any distance is sent, if the ranks disagree on n, d or the rows, if a rank cannot reserve
+        its buffers, or if rank 0's memory fits neither layout; AlqError with rank 0's message if K8 fails there."""
+        from ._lib import AlqError
+        from .engine import Engine
+        n, d = int(x.shape[0]), int(x.shape[1])
+        if n < max(2, int(n_clusters)):
+            raise ValueError(f"cannot extract {n_clusters} clusters from {n} rows")
+        if not bool(torch.isfinite(x).all()):
+            raise ValueError("ward: the embeddings contain NaN or infinity")
+        world, rank = self.world_size, self.rank
+        bands = ward_bands(n, world)
+        plan = [ward_chunks(n, bands[r], bands[r + 1], WARD_CHUNK_BYTES) for r in range(world)]
+        piece = max([band_pairs(n, a, b) for p in plan for a, b in p] + [1])      # entries of the largest chunk
+        nbufs = 2 if world == 1 else 4              # square layout on rank 0: its own band's pair, the receiving pair
+        staging = nbufs * 8 * piece
+
+        # reserve this rank's buffers (rank 0: D too) before the agreement, so that a failure is raised on every rank
+        # there rather than leaving the other ranks waiting on a send or a receive
+        free, err, bufs, hold = 0, None, [], []
+        layout0 = None
+        if rank == 0:
+            free = int(engine._ward_free_bytes())
+            try:
+                layout0 = ward_group_layout(n, free, staging)
+            except AlqError:
+                pass                                   # neither layout fits: the agreement raises it on every rank
+        try:
+            if rank != 0:
+                engine.pdist_rows(x, bands[rank], bands[rank])      # the engine's argument checks, on an empty band
+            elif layout0 == "square":
+                hold.append(torch.empty((n, n), dtype=torch.float64, device=x.device))
+            elif layout0 == "condensed":
+                hold.append(torch.empty(n * (n - 1) // 2, dtype=torch.float64, device=x.device))
+            if rank != 0 or layout0 == "square":                    # the staging buffers
+                bufs = [torch.empty(piece, dtype=torch.float64, device=x.device)
+                        for _ in range(2 if rank != 0 else nbufs)]
+        except Exception as exc:                       # noqa: BLE001 -- e.g. CUDA out of memory
+            err = f"rank {rank}: {type(exc).__name__}: {exc}"
+        try:
+            record = {"n, d": (n, d), "rows": str(rows_digest), "n_clusters": int(n_clusters)}
+            locals_ = check_replicated("ward_labels", record, (free, err), self.pg)
+            errs = [e for _, e in locals_ if e]
+            if errs:
+                raise AlqError("ward_labels: a rank could not reserve its K7 buffers: " + "; ".join(errs))
+            layout = ward_group_layout(n, locals_[0][0], staging)     # the same decision (or error) on every rank
+
+            if rank != 0:
+                sends = []
+                for k, (a, b) in enumerate(plan[rank]):
+                    if band_pairs(n, a, b) == 0:
+                        continue                       # row n - 1 alone: nothing to send (rank 0 skips it too)
+                    if len(sends) >= 2:
+                        sends[-2].wait()               # the send of two chunks ago released this buffer
+                    buf = bufs[k % 2][:band_pairs(n, a, b)]
+                    engine.pdist_rows(x, a, b, out=buf)
+                    sends.append(dist.isend(buf, dst=self._global_rank(0), group=self.pg))
+                for w in sends[-2:]:
+                    w.wait()
+                box = [None]
+            else:
+                box = [self._ward_rank0(x, n, int(n_clusters), engine, layout, plan, bufs, hold)]
+        finally:
+            bufs.clear()
+            on_device = bool(hold) and hold[0].is_cuda
+            hold.clear()
+            if on_device:
+                torch.cuda.empty_cache()               # rank 0's distances go back to the device (as Engine.ward_tree)
+        dist.broadcast_object_list(box, src=self._global_rank(0), group=self.pg)
+        msg, labels = box[0]
+        if msg is not None:
+            raise AlqError(f"ward_labels on rank 0: {msg}")
+        return np.asarray(labels).astype(np.int64)
+
+    def _global_rank(self, r):
+        return r if self.pg is None else dist.get_global_rank(self.pg, r)
+
+    def _ward_rank0(self, x, n, n_clusters, engine, layout, plan, bufs, hold):
+        """Rank 0's half of ward_labels: its own band and every peer's chunks into D = hold[0], K8, the labels.  Returns
+        (error message or None, labels as int32); D is released by the caller."""
+        import contextlib
+        from .engine import ward_labels_host
+        D = hold[0]
+        cur = torch.cuda.current_stream(D.device) if D.is_cuda else None
+        side = torch.cuda.Stream(device=D.device) if D.is_cuda else None
+        try:
+            square = layout == "square"
+            own, recv = bufs[-2:], bufs[:2]             # the same pair when there are no peers
+            if side is not None:
+                side.wait_stream(cur)                   # x and D are ready on the current stream
+            # rank 0's own band, on the side stream: an NCCL receive waits for the stream it is posted from, so on the
+            # current stream every receive would wait for the whole band
+            with torch.cuda.stream(side) if side is not None else contextlib.nullcontext():
+                for j, (a, b) in enumerate(plan[0]):
+                    m = band_pairs(n, a, b)
+                    if square:
+                        buf = own[j % 2][:m]
+                        engine.pdist_rows(x, a, b, out=buf)
+                        engine.pdist_expand(buf, n, a, b, D)
+                    else:
+                        at = band_pairs(n, 0, a)
+                        engine.pdist_rows(x, a, b, out=D[at:at + m])
+            src = {r: self._global_rank(r) for r in range(1, len(plan))}
+            order = ward_receive_order(plan)
+            if not square:                              # every receive straight into its slice, all in flight at once
+                works = []
+                for r, a, b in order:
+                    m, at = band_pairs(n, a, b), band_pairs(n, 0, a)
+                    if m:
+                        works.append(dist.irecv(D[at:at + m], src=src[r], group=self.pg))
+                for w in works:
+                    w.wait()
+            else:
+                def post(k):
+                    """Receive chunk k of the order into staging buffer k % 2 (a pairless chunk, row n - 1 alone, is
+                    not sent: only its diagonal entry is written)."""
+                    r, a, b = order[k]
+                    m = band_pairs(n, a, b)
+                    dst = recv[k % 2][:m]
+                    return dst, (dist.irecv(dst, src=src[r], group=self.pg) if m else None)
+
+                pending = post(0) if order else None
+                for k in range(len(order)):
+                    # chunk k + 1 is posted before chunk k is expanded: its buffer's last reader, the expand of chunk
+                    # k - 1, is already on the stream ahead of it
+                    nxt = post(k + 1) if k + 1 < len(order) else None
+                    dst, work = pending
+                    if work is not None:
+                        work.wait()
+                    _, a, b = order[k]
+                    engine.pdist_expand(dst, n, a, b, D)
+                    pending = nxt
+            if side is not None:
+                cur.wait_stream(side)
+            own, recv = [], []
+            bufs.clear()
+            xy, md = engine.nn_chain(D, n)
+            xy = xy.cpu().numpy() if isinstance(xy, torch.Tensor) else np.asarray(xy)
+            md = md.cpu().numpy() if isinstance(md, torch.Tensor) else np.asarray(md)
+            return None, ward_labels_host(xy, md, n, n_clusters).astype(np.int32)
+        except Exception as exc:                       # noqa: BLE001 -- every rank raises rank 0's message
+            return f"{type(exc).__name__}: {exc}", None
+        finally:
+            if side is not None:
+                cur.wait_stream(side)                   # nothing on the side stream outlives D and the buffers

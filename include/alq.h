@@ -314,6 +314,18 @@ int alq_base_select(alq_ctx* ctx, const float* min_margin, const float* radius, 
  *   entries (4 n (n - 1) bytes, half the square matrix: 25.6 GB at n = 80 000, 53.7 GB at n = 115 846).  Nothing past
  *   them is written.  Same arguments, limits and caller-owned buffer as alq_pdist_f64, without ldd.  Offsets are
  *   int64 (the vector passes 2^31 entries at n = 65 537).
+ * alq_pdist_f64_condensed_rows (K7, a band of rows): the entries (i, j), row_lo <= i < row_hi, j > i, of the condensed
+ *   vector -- bit for bit those alq_pdist_f64_condensed writes (a pair's sum does not depend on the tile computing it)
+ *   -- at dist[cidx(i, j) - cidx(row_lo, row_lo + 1)], cidx(i, j) = n*i - i*(i+1)/2 + (j - i - 1): the band is one
+ *   contiguous slice of cidx(row_hi, row_hi + 1) - cidx(row_lo, row_lo + 1) entries, nothing past it is written.
+ *   Bands that cover [0, n) concatenate to alq_pdist_f64_condensed's vector.  An empty band (row_lo == row_hi) is
+ *   valid and writes nothing.  ALQ_ERR_INVALID for row_lo < 0, row_hi > n, row_lo > row_hi, null pointers, and as
+ *   alq_pdist_f64_condensed.  This is how the ranks of a group split K7 (sharding.py: ShardGroup.ward_labels).
+ * alq_pdist_f64_expand: a condensed band as alq_pdist_f64_condensed_rows writes it (`rows`, same n, row_lo, row_hi)
+ *   into the square matrix: dist[i, j] = dist[j, i] = its entry for row_lo <= i < row_hi and every j > i, and
+ *   dist[i, i] = 0.0 (row-major, ldd >= n).  Nothing else is written.  Expanding bands that cover [0, n) gives exactly
+ *   what alq_pdist_f64 writes, diagonal included.  HBM-bound (64 x 64 tiles staged through shared memory, so the
+ *   row-wise and the mirrored stores are both coalesced).  Same argument checks as the band call, plus ldd < n.
  * alq_ward_nn_chain (K8): scipy's nn_chain with the Ward update, in ONE launch of one thread-block cluster, consuming
  *   `dist` in place (its contents are unspecified afterwards).  merge_xy[k] = (x, y) with x < y and merge_dist[k], for
  *   k < n - 1, in the chain's discovery order (before scipy's sort).  n >= 2.  Synchronous; ALQ_ERR_NUMERIC if a scan
@@ -333,6 +345,10 @@ int alq_ward_nn_chain(alq_ctx* ctx, double* dist, int64_t n, int64_t ldd, int32_
 int alq_pdist_f64_condensed(alq_ctx* ctx, const float* x, int64_t n, int32_t d, int64_t ldx, double* dist, void* stream);
 int alq_ward_nn_chain_condensed(alq_ctx* ctx, double* dist, int64_t n, int32_t* merge_xy, double* merge_dist,
                                 void* stream);
+int alq_pdist_f64_condensed_rows(alq_ctx* ctx, const float* x, int64_t n, int32_t d, int64_t ldx, int64_t row_lo,
+                                 int64_t row_hi, double* dist, void* stream);
+int alq_pdist_f64_expand(alq_ctx* ctx, const double* rows, int64_t n, int64_t row_lo, int64_t row_hi, double* dist,
+                         int64_t ldd, void* stream);
 int alq_ward_labels(const int32_t* merge_xy_host, const double* merge_dist_host, int64_t n, int32_t n_clusters,
                     int32_t* labels_host);
 
