@@ -17,6 +17,7 @@ ERR_NAMES = {1: "ALQ_ERR_INVALID", 2: "ALQ_ERR_CUDA", 3: "ALQ_ERR_NOMEM", 4: "AL
              5: "ALQ_ERR_NUMERIC"}
 MODE_MARGIN, MODE_LEAST_CONFIDENCE, MODE_ENTROPY = 0, 1, 2
 ABI_VERSION = 10
+IPC_HANDLE_BYTES = 64          # ALQ_IPC_HANDLE_BYTES
 
 c_f32p = C.c_void_p
 c_i32p = C.c_void_p
@@ -126,6 +127,12 @@ SIGNATURES = {
                                                C.c_void_p, C.c_void_p]),
     "alq_pdist_f64_expand": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_int64,
                                        C.c_void_p]),
+    "alq_ward_nn_chain_banded": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, c_i32p, C.c_void_p,
+                                           C.c_void_p]),
+    "alq_band_alloc": (C.c_int, [C.c_void_p, C.c_size_t, C.POINTER(C.c_void_p), C.c_void_p]),
+    "alq_band_open": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p)]),
+    "alq_band_close": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "alq_band_free": (C.c_int, [C.c_void_p, C.c_void_p]),
     "alq_vaal_scores": (C.c_int, [C.c_void_p, c_f32p, C.c_int64, C.c_int32, C.c_int64, c_f32p, C.c_int64, c_f32p,
                                   c_f32p, C.c_int64, c_f32p, c_f32p, c_f32p, C.c_int32, c_f32p, c_f32p, C.c_void_p]),
     "alq_class_counts": (C.c_int, [C.c_void_p, c_i32p, C.c_void_p, C.c_int64, C.c_int32, c_i32p, C.c_void_p]),

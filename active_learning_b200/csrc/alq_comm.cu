@@ -93,3 +93,59 @@ extern "C" int alq_comm_destroy(alq_ctx* ctx) {
     ctx->comm = AlqComm{};
     return ALQ_OK;
 }
+
+// Exportable device memory for one rank's band of Ward's condensed distances (alq_ward_nn_chain_banded): a cudaMalloc
+// allocation of its own, since an IPC handle names the base of an allocation (a sub-allocated block of a caching
+// allocator cannot be exported on its own).
+extern "C" int alq_band_alloc(alq_ctx* ctx, size_t bytes, void** ptr_out, void* handle_out) {
+    if (!ctx) return ALQ_ERR_INVALID;
+    if (!bytes || !ptr_out || !handle_out) ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_band_alloc: bad arguments (bytes=%zu)", bytes);
+    ALQ_CUDA(ctx, cudaSetDevice(ctx->device));
+    void* p = nullptr;
+    if (cudaMalloc(&p, bytes) != cudaSuccess) {
+        cudaGetLastError();
+        ALQ_FAIL(ctx, ALQ_ERR_NOMEM, "alq_band_alloc: allocation of %zu bytes failed", bytes);
+    }
+    cudaIpcMemHandle_t h;
+    if (cudaIpcGetMemHandle(&h, p) != cudaSuccess) {
+        const char* e = cudaGetErrorString(cudaGetLastError());
+        cudaFree(p);
+        ALQ_FAIL(ctx, ALQ_ERR_CUDA, "alq_band_alloc: cudaIpcGetMemHandle failed: %s", e);
+    }
+    memcpy(handle_out, &h, sizeof(h));
+    *ptr_out = p;
+    return ALQ_OK;
+}
+
+extern "C" int alq_band_open(alq_ctx* ctx, const void* handle, void** ptr_out) {
+    if (!ctx) return ALQ_ERR_INVALID;
+    if (!handle || !ptr_out) ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_band_open: bad arguments");
+    ALQ_CUDA(ctx, cudaSetDevice(ctx->device));
+    cudaIpcMemHandle_t h;
+    memcpy(&h, handle, sizeof(h));
+    void* p = nullptr;
+    const cudaError_t e = cudaIpcOpenMemHandle(&p, h, cudaIpcMemLazyEnablePeerAccess);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        ALQ_FAIL(ctx, ALQ_ERR_CUDA, "alq_band_open: cudaIpcOpenMemHandle failed: %s (needs NVLink/PCIe peer access)",
+                 cudaGetErrorString(e));
+    }
+    *ptr_out = p;
+    return ALQ_OK;
+}
+
+extern "C" int alq_band_close(alq_ctx* ctx, void* ptr) {
+    if (!ctx) return ALQ_ERR_INVALID;
+    if (!ptr) ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_band_close: null pointer");
+    ALQ_CUDA(ctx, cudaSetDevice(ctx->device));
+    ALQ_CUDA(ctx, cudaIpcCloseMemHandle(ptr));
+    return ALQ_OK;
+}
+
+extern "C" int alq_band_free(alq_ctx* ctx, void* ptr) {
+    if (!ctx) return ALQ_ERR_INVALID;
+    if (!ptr) ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_band_free: null pointer");
+    ALQ_CUDA(ctx, cudaSetDevice(ctx->device));
+    ALQ_CUDA(ctx, cudaFree(ptr));
+    return ALQ_OK;
+}

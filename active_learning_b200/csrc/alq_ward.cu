@@ -19,11 +19,28 @@
 //   square     the full symmetric n x n matrix, row-major with leading dimension ldd (8 n^2 bytes);
 //   condensed  scipy's pdist vector: (i, j), i < j, at n i - i (i + 1) / 2 + (j - i - 1) (4 n (n - 1) bytes).  Row x
 //              of the symmetric matrix is then the entries (j, x), j < x, one per row j (strided), and (x, j), j > x,
-//              contiguous.
+//              contiguous;
+//   banded     (K8 only) the condensed vector cut into up to ALQ_MAX_WORLD bands of rows, each at its own pointer --
+//              possibly in another GPU's memory, mapped through CUDA IPC (sharding.py: ShardGroup.ward_labels).  Band b
+//              holds rows [cut[b], cut[b + 1]): (i, j), i < j, lies in the band of row i at cidx(i, j) - cidx(cut[b],
+//              cut[b] + 1), exactly where alq_pdist_f64_condensed_rows puts it.  In a scan of row x the contiguous half
+//              lies in x's band and each strided entry (j, x) in j's; a merge's store of (i, b) goes to min(i, b)'s band.
 //
 // Memory ordering of K8 (entries of D written by one SM and read by another): every write happens before a
 // `barrier.cluster.arrive.release` of its CTA and every read after a `barrier.cluster.wait.acquire` of the reader;
 // all reads of D go through ld.global.cg (L2, never a possibly stale L1 line) and all writes through st.global.cg.
+// In the banded layout some bands live in a peer GPU's memory; the same argument holds there unchanged:
+//   * during the launch the CTAs of this one cluster are the only readers and writers of every band: the peer that
+//     owns a band synchronised its stream after its K7 before it handed out the band's handle, and it neither reads,
+//     writes nor frees the band until this rank has broadcast the labels (after this launch has completed);
+//   * the PTX memory model orders accesses by scope, not by where the memory lives: a weak st.global.cg before a
+//     cluster-scope release and a weak ld.global.cg after the matching cluster-scope acquire of another thread of the
+//     same cluster are ordered for every global address, NVLink peer memory included.  No access of another agent
+//     (another GPU, the host) has to be ordered against them, so no gpu- or sys-scope fence is needed.  .cg keeps
+//     the loads out of the SM's L1; a peer's bytes are served by the owning GPU's L2, the one point every access of
+//     this cluster reaches.
+// The peer's K7 writes themselves are complete before the launch: the kernel boundary of K7 and the peer's stream
+// synchronisation order them before the host-side handle exchange, which precedes this launch.
 //
 // Offsets into `dist` are int64 (n^2 passes 2^31 at n = 46 341, n (n - 1) / 2 at n = 65 537); row indices themselves
 // are int32.
@@ -44,17 +61,59 @@ namespace ward {
 __device__ __forceinline__ int64_t cidx(int i, int j, int n) {
     return static_cast<int64_t>(n) * i - static_cast<int64_t>(i) * (i + 1) / 2 + (j - i - 1);
 }
+enum class Layout { SQUARE, CONDENSED, BANDED };
+
+// The banded layout's bands, by value (a __grid_constant__ kernel parameter).  base[b] is band b's pointer minus
+// cidx(cut[b], cut[b] + 1), formed on the host, so that (i, j) of a row i of band b sits at base[b] + cidx(i, j) (the
+// base itself may lie outside the band; only entries of the band's rows are dereferenced).  The cuts past the last
+// band are n, so the band of row r is the number of cut[1 .. ALQ_MAX_WORLD) that are <= r.
+struct Bands {
+    double* base[ALQ_MAX_WORLD];
+    int cut[ALQ_MAX_WORLD + 1];
+};
+
+__device__ __forceinline__ int band_of(const Bands& B, int r) {
+    int b = 0;
+#pragma unroll
+    for (int k = 1; k < ALQ_MAX_WORLD; ++k) b += B.cut[k] <= r;
+    return b;
+}
+
+// base[] of the band of row r for rows visited in ascending order (one thread's strided entries (j, x), j < x, of a scan,
+// or its rows i of a merge): the band index only moves forward and the band's base is kept in a register, so an entry
+// costs one compare and no load
+struct BandCursor {
+    const Bands& B;
+    double* p;
+    int b, next;
+    __device__ __forceinline__ explicit BandCursor(const Bands& bands)
+        : B(bands), p(bands.base[0]), b(0), next(bands.cut[1]) {}
+    __device__ __forceinline__ double* base(int r) {
+        while (r >= next) {
+            next = B.cut[++b + 1];
+            p = B.base[b];
+        }
+        return p;
+    }
+};
+
 // row x's base: (x, j) sits at row + j -- for every j in the square layout, for j > x in the condensed one (where the
 // base itself may lie before D: only row + j, j > x, is ever dereferenced)
-template <bool CONDENSED>
+template <Layout L>
 __device__ __forceinline__ int64_t row_off(int x, int n, int64_t ldd) {
-    if constexpr (CONDENSED) return cidx(x, x + 1, n) - (x + 1);
+    if constexpr (L != Layout::SQUARE) return cidx(x, x + 1, n) - (x + 1);
     else return static_cast<int64_t>(x) * ldd;
 }
-// address of the symmetric entry (x, j), j != x, given row x's base
-template <bool CONDENSED, typename T>
-__device__ __forceinline__ T* at(double* D, T* row, int x, int j, int n) {
-    if constexpr (CONDENSED) return j < x ? D + cidx(j, x, n) : row + j;
+template <Layout L>
+__device__ __forceinline__ double* row_ptr(double* D, const Bands& B, int x, int n, int64_t ldd) {
+    if constexpr (L == Layout::BANDED) return B.base[band_of(B, x)] + row_off<L>(x, n, ldd);
+    else return D + row_off<L>(x, n, ldd);
+}
+// address of the symmetric entry (x, j), j != x, given row x's base (and, banded, the cursor over j's band)
+template <Layout L, typename T>
+__device__ __forceinline__ T* at(double* D, T* row, int x, int j, int n, BandCursor& bc) {
+    if constexpr (L == Layout::BANDED) return j < x ? bc.base(j) + cidx(j, x, n) : row + j;
+    else if constexpr (L == Layout::CONDENSED) return j < x ? D + cidx(j, x, n) : row + j;
     else return row + j;
 }
 
@@ -231,13 +290,14 @@ __device__ __forceinline__ double ward_update(double dxi, double dyi, double dxy
     return __dsqrt_rn(__dsub_rn(__dadd_rn(a, b), c));
 }
 
-// dist: n x n (ldd) or condensed, consumed.  chain_all: [cluster size][n] int2 (index, cluster size), one stack per CTA (every CTA
+// dist: n x n (ldd) or condensed, consumed; banded: D is unused and B names the bands (square and condensed: B is unused).
+// chain_all: [cluster size][n] int2 (index, cluster size), one stack per CTA (every CTA
 // walks the same chain; private copies need no cross-CTA ordering).  status: 0, or ALQ_ERR_NUMERIC if a scan of a
 // one-element chain found no finite candidate (non-finite distances).
-template <bool CONDENSED>
+template <Layout L>
 __global__ void __launch_bounds__(NC_THREADS, 1)
 ward_chain_kernel(double* __restrict__ D, int n, int64_t ldd, int2* __restrict__ chain_all, int32_t* __restrict__ merge_xy,
-                  double* __restrict__ merge_dist, int* __restrict__ status) {
+                  double* __restrict__ merge_dist, int* __restrict__ status, const __grid_constant__ Bands B) {
     extern __shared__ int sz[];                            // cluster sizes of this CTA's columns, 0 = merged away
     __shared__ Cand part[2];                               // this CTA's scan result, double-buffered across scans
     __shared__ Cand wpart[NC_WARPS];
@@ -274,18 +334,25 @@ ward_chain_kernel(double* __restrict__ D, int n, int64_t ldd, int2* __restrict__
 #pragma unroll 1
         while (true) {
             // ---- scan row x over this CTA's live columns -------------------------------------------------------
-            const double* row = D + row_off<CONDENSED>(x, n, ldd);
+            const double* row = row_ptr<L>(D, B, x, n, ldd);
+            BandCursor bc(B);
             Cand c{CUDART_INF, INT_MAX, 0};
             int i = lo + tid;
 #pragma unroll 1
             for (; i + 3 * NC_THREADS < hi; i += 4 * NC_THREADS) {
                 double v[4];
                 bool live[4];
-#pragma unroll
+                const double* ad[4];                       // banded: the cursor's branches come before the four
+#pragma unroll                                             // loads, not between them
                 for (int u = 0; u < 4; ++u) {
                     const int j = i + u * NC_THREADS;
                     live[u] = sz[j - lo] > 0 && j != x;
-                    v[u] = live[u] ? __ldcg(at<CONDENSED>(D, row, x, j, n)) : CUDART_INF;
+                    if constexpr (L == Layout::BANDED) ad[u] = at<L>(D, row, x, j, n, bc);
+                    else v[u] = live[u] ? __ldcg(at<L>(D, row, x, j, n, bc)) : CUDART_INF;
+                }
+                if constexpr (L == Layout::BANDED) {
+#pragma unroll
+                    for (int u = 0; u < 4; ++u) v[u] = live[u] ? __ldcg(ad[u]) : CUDART_INF;
                 }
 #pragma unroll
                 for (int u = 0; u < 4; ++u)
@@ -294,7 +361,7 @@ ward_chain_kernel(double* __restrict__ D, int n, int64_t ldd, int2* __restrict__
             for (; i < hi; i += NC_THREADS) {
                 const int s = sz[i - lo];
                 if (s > 0 && i != x) {
-                    const double v = __ldcg(at<CONDENSED>(D, row, x, i, n));
+                    const double v = __ldcg(at<L>(D, row, x, i, n, bc));
                     if (v < c.v) { c.v = v; c.i = i; c.s = s; }
                 }
             }
@@ -312,7 +379,8 @@ ward_chain_kernel(double* __restrict__ D, int n, int64_t ldd, int2* __restrict__
             if (lane < cs) m = *cluster.map_shared_rank(&part[par], lane);
             warp_cand_min(m);
             par ^= 1;                                      // part[par] is rewritten only after one more barrier
-            cur = p >= 0 ? __ldcg(at<CONDENSED>(D, row, x, p, n)) : CUDART_INF;   // scipy starts from D[x, prev]: ties go to prev
+            BandCursor pc(B);
+            cur = p >= 0 ? __ldcg(at<L>(D, row, x, p, n, pc)) : CUDART_INF;   // scipy starts from D[x, prev]: ties go to prev
             int y, ys;
             if (m.v < cur) { y = m.i; ys = m.s; cur = m.v; }
             else { y = p; ys = ps; }
@@ -335,14 +403,15 @@ ward_chain_kernel(double* __restrict__ D, int n, int64_t ldd, int2* __restrict__
             merge_xy[2 * static_cast<int64_t>(k) + 1] = b;
             merge_dist[k] = cur;
         }
-        const double* rowa = D + row_off<CONDENSED>(a, n, ldd);
-        double* rowb = D + row_off<CONDENSED>(b, n, ldd);
+        const double* rowa = row_ptr<L>(D, B, a, n, ldd);
+        double* rowb = row_ptr<L>(D, B, b, n, ldd);
+        BandCursor bc(B);
         for (int i = lo + tid; i < hi; i += NC_THREADS) {
             const int ni = sz[i - lo];
             if (ni > 0 && i != a && i != b) {
-                if constexpr (CONDENSED) {                 // one store per (i, b)
-                    double* bi = at<CONDENSED>(D, rowb, b, i, n);
-                    __stcg(bi, ward_update(__ldcg(at<CONDENSED>(D, rowa, a, i, n)), __ldcg(bi), cur, na, nb, ni));
+                if constexpr (L != Layout::SQUARE) {       // one store per (i, b)
+                    double* bi = at<L>(D, rowb, b, i, n, bc);
+                    __stcg(bi, ward_update(__ldcg(at<L>(D, rowa, a, i, n, bc)), __ldcg(bi), cur, na, nb, ni));
                 } else {                                   // row b and the mirrored column
                     const double v = ward_update(__ldcg(rowa + i), __ldcg(rowb + i), cur, na, nb, ni);
                     __stcg(rowb + i, v);
@@ -367,9 +436,9 @@ ward_chain_kernel(double* __restrict__ D, int n, int64_t ldd, int2* __restrict__
     }
 }
 
-template <bool CONDENSED>
+template <Layout L>
 int ward_cluster_size(alq_ctx* ctx, size_t smem, int* out) {
-    auto* kern = ward_chain_kernel<CONDENSED>;
+    auto* kern = ward_chain_kernel<L>;
     ALQ_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
     ALQ_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
     for (int cs : {16, 8}) {
@@ -470,16 +539,16 @@ int pdist_run(alq_ctx* ctx, const char* name, const float* x, int64_t n, int32_t
     return ALQ_OK;
 }
 
-template <bool CONDENSED>
-int nn_chain_run(alq_ctx* ctx, const char* name, double* dist, int64_t n, int64_t ldd, int32_t* merge_xy,
-                 double* merge_dist, void* stream) {
+template <Layout L>
+int nn_chain_run(alq_ctx* ctx, const char* name, double* dist, int64_t n, int64_t ldd, const Bands& bands,
+                 int32_t* merge_xy, double* merge_dist, void* stream) {
     ALQ_CUDA(ctx, cudaSetDevice(ctx->device));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const size_t smem = static_cast<size_t>((n + 7) / 8) * sizeof(int) + 16;   // sized for the 8-CTA fallback
     if (smem + 4096 > ctx->smem_optin)
         ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: n=%lld does not fit the shared memory of a cluster", name, (long long)n);
     int cs = 0;
-    int rc = ward_cluster_size<CONDENSED>(ctx, smem, &cs);
+    int rc = ward_cluster_size<L>(ctx, smem, &cs);
     if (rc) return rc;
     rc = alq_scratch_reserve(ctx, scratch_need({static_cast<size_t>(cs) * n * sizeof(int2), sizeof(int)}));
     if (rc) return rc;
@@ -500,8 +569,8 @@ int nn_chain_run(alq_ctx* ctx, const char* name, double* dist, int64_t n, int64_
     attr.val.clusterDim.z = 1;
     cfg.attrs = &attr;
     cfg.numAttrs = 1;
-    ALQ_CUDA(ctx, cudaLaunchKernelEx(&cfg, ward_chain_kernel<CONDENSED>, dist, static_cast<int>(n), ldd, chain, merge_xy,
-                                     merge_dist, status));
+    ALQ_CUDA(ctx, cudaLaunchKernelEx(&cfg, ward_chain_kernel<L>, dist, static_cast<int>(n), ldd, chain, merge_xy,
+                                     merge_dist, status, bands));
     ALQ_LAUNCH_CHECK(ctx);
     int h_status = 0;
     ALQ_CUDA(ctx, cudaMemcpyAsync(&h_status, status, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -565,7 +634,7 @@ extern "C" int alq_ward_nn_chain(alq_ctx* ctx, double* dist, int64_t n, int64_t 
     if (!ctx) return ALQ_ERR_INVALID;
     if (!dist || !merge_xy || !merge_dist || n < 2 || n >= (1LL << 31) - 1 || ldd < n)
         ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_ward_nn_chain: bad arguments (n=%lld ldd=%lld)", (long long)n, (long long)ldd);
-    return nn_chain_run<false>(ctx, "alq_ward_nn_chain", dist, n, ldd, merge_xy, merge_dist, stream);
+    return nn_chain_run<Layout::SQUARE>(ctx, "alq_ward_nn_chain", dist, n, ldd, Bands{}, merge_xy, merge_dist, stream);
 }
 
 extern "C" int alq_ward_nn_chain_condensed(alq_ctx* ctx, double* dist, int64_t n, int32_t* merge_xy, double* merge_dist,
@@ -573,7 +642,37 @@ extern "C" int alq_ward_nn_chain_condensed(alq_ctx* ctx, double* dist, int64_t n
     if (!ctx) return ALQ_ERR_INVALID;
     if (!dist || !merge_xy || !merge_dist || n < 2 || n >= (1LL << 31) - 1)
         ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_ward_nn_chain_condensed: bad arguments (n=%lld)", (long long)n);
-    return nn_chain_run<true>(ctx, "alq_ward_nn_chain_condensed", dist, n, 0, merge_xy, merge_dist, stream);
+    return nn_chain_run<Layout::CONDENSED>(ctx, "alq_ward_nn_chain_condensed", dist, n, 0, Bands{}, merge_xy, merge_dist,
+                                           stream);
+}
+
+extern "C" int alq_ward_nn_chain_banded(alq_ctx* ctx, const int64_t* row_cuts_host, void* const* bands_host,
+                                        int32_t nbands, int64_t n, int32_t* merge_xy, double* merge_dist, void* stream) {
+    if (!ctx) return ALQ_ERR_INVALID;
+    if (!row_cuts_host || !bands_host || !merge_xy || !merge_dist || nbands < 1 || nbands > ALQ_MAX_WORLD || n < 2 ||
+        n >= (1LL << 31) - 1)
+        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_ward_nn_chain_banded: bad arguments (n=%lld nbands=%d, max %d bands)",
+                 (long long)n, nbands, ALQ_MAX_WORLD);
+    if (row_cuts_host[0] != 0 || row_cuts_host[nbands] != n)
+        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_ward_nn_chain_banded: the cuts must run from 0 to n=%lld (got %lld .. %lld)",
+                 (long long)n, (long long)row_cuts_host[0], (long long)row_cuts_host[nbands]);
+    Bands B{};
+    for (int b = 0; b <= ALQ_MAX_WORLD; ++b) B.cut[b] = static_cast<int>(n);
+    for (int b = 0; b < nbands; ++b) {
+        const int64_t lo = row_cuts_host[b], hi = row_cuts_host[b + 1];
+        if (hi < lo)
+            ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_ward_nn_chain_banded: cut %d (%lld) is below cut %d (%lld)", b + 1,
+                     (long long)hi, b, (long long)lo);
+        const int64_t start = lo * n - lo * (lo + 1) / 2;          // cidx(lo, lo + 1): the band's first entry
+        const int64_t pairs = hi * n - hi * (hi + 1) / 2 - start;
+        if (pairs > 0 && !bands_host[b])
+            ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_ward_nn_chain_banded: band %d (rows [%lld, %lld)) has pairs but no pointer",
+                     b, (long long)lo, (long long)hi);
+        B.cut[b] = static_cast<int>(lo);
+        B.base[b] = reinterpret_cast<double*>(reinterpret_cast<uintptr_t>(bands_host[b]) -
+                                              static_cast<uintptr_t>(start) * sizeof(double));
+    }
+    return nn_chain_run<Layout::BANDED>(ctx, "alq_ward_nn_chain_banded", nullptr, n, 0, B, merge_xy, merge_dist, stream);
 }
 
 extern "C" int alq_ward_labels(const int32_t* merge_xy_host, const double* merge_dist_host, int64_t n, int32_t n_clusters,

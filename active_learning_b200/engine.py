@@ -55,6 +55,35 @@ def ward_labels_host(merge_xy: np.ndarray, merge_dist: np.ndarray, n: int, n_clu
     return out.astype(np.int64)
 
 
+class WardBand:
+    """One band of Ward's condensed distances in device memory another process can map: from Engine.band_alloc (owned:
+    release() frees it) or Engine.band_open (a peer's: release() unmaps it).  `handle` is the 64-byte CUDA IPC handle.
+    Exposes __cuda_array_interface__ as a 1-D float64 array of nbytes // 8 entries, so tensor() is a zero-copy view
+    (for pdist_rows(..., out=)); the view must not outlive release()."""
+
+    def __init__(self, engine, ptr: int, nbytes: int, handle: bytes, owned: bool):
+        self.engine, self.ptr, self.nbytes, self.handle, self.owned = engine, int(ptr), int(nbytes), handle, owned
+
+    @property
+    def __cuda_array_interface__(self):
+        return {"shape": (self.nbytes // 8,), "typestr": "<f8", "data": (self.ptr, False), "version": 3,
+                "strides": None}
+
+    def tensor(self) -> torch.Tensor:
+        return torch.as_tensor(self, device=self.engine.device)
+
+    def release(self):
+        """Frees (owned) or unmaps (opened) the band; idempotent."""
+        if not self.ptr:
+            return
+        ptr, self.ptr = self.ptr, 0
+        e = self.engine
+        if self.owned:
+            e._check(e.lib.alq_band_free(e._h, C.c_void_p(ptr)), "alq_band_free")
+        else:
+            e._check(e.lib.alq_band_close(e._h, C.c_void_p(ptr)), "alq_band_close")
+
+
 class Engine:
     """One libalq context bound to one CUDA device."""
 
@@ -430,6 +459,59 @@ class Engine:
             self._check(self.lib.alq_ward_nn_chain(self._h, _ptr(dist), n, dist.stride(0), _ptr(xy), _ptr(md),
                                                    self._stream()), "alq_ward_nn_chain")
         return xy[:n - 1], md[:n - 1]
+
+    def nn_chain_banded(self, row_cuts: Sequence[int], bands: Sequence, n: int):
+        """K8 over the condensed vector cut into bands of rows (alq_ward_nn_chain_banded): band b holds rows
+        [row_cuts[b], row_cuts[b + 1]) as pdist_rows writes them, at bands[b] -- a WardBand (this process's or one opened
+        from a peer), a contiguous float64 CUDA tensor of at least the band's entries, or None for a band without pairs.
+        Consumed.  The same merge list, bit for bit, as nn_chain over the whole vector; synchronous; AlqError
+        (ALQ_ERR_INVALID) for bad cuts or a missing band, (ALQ_ERR_NUMERIC) if a scan meets no finite distance."""
+        n = int(n)
+        cuts = np.ascontiguousarray([int(c) for c in row_cuts], dtype=np.int64)
+        nb = len(cuts) - 1
+        if len(bands) != nb or nb < 1:
+            raise AlqError(f"nn_chain_banded: {len(cuts)} cuts need {max(nb, 0)} bands, got {len(bands)}")
+        ptrs = (C.c_void_p * nb)()
+        for b, band in enumerate(bands):
+            m = band_pairs(n, cuts[b], cuts[b + 1]) if 0 <= cuts[b] <= cuts[b + 1] <= n else 0
+            if band is None:
+                continue
+            if isinstance(band, WardBand):
+                size, ptr = band.nbytes // 8, band.ptr
+            elif (band.is_cuda and band.dtype == torch.float64 and band.dim() == 1 and band.stride(0) == 1
+                  and band.device == self.device):
+                size, ptr = band.shape[0], band.data_ptr()
+            else:
+                raise AlqError("nn_chain_banded: a band must be a WardBand or a contiguous 1-D float64 tensor on "
+                               f"{self.device}")
+            if size < m:
+                raise AlqError(f"nn_chain_banded: band {b} holds {size} entries, rows [{cuts[b]}, {cuts[b + 1]}) "
+                               f"have {m}")
+            ptrs[b] = ptr
+        xy = torch.empty((max(n - 1, 1), 2), dtype=torch.int32, device=self.device)
+        md = torch.empty(max(n - 1, 1), dtype=torch.float64, device=self.device)
+        self._check(self.lib.alq_ward_nn_chain_banded(self._h, C.c_void_p(cuts.ctypes.data), ptrs, nb, n, _ptr(xy),
+                                                      _ptr(md), self._stream()), "alq_ward_nn_chain_banded")
+        return xy[:max(n - 1, 0)], md[:max(n - 1, 0)]
+
+    def band_alloc(self, nbytes: int) -> "WardBand":
+        """Device memory for one band of Ward's distances that another process of the group can map (alq_band_alloc:
+        a cudaMalloc allocation of its own, outside torch's caching allocator, so call torch.cuda.empty_cache() first if
+        the bytes may sit in torch's cache).  AlqError (ALQ_ERR_NOMEM) if the device cannot hold it."""
+        nbytes = max(8, int(nbytes))
+        p = C.c_void_p()
+        handle = (C.c_char * _lib.IPC_HANDLE_BYTES)()
+        self._check(self.lib.alq_band_alloc(self._h, nbytes, C.byref(p), handle), "alq_band_alloc")
+        return WardBand(self, p.value, nbytes, bytes(handle.raw), owned=True)
+
+    def band_open(self, handle: bytes, nbytes: int) -> "WardBand":
+        """Maps a peer's band (its WardBand.handle) into this process: alq_band_open.  Release it with release()."""
+        handle = bytes(handle)
+        if len(handle) != _lib.IPC_HANDLE_BYTES:
+            raise AlqError(f"band_open: a handle has {_lib.IPC_HANDLE_BYTES} bytes, got {len(handle)}")
+        p = C.c_void_p()
+        self._check(self.lib.alq_band_open(self._h, handle, C.byref(p)), "alq_band_open")
+        return WardBand(self, p.value, int(nbytes), handle, owned=False)
 
     @classmethod
     def ward_bytes(cls, n: int) -> int:

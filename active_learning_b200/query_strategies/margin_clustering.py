@@ -14,7 +14,9 @@ raises AlqError.  The round robin is O(n log n) host NumPy over n margins.
 In a ShardGroup of G > 1 ranks (with an engine that has the band kernel, `pdist_rows`) each rank forwards and scores its
 row_range of the HAC rows, one all_gather_rows replicates the margins (and, in a round that clusters, the embeddings),
 and ShardGroup.ward_labels splits K7 by pair-balanced bands of rows, sends the bands to rank 0 for K8 and broadcasts the
-labels; every rank then runs the same round robin and returns the one-GPU picks.
+labels; every rank then runs the same round robin and returns the one-GPU picks.  When rank 0 cannot hold the distances
+and the engine has the band calls (`band_alloc`, `nn_chain_banded`), each band stays on its rank and rank 0's K8 reads
+the peers' bands through CUDA IPC peer memory, so the row limit becomes the ranks' memory together.
 """
 from __future__ import annotations
 

@@ -6,7 +6,8 @@ independent, so the data path needs no collective; what is exchanged is
                            G*B 12-byte records -> the same stable merge on every rank;
   * partitioned samplers : partition i runs on rank i % G; the picked row lists are gathered once;
   * Ward clustering      : K7 by pair-balanced bands of rows (ward_bands), each band sent to rank 0 in chunks, K8 on
-                           rank 0, the n labels broadcast back (ShardGroup.ward_labels).
+                           rank 0, the n labels broadcast back (ShardGroup.ward_labels); when rank 0 cannot hold the
+                           distances, each band stays on its rank and K8 reads it through CUDA IPC peer memory.
 
 Works with backend "nccl" (GPU) and "gloo" (the CPU tests of this host logic).
 """
@@ -174,6 +175,36 @@ def ward_group_layout(n: int, free_bytes: int, staging_bytes: int) -> str:
     return Engine.ward_layout(n, free_bytes)          # raises: neither fits
 
 
+def ward_band_bytes(n: int, world: int) -> list:
+    """Bytes of each rank's ward_bands(n, world) band of scipy's condensed vector (8 per pair)."""
+    b = ward_bands(n, world)
+    return [8 * band_pairs(n, lo, hi) for lo, hi in zip(b, b[1:])]
+
+
+def ward_group_placement(n: int, free_bytes, staging_bytes: int, distributed: bool = True) -> str:
+    """Where ShardGroup.ward_labels keeps the distances, from every rank's free device memory `free_bytes` (rank order):
+    ward_group_layout's 'square' or 'condensed' on rank 0 whenever rank 0 fits one of them, else 'distributed' -- each
+    rank keeps its own ward_bands band, K8 on rank 0 reads the peers' through peer memory -- when `distributed` (every
+    rank's engine has the band calls) and every rank's free memory holds its band plus Engine.WARD_HEADROOM_BYTES, else an
+    AlqError naming n, both of rank 0's byte counts and the largest band's."""
+    from ._lib import AlqError
+    from .engine import Engine
+    free_bytes = [int(f) for f in free_bytes]
+    try:
+        return ward_group_layout(n, free_bytes[0], staging_bytes)
+    except AlqError:
+        if not distributed:
+            raise
+    need = [b + Engine.WARD_HEADROOM_BYTES for b in ward_band_bytes(n, len(free_bytes))]
+    if all(m <= f for m, f in zip(need, free_bytes)):
+        return "distributed"
+    raise AlqError(f"ward_labels: n={n} rows need {Engine.ward_bytes(n)} bytes of device memory on rank 0 as the n x n "
+                   f"matrix or {Engine.ward_condensed_bytes(n)} as scipy's condensed vector, or, distributed over "
+                   f"{len(free_bytes)} ranks, {max(need)} on the rank with the largest band ({max(need) - Engine.WARD_HEADROOM_BYTES} "
+                   f"bytes of distances), each with {Engine.WARD_HEADROOM_BYTES} headroom; the ranks have {free_bytes} "
+                   f"bytes free; use a smaller subset_unlabeled")
+
+
 class ShardGroup:
     def __init__(self, process_group=None):
         if not dist.is_initialized():
@@ -266,7 +297,7 @@ class ShardGroup:
         return merged
 
     # ---- Ward clustering (MarginClusteringSampler) ---------------------------------------------------
-    def ward_labels(self, x, n_clusters, engine, rows_digest=""):
+    def ward_labels(self, x, n_clusters, engine, rows_digest="", layout=None):
         """sklearn's AgglomerativeClustering(n_clusters) labels of the replicated rows x [n, D], on every rank, with K7
         split over the ranks: rank r computes the pairs of its ward_bands(n, G) band (engine.pdist_rows) in chunks of
         at most WARD_CHUNK_BYTES and sends them to rank 0, which assembles the distances (the n x n matrix through
@@ -281,10 +312,19 @@ class ShardGroup:
         the middle of the transfer (the arguments and buffers are checked before it) leaves the other side waiting on
         its send or receive until the process group's timeout; errors before the transfer and in K8 reach every rank.
 
+        Distributed placement (ward_group_placement: only when rank 0 fits neither layout, or when layout="distributed"
+        forces it): every rank reserves its band in memory another process can map (engine.band_alloc) before the
+        agreement, writes it with one pdist_rows call and synchronises its stream; one all_gather_object exchanges the
+        bands' IPC handles; rank 0 maps the peers' bands, runs K8 over all of them in place (engine.nn_chain_banded)
+        and the labelling, unmaps them and broadcasts the labels.  Nothing is sent between the GPUs but K8's own peer
+        reads and writes.  A peer neither touches nor frees its band until that broadcast has arrived, so the peers wait
+        in the broadcast while K8 runs on rank 0: the process group's timeout bounds K8's time.
+
         `rows_digest` names the pool rows of x (the caller's digest of their positions): the ranks must agree on it.
         ValueError on every rank for fewer than max(2, n_clusters) rows or non-finite rows (sklearn's errors); AlqError on
-        every rank, before any distance is sent, if the ranks disagree on n, d or the rows, if a rank cannot reserve
-        its buffers, or if rank 0's memory fits neither layout; AlqError with rank 0's message if K8 fails there."""
+        every rank, before any distance is sent, if the ranks disagree on n, d, the rows or `layout`, if a rank cannot
+        reserve its buffers (or its band), or if the ranks' memory fits no placement; AlqError with rank 0's message if
+        K8 fails there or if rank 0 cannot map a peer's band."""
         from ._lib import AlqError
         from .engine import Engine
         n, d = int(x.shape[0]), int(x.shape[1])
@@ -292,6 +332,8 @@ class ShardGroup:
             raise ValueError(f"cannot extract {n_clusters} clusters from {n} rows")
         if not bool(torch.isfinite(x).all()):
             raise ValueError("ward: the embeddings contain NaN or infinity")
+        if layout not in (None, "distributed"):
+            raise ValueError(f"ward_labels: layout must be None or 'distributed', got {layout!r}")
         world, rank = self.world_size, self.rank
         bands = ward_bands(n, world)
         plan = [ward_chunks(n, bands[r], bands[r + 1], WARD_CHUNK_BYTES) for r in range(world)]
@@ -301,33 +343,53 @@ class ShardGroup:
 
         # reserve this rank's buffers (rank 0: D too) before the agreement, so that a failure is raised on every rank
         # there rather than leaving the other ranks waiting on a send or a receive
-        free, err, bufs, hold = 0, None, [], []
+        # (every rank probes its own free memory: the distributed placement needs each rank's)
+        free, err, bufs, hold, band = int(engine._ward_free_bytes()), None, [], [], None
+        can_band = hasattr(engine, "nn_chain_banded") and hasattr(engine, "band_alloc")
         layout0 = None
-        if rank == 0:
-            free = int(engine._ward_free_bytes())
+        if rank == 0 and layout is None:
             try:
                 layout0 = ward_group_layout(n, free, staging)
             except AlqError:
-                pass                                   # neither layout fits: the agreement raises it on every rank
+                pass                                   # neither layout fits: the agreement decides on every rank
         try:
-            if rank != 0:
+            if layout == "distributed":
+                band = self._ward_band(x, n, bands, engine)
+            elif rank != 0:
                 engine.pdist_rows(x, bands[rank], bands[rank])      # the engine's argument checks, on an empty band
             elif layout0 == "square":
                 hold.append(torch.empty((n, n), dtype=torch.float64, device=x.device))
             elif layout0 == "condensed":
                 hold.append(torch.empty(n * (n - 1) // 2, dtype=torch.float64, device=x.device))
-            if rank != 0 or layout0 == "square":                    # the staging buffers
+            if layout is None and (rank != 0 or layout0 == "square"):     # the staging buffers
                 bufs = [torch.empty(piece, dtype=torch.float64, device=x.device)
                         for _ in range(2 if rank != 0 else nbufs)]
         except Exception as exc:                       # noqa: BLE001 -- e.g. CUDA out of memory
             err = f"rank {rank}: {type(exc).__name__}: {exc}"
         try:
-            record = {"n, d": (n, d), "rows": str(rows_digest), "n_clusters": int(n_clusters)}
-            locals_ = check_replicated("ward_labels", record, (free, err), self.pg)
-            errs = [e for _, e in locals_ if e]
+            record = {"n, d": (n, d), "rows": str(rows_digest), "n_clusters": int(n_clusters), "layout": layout}
+            locals_ = check_replicated("ward_labels", record, (free, err, can_band), self.pg)
+            errs = [e for _, e, _ in locals_ if e]
             if errs:
                 raise AlqError("ward_labels: a rank could not reserve its K7 buffers: " + "; ".join(errs))
-            layout = ward_group_layout(n, locals_[0][0], staging)     # the same decision (or error) on every rank
+            # the same decision (or error) on every rank
+            placement = layout or ward_group_placement(n, [f for f, _, _ in locals_], staging,
+                                                       all(c for _, _, c in locals_))
+            if placement == "distributed":
+                if layout is None:
+                    # rank 0 fits neither layout: the staging buffers go, each rank reserves its band, and one more
+                    # agreement raises a failed reservation on every rank before any band is computed
+                    bufs.clear()
+                    err = None
+                    try:
+                        band = self._ward_band(x, n, bands, engine)
+                    except Exception as exc:           # noqa: BLE001
+                        err = f"rank {rank}: {type(exc).__name__}: {exc}"
+                    errs = [e for e in check_replicated("ward_labels", {}, err, self.pg) if e]
+                    if errs:
+                        raise AlqError("ward_labels: a rank could not reserve its band: " + "; ".join(errs))
+                return self._ward_distributed(x, n, int(n_clusters), engine, bands, band)
+            layout = placement
 
             if rank != 0:
                 sends = []
@@ -350,11 +412,85 @@ class ShardGroup:
             hold.clear()
             if on_device:
                 torch.cuda.empty_cache()               # rank 0's distances go back to the device (as Engine.ward_tree)
+            if band is not None:
+                band.release()                         # an error before the bands were handed out (else a no-op)
         dist.broadcast_object_list(box, src=self._global_rank(0), group=self.pg)
         msg, labels = box[0]
         if msg is not None:
             raise AlqError(f"ward_labels on rank 0: {msg}")
         return np.asarray(labels).astype(np.int64)
+
+    def _ward_band(self, x, n, bands, engine):
+        """This rank's band of the distributed placement, reserved in memory another process can map (None when the
+        band holds no pair).  The engine's argument checks run first, on an empty band."""
+        from ._lib import AlqError
+        if not (hasattr(engine, "nn_chain_banded") and hasattr(engine, "band_alloc")):
+            raise AlqError("the engine has no band calls (band_alloc, nn_chain_banded) for the distributed placement")
+        lo, hi = bands[self.rank], bands[self.rank + 1]
+        engine.pdist_rows(x, lo, lo)
+        m = band_pairs(n, lo, hi)
+        if not m:
+            return None
+        if x.is_cuda:
+            torch.cuda.empty_cache()                   # the band is the library's cudaMalloc: torch's cache is no use to it
+        return engine.band_alloc(8 * m)
+
+    def _ward_distributed(self, x, n, n_clusters, engine, bands, band):
+        """The distributed placement of ward_labels, after the agreement: this rank's band from one pdist_rows call,
+        the stream synchronised, the handles exchanged, K8 on rank 0 over every band, the labels broadcast.  The band is
+        released only after the broadcast (rank 0 has unmapped the peers' bands by then)."""
+        from ._lib import AlqError
+        rank = self.rank
+        box = [None]
+        try:
+            err = None
+            try:
+                if band is not None:
+                    engine.pdist_rows(x, bands[rank], bands[rank + 1], out=band.tensor())
+                    if x.is_cuda:
+                        torch.cuda.current_stream(x.device).synchronize()   # K7 is complete before the handle leaves
+            except Exception as exc:                   # noqa: BLE001 -- reported by rank 0 on every rank
+                err = f"rank {rank}: {type(exc).__name__}: {exc}"
+            mine = (err, None if band is None else band.handle, 0 if band is None else band.nbytes)
+            shared = [None] * self.world_size
+            dist.all_gather_object(shared, mine, group=self.pg)
+            if rank == 0:
+                box = [self._ward_rank0_banded(n, n_clusters, engine, bands, band, shared)]
+            dist.broadcast_object_list(box, src=self._global_rank(0), group=self.pg)
+        finally:
+            if band is not None:
+                band.release()
+        msg, labels = box[0]
+        if msg is not None:
+            raise AlqError(f"ward_labels on rank 0: {msg}")
+        return np.asarray(labels).astype(np.int64)
+
+    def _ward_rank0_banded(self, n, n_clusters, engine, bands, band, shared):
+        """Rank 0's half of the distributed placement: the peers' bands mapped, K8 over every band, the labels, the
+        mappings closed.  Returns (error message or None, labels as int32)."""
+        from .engine import ward_labels_host
+        errs = [e for e, _, _ in shared if e]
+        if errs:
+            return "K7 failed: " + "; ".join(errs), None
+        opened = []
+        try:
+            parts = [band]
+            for handle, nbytes in ((h, b) for _, h, b in shared[1:]):
+                parts.append(None if handle is None else engine.band_open(handle, nbytes))
+                if handle is not None:
+                    opened.append(parts[-1])
+            xy, md = engine.nn_chain_banded(bands, parts, n)          # synchronous: the bands are idle when it returns
+            xy = xy.cpu().numpy() if isinstance(xy, torch.Tensor) else np.asarray(xy)
+            md = md.cpu().numpy() if isinstance(md, torch.Tensor) else np.asarray(md)
+            return None, ward_labels_host(xy, md, n, n_clusters).astype(np.int32)
+        except Exception as exc:                       # noqa: BLE001 -- every rank raises rank 0's message
+            return f"{type(exc).__name__}: {exc}", None
+        finally:
+            for b in opened:
+                try:
+                    b.release()
+                except Exception:                      # noqa: BLE001 -- an unmap error must not keep the peers waiting
+                    pass
 
     def _global_rank(self, r):
         return r if self.pg is None else dist.get_global_rank(self.pg, r)

@@ -333,6 +333,21 @@ int alq_base_select(alq_ctx* ctx, const float* min_margin, const float* radius, 
  * alq_ward_nn_chain_condensed (K8, condensed layout): the same walk and the same merge list, bit for bit, over a
  *   condensed vector of n (n - 1) / 2 entries (as alq_pdist_f64_condensed writes it), consumed in place.  Same
  *   arguments and contract as alq_ward_nn_chain, without ldd.
+ * alq_ward_nn_chain_banded (K8, banded layout): the same walk and the same merge list, bit for bit, over the condensed
+ *   vector cut into 1 <= nbands <= 8 bands of rows, each at its own device pointer (which may be a peer GPU's memory
+ *   mapped with alq_band_open): band b holds rows [row_cuts_host[b], row_cuts_host[b + 1]) as
+ *   alq_pdist_f64_condensed_rows writes them, at bands_host[b].  The nbands + 1 cuts run from 0 to n and never
+ *   decrease (empty bands are allowed); a band without pairs (row n - 1 alone, or empty) may have a null pointer.
+ *   Consumed in place.  Every band must stay untouched by any other stream, process or GPU until this call returns.
+ *   ALQ_ERR_INVALID for cuts that decrease or do not cover [0, n), a null pointer for a band with pairs, nbands
+ *   outside [1, 8], and as alq_ward_nn_chain_condensed.  This is how a group runs K8 over the ranks' bands without
+ *   gathering them (sharding.py: ShardGroup.ward_labels, the distributed placement).
+ * alq_band_alloc / alq_band_open / alq_band_close / alq_band_free: device memory for one band that another process can
+ *   map.  alloc: a cudaMalloc allocation of `bytes` (> 0) of its own -- an IPC handle names the base of an allocation,
+ *   so a block of a caching allocator cannot be exported -- and its ALQ_IPC_HANDLE_BYTES handle (ALQ_ERR_NOMEM if the
+ *   device cannot hold it).  open: maps a handle from another process (cudaIpcOpenMemHandle; ALQ_ERR_CUDA without
+ *   peer access).  close: unmaps what open returned.  free: releases what alloc returned; the owner frees only after
+ *   every process that opened the band has closed it.
  * alq_ward_labels: host-only, needs no GPU.  From K8's merge list: the stable sort by distance and scipy's union-find
  *   relabelling (hierarchy.ward's Z), then sklearn's _hc_cut(n_clusters): labels_host[0..n) in [0, n_clusters),
  *   numbered in the order of the cut's final heap.  ALQ_ERR_INVALID if n_clusters > n, or if the list is not a merge
@@ -351,6 +366,12 @@ int alq_pdist_f64_expand(alq_ctx* ctx, const double* rows, int64_t n, int64_t ro
                          int64_t ldd, void* stream);
 int alq_ward_labels(const int32_t* merge_xy_host, const double* merge_dist_host, int64_t n, int32_t n_clusters,
                     int32_t* labels_host);
+int alq_ward_nn_chain_banded(alq_ctx* ctx, const int64_t* row_cuts_host, void* const* bands_host, int32_t nbands,
+                             int64_t n, int32_t* merge_xy, double* merge_dist, void* stream);
+int alq_band_alloc(alq_ctx* ctx, size_t bytes, void** ptr_out, void* handle_out);
+int alq_band_open(alq_ctx* ctx, const void* handle, void** ptr_out);
+int alq_band_close(alq_ctx* ctx, void* ptr);
+int alq_band_free(alq_ctx* ctx, void* ptr);
 
 /* ---- K9: the VAAL discriminator (VAALSampler) ---------------------------------------------------------------------
  * vaal_sampler.py:57-58 scores every pool row by the discriminator of vaal_discriminator.py on the VAE's mu:
