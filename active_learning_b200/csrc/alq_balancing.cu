@@ -23,9 +23,9 @@
 // warp, nor the CTA, nor the grid size changes it, so the picks are bit-reproducible.
 // Sharded over a group (shard_off_host), the segments above are every rank's CTA segments (BalShard): every CTA of every
 // rank keeps all of their counts, the key words go into every rank's window and the owner of a random pick stores its
-// word there too; K12 shares the layout and the host steps below.
-#include <limits.h>
-
+// word there too; K12 shares the layout.
+// The host side of a call is bal_select (alq_balancing.cuh), shared with K12; this file supplies K11's part of it
+// (BalLoop: the shared-memory limit, the class-sum scratch and launches) and the segment count of both.
 #include "alq_balancing.cuh"
 
 namespace {
@@ -315,240 +315,61 @@ __global__ void __launch_bounds__(kBalThreads, 1) balancing_loop_kernel(const __
     }
 }
 
-constexpr size_t kWordsHead = 128;               // u64 ready[ALQ_MAX_WORLD] in front of a window's words (greedy's layout)
+// K11's steps of bal_select
+struct BalLoop {
+    using Args = BalArgs;
+    static constexpr const char* kName = "alq_balancing_select";
+    static constexpr int kForce = 2;                 // balancing_loop = 2 forces K11; 1 and 3 make it decline
+    static constexpr int kThreads = kBalThreads;
+    static constexpr auto kernel = balancing_loop_kernel;
+    size_t smem = 0, sum_smem = 0;
 
-size_t up128(size_t v) { return (v + 127) & ~size_t(127); }
+    int plan_smem(alq_ctx* ctx, BalCall& B) {
+        smem = bal_loop_smem(B.c, B.d, B.nseg);
+        sum_smem = static_cast<size_t>(B.c) * kSumDims * sizeof(double);
+        if (smem > B.smem_cap || sum_smem > B.smem_cap)
+            BAL_LIMIT(B, "%s: the %d centres of %d floats need %zu bytes of shared memory, %zu are available (limit: centres "
+                      "in shared memory)", kName, B.c, B.d, std::max(smem, sum_smem), B.smem_cap);
+        return ALQ_OK;
+    }
+    static int nchunks(const BalCall& B) { return (B.n + kSumChunk - 1) / kSumChunk; }
+    // all of K11's scratch, reserved with the counts' (the first four) and sized from the shape
+    size_t need_with_counts(const BalCall& B) const {
+        const size_t cd = static_cast<size_t>(B.c) * B.d;
+        return scratch_need({B.entries * 4, static_cast<size_t>(B.c) * 4, 8, static_cast<size_t>(B.nseg) * 4,
+                             static_cast<size_t>(nchunks(B)) * cd * 8, cd * 8, static_cast<size_t>(B.S.grid) * cd * 8,
+                             static_cast<size_t>(B.n), (kMtN + 1) * 4 * 2, B.sharded ? 0 : B.words_max, 16});
+    }
+    // the fp64 class sums
+    int setup(alq_ctx* ctx, BalCall& B, ScratchCursor& cur, BalArgs& A) {
+        const alq_balancing_desc* D = B.D;
+        const int n = B.n, c = B.c, d = B.d, nch = nchunks(B);
+        const size_t cd = static_cast<size_t>(c) * d;
+        double* partial = cur.take<double>(static_cast<size_t>(nch) * cd);
+        double* sums0 = cur.take<double>(cd);
+        A.sums = cur.take<double>(static_cast<size_t>(B.S.grid) * cd);
+        A.sums0 = sums0;
+        A.xn = D->xn;
+        if (sum_smem > 48u * 1024u)
+            ALQ_CUDA(ctx, cudaFuncSetAttribute(bal_class_sum_partial_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(sum_smem)));
+        bal_class_sum_partial_kernel<<<dim3((d + kSumDims - 1) / kSumDims, nch), kSumDims, sum_smem, B.st>>>(
+            D->x, D->ldx, d, D->labels, D->labeled, n, c, partial);
+        ALQ_LAUNCH_CHECK(ctx);
+        bal_class_sum_reduce_kernel<<<static_cast<int>((cd + 255) / 256), 256, 0, B.st>>>(partial, nch, static_cast<long long>(cd), sums0);
+        ALQ_LAUNCH_CHECK(ctx);
+        return ALQ_OK;
+    }
+};
 
 }  // namespace
 
-// descriptors of the shorter, single-GPU layout end here
-constexpr size_t kBalDescV1 = offsetof(alq_balancing_desc, shard_off_host);
-
-int alq_bal_shard(alq_ctx* ctx, const alq_balancing_desc* D, int n, BalShard* S, bool* sharded, const char* fn) {
-    const int32_t* so = D->struct_size >= sizeof(alq_balancing_desc) ? D->shard_off_host : nullptr;
-    *sharded = so != nullptr;
-    S->world = 1;
-    S->rank = 0;
-    S->off[0] = 0;
-    S->off[1] = n;
-    if (so) {
-        const AlqComm& G = ctx->comm;
-        if (!G.window || !G.connected)
-            ALQ_FAIL(ctx, ALQ_ERR_STATE, "%s: a sharded call (shard_off_host) needs the group of alq_comm_create/connect", fn);
-        if (so[0] != 0 || so[G.world] != n)
-            ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: shard_off must run from 0 to n=%d, got %d .. %d", fn, n, so[0], so[G.world]);
-        for (int r = 0; r < G.world; ++r)
-            if (so[r + 1] < so[r]) ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: shard_off[%d] = %d < shard_off[%d] = %d", fn, r + 1, so[r + 1], r, so[r]);
-        S->world = G.world;
-        S->rank = G.rank;
-        std::copy(so, so + G.world + 1, S->off);
-    }
-    int rows_min = n;
-    for (int r = 0; r < S->world; ++r) rows_min = std::min(rows_min, S->off[r + 1] - S->off[r]);
-    S->grid = std::max(1, std::min(ctx->sm_count, (rows_min + 127) / 128));
-    return ALQ_OK;
-}
-
-int alq_bal_seg_rows_max(const BalShard& S) {
-    int m = 0;
-    for (int g = 0; g < S.world * S.grid; ++g) m = std::max(m, gseg_lo(S, g + 1) - gseg_lo(S, g));
-    return m;
-}
-
-size_t alq_bal_words_bytes(const BalShard& S, int64_t budget, bool sharded) {
-    const size_t keyw = sharded ? kWordsHead : 0;
-    return up128(keyw + static_cast<size_t>(2) * S.world * S.grid * 8) + static_cast<size_t>(budget) * 8;
-}
-
-int alq_bal_words_begin(alq_ctx* ctx, const BalShard& S, bool sharded, int budget, char* scratch, BalWords* W, cudaStream_t st) {
-    *W = BalWords{};
-    W->keyw = static_cast<unsigned int>(sharded ? kWordsHead : 0);
-    W->pickw = static_cast<unsigned int>(up128(W->keyw + static_cast<size_t>(2) * S.world * S.grid * 8));
-    const size_t end = alq_bal_words_bytes(S, budget, sharded);
-    W->tag_base = 0x80000000u;
-    if (!sharded) {
-        W->peer[0] = scratch;
-        ALQ_CUDA(ctx, cudaMemsetAsync(scratch, 0, end, st));
-        return ALQ_OK;
-    }
-    // the words start without a valid tag; peers write them only after our ready word, which follows the clear
-    ALQ_CUDA(ctx, cudaMemsetAsync(ctx->comm.window + kWordsHead, 0, end - kWordsHead, st));
-    for (int r = 0; r < S.world; ++r) W->peer[r] = ctx->comm.peer[r];
-    ctx->comm.epoch += 1;
-    W->ready_tag = ctx->comm.epoch << 32;
-    W->tag_base |= static_cast<unsigned int>(ctx->comm.epoch & 0x7fu) << 24;
-    return alq_comm_ready(ctx, W->ready_tag, st);
-}
-
-int alq_bal_check_desc(alq_ctx* ctx, const alq_balancing_desc* D, const char* fn) {
-    if (!D || D->struct_size < kBalDescV1) ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: bad descriptor", fn);
-    const int64_t n64 = D->n;
-    const int c = D->c, d = D->d;
-    if (n64 < 0 || n64 >= (1LL << 31)) ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: n=%lld outside [0, 2^31)", fn, (long long)n64);
-    if (c < 1 || c > ALQ_CLASS_MAX) ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: C=%d outside [1, %d]", fn, c, ALQ_CLASS_MAX);
-    if (d <= 0 || D->ldx < d || D->budget < 0)
-        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: bad shape d=%d ldx=%lld budget=%lld", fn, d, (long long)D->ldx, (long long)D->budget);
-    if (!D->mt_key_host || !D->mt_pos_host || !D->n_picks_host || !D->n_balancing_host ||
-        (n64 > 0 && (!D->x || !D->xn || !D->labels || !D->avail || !D->labeled)) || (D->budget > 0 && !D->picks))
-        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: null pointer", fn);
-    if ((d % 4) || (D->ldx % 4) || (n64 > 0 && !aligned16(D->x)))
-        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: d and ldx must be multiples of 4 and x 16-byte aligned", fn);
-    if (*D->mt_pos_host < 0 || *D->mt_pos_host > kMtN)
-        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: MT19937 position %d outside [0, %d]", fn, *D->mt_pos_host, kMtN);
-    *D->n_picks_host = -1;
-    *D->n_balancing_host = 0;
-    return ALQ_OK;
-}
-
-int alq_bal_counts(alq_ctx* ctx, const alq_balancing_desc* D, int n, int c, const BalShard& S, int32_t* tab, unsigned int* bad,
-                   int32_t* counts, int32_t* seg_avail, int32_t* counts_h, int32_t* seg_h, cudaStream_t st, const char* fn) {
-    const int nseg = S.world * S.grid;
-    ALQ_CUDA(ctx, cudaMemsetAsync(bad, 0xff, 2 * sizeof(unsigned int), st));
-    const int rc = alq_class_table_pass(ctx, D->labels, D->labeled, n, c, tab, bad, counts, st);
-    if (rc != ALQ_OK) return rc;
-    bal_seg_count_kernel<<<nseg, 256, 0, st>>>(D->labels, D->avail, c, S, seg_avail, bad + 1);
+int bal_seg_count(alq_ctx* ctx, const int32_t* labels, const uint8_t* avail, int c, const BalShard& S, int32_t* seg_avail,
+                  unsigned int* bad, cudaStream_t st) {
+    bal_seg_count_kernel<<<S.world * S.grid, 256, 0, st>>>(labels, avail, c, S, seg_avail, bad);
     ALQ_LAUNCH_CHECK(ctx);
-    unsigned int bad_h[2] = {UINT_MAX, UINT_MAX};
-    ALQ_CUDA(ctx, cudaMemcpyAsync(bad_h, bad, sizeof(bad_h), cudaMemcpyDeviceToHost, st));
-    ALQ_CUDA(ctx, cudaMemcpyAsync(counts_h, counts, static_cast<size_t>(c) * 4, cudaMemcpyDeviceToHost, st));
-    ALQ_CUDA(ctx, cudaMemcpyAsync(seg_h, seg_avail, static_cast<size_t>(nseg) * 4, cudaMemcpyDeviceToHost, st));
-    ALQ_CUDA(ctx, cudaStreamSynchronize(st));
-    for (int k = 1; k >= 0; --k)
-        if (bad_h[k] != UINT_MAX) {
-            int32_t y = 0;
-            ALQ_CUDA(ctx, cudaMemcpy(&y, D->labels + bad_h[k], sizeof(int32_t), cudaMemcpyDeviceToHost));
-            ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: %s row %u has label %d, outside [0, %d)", fn,
-                     k ? "available" : "labeled", bad_h[k], y, c);
-        }
     return ALQ_OK;
 }
 
 extern "C" int alq_balancing_select(alq_ctx* ctx, const alq_balancing_desc* D, void* stream) {
-    if (!ctx) return ALQ_ERR_INVALID;
-    int rc = alq_bal_check_desc(ctx, D, "alq_balancing_select");
-    if (rc != ALQ_OK) return rc;
-    const int64_t n64 = D->n;
-    const int c = D->c, d = D->d;
-    if (ctx->balancing_loop == 1 || ctx->balancing_loop == 3) return ALQ_OK;   // the per-step path or K12 runs
-    const int n = static_cast<int>(n64);
-    const bool forced = ctx->balancing_loop == 2;
-    if (n == 0 || D->budget == 0) {
-        *D->n_picks_host = 0;
-        return ALQ_OK;
-    }
-    const cudaStream_t st = static_cast<cudaStream_t>(stream);
-
-    // ---- limits that the shape decides (the same on every rank of a sharded call) -------------------------------------
-    BalShard S;
-    bool sharded = false;
-    rc = alq_bal_shard(ctx, D, n, &S, &sharded, "alq_balancing_select");
-    if (rc != ALQ_OK) return rc;
-    const int grid = S.grid, nseg = S.world * grid;
-    const size_t smem = bal_loop_smem(c, d, nseg);
-    const size_t sum_smem = static_cast<size_t>(c) * kSumDims * sizeof(double);
-    const size_t smem_cap = ctx->smem_optin > 4096 ? ctx->smem_optin - 1024 : 0;   // the kernels' static shared memory
-    if (smem > smem_cap || sum_smem > smem_cap) {
-        if (!forced) return ALQ_OK;
-        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_balancing_select: the %d centres of %d floats need %zu bytes of shared memory, "
-                 "%zu are available (limit: centres in shared memory)", c, d, std::max(smem, sum_smem), smem_cap);
-    }
-    if (alq_bal_seg_rows_max(S) > kSegRowsMax) {
-        if (!forced) return ALQ_OK;
-        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_balancing_select: n=%d rows over %d CTAs exceed %d rows per CTA segment "
-                 "(limit: rows per segment)", n, nseg, kSegRowsMax);
-    }
-    const int64_t budget_req = D->budget;
-    const size_t words = alq_bal_words_bytes(S, std::min<int64_t>(budget_req, n), sharded);
-    if (sharded && words > ctx->comm.greedy_bytes()) {
-        if (!forced) return ALQ_OK;
-        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_balancing_select: a budget of %lld needs %zu bytes of the peer window, %zu are "
-                 "usable (limit: words in the peer window)", (long long)budget_req, words, ctx->comm.greedy_bytes());
-    }
-
-    // ---- set-up: counts, segment counts, label checks -----------------------------------------------------------
-    const int nchunks = (n + kSumChunk - 1) / kSumChunk;
-    const size_t cd = static_cast<size_t>(c) * d;
-    const size_t entries = alq_class_table_entries(n, c);
-    const size_t need = scratch_need({entries * 4, static_cast<size_t>(c) * 4, 8, static_cast<size_t>(nseg) * 4,
-                                      static_cast<size_t>(nchunks) * cd * 8, cd * 8, static_cast<size_t>(grid) * cd * 8,
-                                      static_cast<size_t>(n), (kMtN + 1) * 4 * 2, sharded ? 0 : words, 16});
-    rc = alq_scratch_reserve(ctx, need);
-    if (rc != ALQ_OK) return rc;
-    ScratchCursor cur(ctx->scratch);
-    int32_t* tab = cur.take<int32_t>(entries);
-    int32_t* counts = cur.take<int32_t>(c);
-    unsigned int* bad = cur.take<unsigned int>(2);
-    int32_t* seg_avail = cur.take<int32_t>(nseg);
-    double* partial = cur.take<double>(static_cast<size_t>(nchunks) * cd);
-    double* sums0 = cur.take<double>(cd);
-    double* sums = cur.take<double>(static_cast<size_t>(grid) * cd);
-    uint8_t* avail = cur.take<uint8_t>(n);
-    unsigned int* mt = cur.take<unsigned int>(2 * (kMtN + 1));
-    char* word_scratch = cur.take<char>(sharded ? 0 : words);
-    int* small = cur.take<int>(4);                                     // [0] status, [1] balancing steps
-
-    std::vector<int32_t> counts_h(c), seg_h(nseg);
-    rc = alq_bal_counts(ctx, D, n, c, S, tab, bad, counts, seg_avail, counts_h.data(), seg_h.data(), st, "alq_balancing_select");
-    if (rc != ALQ_OK) return rc;
-    int64_t n_avail = 0, labeled_total = 0;
-    for (int g = 0; g < nseg; ++g) n_avail += seg_h[g];
-    for (int k = 0; k < c; ++k) labeled_total += counts_h[k];
-    const int budget = static_cast<int>(std::min<int64_t>(budget_req, n_avail));
-    if (labeled_total + budget >= (1LL << 24)) {
-        if (!forced) return ALQ_OK;
-        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_balancing_select: %lld labeled rows plus a budget of %d reach 2^24 "
-                 "(limit: counts plus budget below 2^24)", (long long)labeled_total, budget);
-    }
-    if (budget == 0) {
-        *D->n_picks_host = 0;
-        return ALQ_OK;
-    }
-
-    // ---- fp64 class sums, the working mask, the RNG state -------------------------------------------------------
-    if (sum_smem > 48u * 1024u)
-        ALQ_CUDA(ctx, cudaFuncSetAttribute(bal_class_sum_partial_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(sum_smem)));
-    bal_class_sum_partial_kernel<<<dim3((d + kSumDims - 1) / kSumDims, nchunks), kSumDims, sum_smem, st>>>(
-        D->x, D->ldx, d, D->labels, D->labeled, n, c, partial);
-    ALQ_LAUNCH_CHECK(ctx);
-    bal_class_sum_reduce_kernel<<<static_cast<int>((cd + 255) / 256), 256, 0, st>>>(partial, nchunks, static_cast<long long>(cd), sums0);
-    ALQ_LAUNCH_CHECK(ctx);
-    std::vector<unsigned int> mt_h(kMtN + 1);
-    std::copy(D->mt_key_host, D->mt_key_host + kMtN, mt_h.begin());
-    mt_h[kMtN] = static_cast<unsigned int>(*D->mt_pos_host);
-    ALQ_CUDA(ctx, cudaMemcpyAsync(mt, mt_h.data(), (kMtN + 1) * 4, cudaMemcpyHostToDevice, st));
-    ALQ_CUDA(ctx, cudaMemcpyAsync(avail, D->avail, static_cast<size_t>(n), cudaMemcpyDeviceToDevice, st));
-    ALQ_CUDA(ctx, cudaMemsetAsync(small, 0, 4 * sizeof(int), st));
-
-    // ---- the loop ---------------------------------------------------------------------------------------------------
-    BalArgs A{};
-    rc = alq_bal_words_begin(ctx, S, sharded, budget, word_scratch, &A.W, st);
-    if (rc != ALQ_OK) return rc;
-    A.x = D->x; A.ldx = D->ldx; A.d = d;
-    A.xn = D->xn; A.labels = D->labels; A.avail = avail;
-    A.sums0 = sums0; A.sums = sums; A.counts0 = counts; A.seg_avail0 = seg_avail;
-    A.mt_in = mt; A.mt_out = mt + kMtN + 1;
-    A.picks = D->picks; A.n_bal = small + 1; A.status = small;
-    A.S = S;
-    A.n = n; A.c = c; A.budget = budget; A.n_avail = static_cast<int>(n_avail);
-    A.timeout_cycles = static_cast<long long>(ctx->spin_timeout_ms) * ctx->clock_khz;
-    ALQ_CUDA(ctx, cudaFuncSetAttribute(balancing_loop_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-    // every CTA spins on the others' words, so all of them must be resident: grid <= SMs, one CTA per SM at most
-    // (see alq_score.cu on why this is an ordinary launch and what alq_gridsync_begin/end guard against)
-    alq_gridsync_begin(ctx, st);
-    balancing_loop_kernel<<<grid, kBalThreads, smem, st>>>(A);
-    const cudaError_t le = cudaGetLastError();
-    alq_gridsync_end(ctx, st);
-    ctx->launches++;
-    if (le != cudaSuccess) ALQ_FAIL(ctx, ALQ_ERR_CUDA, "alq_balancing_select: launch failed: %s (grid %d, %zu B shared)", cudaGetErrorString(le), grid, smem);
-
-    int small_h[2] = {0, 0};
-    ALQ_CUDA(ctx, cudaMemcpyAsync(small_h, small, sizeof(small_h), cudaMemcpyDeviceToHost, st));
-    ALQ_CUDA(ctx, cudaMemcpyAsync(mt_h.data(), A.mt_out, (kMtN + 1) * 4, cudaMemcpyDeviceToHost, st));
-    ALQ_CUDA(ctx, cudaStreamSynchronize(st));
-    if (small_h[0] != 0) ALQ_FAIL(ctx, small_h[0], "alq_balancing_select: timed out waiting for a peer GPU or a CTA of the grid");
-    std::copy(mt_h.begin(), mt_h.begin() + kMtN, D->mt_key_host);
-    *D->mt_pos_host = static_cast<int32_t>(mt_h[kMtN]);
-    *D->n_picks_host = budget;
-    *D->n_balancing_host = small_h[1];
-    return ALQ_OK;
+    return bal_select<BalLoop>(ctx, D, stream);
 }

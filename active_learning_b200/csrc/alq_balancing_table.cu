@@ -7,7 +7,7 @@
 //     d2(i, c) = xn64_i - 2 T[i, c] / den_c + q_c / den_c^2,   den_c = fl32(n_c + 1e-5),  q_c = <S_c, S_c>  (fp64),
 // i.e. |x_i - m_c|^2 for the unrounded centre m_c = S_c / den_c.  Everything else is K11's: the branch test, the
 // numerator 1, NumPy's draws, the tie rule and the LL-word agreement.
-//   set-up   K10's table pass and the segment count (alq_bal_counts, with the label checks); one launch groups the
+//   set-up   K10's table pass and the segment count (with the label checks, as for K11); one launch groups the
 //            labeled rows by class in row order; one launch per class sums them in that order (fp64) and forms q_c;
 //   loop     ONE ordinary launch, one CTA per SM (bracketed by alq_gridsync_begin/end, every wait bounded by
 //            "spin_timeout_ms").  Every CTA keeps the counts, den, q, the majority list, the per-segment available
@@ -25,8 +25,8 @@
 // sum of exact fp32 x fp32 products, lane l taking the float4 chunks l, l + 32, .. in x, y, z, w order, folded by a
 // butterfly; S_c sums the class's rows in row order; q_c is a per-thread fma chain (dimensions tid, tid + 512, ..)
 // folded by a butterfly and the 16 warp partials in order.  So the picks are bit-reproducible.
-#include <limits.h>
-
+// The host side of a call is bal_select (alq_balancing.cuh), shared with K11; this file supplies K12's part of it
+// (TabLoop: the pending list's shared-memory plan, the device-memory limit, the table's scratch and set-up launches).
 #include "alq_balancing.cuh"
 
 namespace {
@@ -463,196 +463,111 @@ __global__ void __launch_bounds__(kTabThreads, 1) balancing_table_kernel(const _
     }
 }
 
+// K12's steps of bal_select
+struct TabLoop {
+    using Args = TabArgs;
+    static constexpr const char* kName = "alq_balancing_table_select";
+    static constexpr int kForce = 3;                 // balancing_loop = 3 forces K12; 1 and 2 make it decline
+    static constexpr int kThreads = kTabThreads;
+    static constexpr auto kernel = balancing_table_kernel;
+    size_t smem = 0, group_smem = 0;
+    int pend_cap = 0;
+
+    int plan_smem(alq_ctx* ctx, BalCall& B) {
+        const int c = B.c, d = B.d, nseg = B.nseg;
+        const size_t smem_cap = B.smem_cap;
+        const size_t fixed = bal_table_smem(c, d, nseg, 0) - kBuildBytes;
+        pend_cap = fixed < smem_cap ? static_cast<int>(std::min<size_t>(kPendMax, (smem_cap - fixed) / (static_cast<size_t>(d) * 4 + 4))) : 0;
+        while (pend_cap > 0 && bal_table_smem(c, d, nseg, pend_cap) > smem_cap) --pend_cap;
+        group_smem = static_cast<size_t>(c) * 4;
+        if (pend_cap < 1 || group_smem > smem_cap)
+            BAL_LIMIT(B, "%s: the tables of %d classes and one pending row of %d floats need %zu bytes of shared memory, %zu "
+                      "are available (limit: class tables in shared memory)", kName, c, d, bal_table_smem(c, d, nseg, 1), smem_cap);
+        smem = bal_table_smem(c, d, nseg, pend_cap);
+        return ALQ_OK;
+    }
+    // the table's rows are the available rows: sized after the counts
+    size_t need_with_counts(const BalCall&) const { return 0; }
+    // the table and the per-CTA sums must fit the device's free memory: checked before anything is reserved for them;
+    // then the table slots, the fp64 class sums in row order per class and their squared norms
+    int setup(alq_ctx* ctx, BalCall& B, ScratchCursor& cur, TabArgs& A) {
+        const alq_balancing_desc* D = B.D;
+        const BalShard& S = B.S;
+        const cudaStream_t st = B.st;
+        const int n = B.n, c = B.c, d = B.d, grid = S.grid, nseg = B.nseg;
+        std::vector<int64_t> avail_of(S.world, 0);                    // available rows per rank: its table rows
+        for (int g = 0; g < nseg; ++g) avail_of[g / grid] += B.seg_h[g];
+        const size_t cd = static_cast<size_t>(c) * d;
+        const size_t words_b = bal_words_bytes(S, B.budget, B.sharded);
+        auto need_for = [&](size_t na) {
+            return scratch_need({static_cast<size_t>(c) * 4, static_cast<size_t>(nseg) * 4, static_cast<size_t>(c + 1) * 4,
+                                 static_cast<size_t>(grid) * 4, static_cast<size_t>(std::max<int64_t>(B.labeled_total, 1)) * 4,
+                                 cd * 8, static_cast<size_t>(c) * 8, static_cast<size_t>(grid) * cd * 8, na * c * 8,
+                                 na * 8, na * 4, static_cast<size_t>(n), (kMtN + 1) * 4 * 2, B.sharded ? 0 : words_b, 16});
+        };
+        const size_t na = static_cast<size_t>(avail_of[S.rank]);
+        const size_t need = need_for(na);
+        if (B.sharded) {
+            // the same decision on every rank: every rank's share against the group's least free memory (the caller's
+            // gather; this context's scratch is not counted, so the check is conservative)
+            for (int r = 0; r < S.world; ++r) {
+                const size_t nr = need_for(static_cast<size_t>(avail_of[r]));
+                const size_t want = nr + (nr >> 2) + (1u << 20);            // what alq_scratch_reserve allocates
+                if (D->group_free_bytes < 0 || want > static_cast<size_t>(D->group_free_bytes))
+                    BAL_LIMIT(B, "%s: rank %d's %lld x %d table (%zu bytes) and %d copies of the class sums (%zu bytes) need "
+                              "%zu bytes of device memory, the group has %lld free (limit: table in device memory)", kName, r,
+                              (long long)avail_of[r], c, static_cast<size_t>(avail_of[r]) * c * 8, grid,
+                              static_cast<size_t>(grid) * cd * 8, want, (long long)D->group_free_bytes);
+            }
+        } else if (need > ctx->scratch_bytes) {
+            size_t free_b = 0, total_b = 0;
+            ALQ_CUDA(ctx, cudaMemGetInfo(&free_b, &total_b));
+            const size_t want = need + (need >> 2) + (1u << 20);           // what alq_scratch_reserve allocates
+            if (want > free_b + ctx->scratch_bytes)
+                BAL_LIMIT(B, "%s: the %lld x %d table (%zu bytes) and %d copies of the class sums (%zu bytes) need %zu bytes "
+                          "of device memory, %zu are free (limit: table in device memory)", kName, (long long)B.n_avail, c,
+                          na * c * 8, grid, static_cast<size_t>(grid) * cd * 8, want, free_b + ctx->scratch_bytes);
+        }
+        const int rc = alq_scratch_reserve(ctx, need);
+        if (rc != ALQ_OK) return rc;
+        cur = ScratchCursor(ctx->scratch);                            // the counts move to the front of the new scratch
+        B.counts = cur.take<int32_t>(c);
+        B.seg_avail = cur.take<int32_t>(nseg);
+        int32_t* off = cur.take<int32_t>(c + 1);
+        int32_t* slot_lo = cur.take<int32_t>(grid);
+        int32_t* grp = cur.take<int32_t>(static_cast<size_t>(std::max<int64_t>(B.labeled_total, 1)));
+        double* sums0 = cur.take<double>(cd);
+        double* q0 = cur.take<double>(c);
+        A.sums0 = sums0; A.q0 = q0;
+        A.sums = cur.take<double>(static_cast<size_t>(grid) * cd);
+        A.table = cur.take<double>(na * c);
+        A.xn64 = cur.take<double>(na);
+        A.slot_row = cur.take<int32_t>(na);
+        A.slot_lo = slot_lo;
+        A.pend_cap = pend_cap;
+
+        // table slots: the available rows of this rank's segments only
+        std::vector<int32_t> off_h(c + 1), slot_lo_h(grid);
+        off_h[0] = 0;
+        for (int k = 0; k < c; ++k) off_h[k + 1] = off_h[k] + B.counts_h[k];
+        for (int b = 0, s = 0; b < grid; ++b) { slot_lo_h[b] = s; s += B.seg_h[S.rank * grid + b]; }
+        ALQ_CUDA(ctx, cudaMemcpyAsync(B.counts, B.counts_h.data(), static_cast<size_t>(c) * 4, cudaMemcpyHostToDevice, st));
+        ALQ_CUDA(ctx, cudaMemcpyAsync(B.seg_avail, B.seg_h.data(), static_cast<size_t>(nseg) * 4, cudaMemcpyHostToDevice, st));
+        ALQ_CUDA(ctx, cudaMemcpyAsync(off, off_h.data(), static_cast<size_t>(c + 1) * 4, cudaMemcpyHostToDevice, st));
+        ALQ_CUDA(ctx, cudaMemcpyAsync(slot_lo, slot_lo_h.data(), static_cast<size_t>(grid) * 4, cudaMemcpyHostToDevice, st));
+
+        if (group_smem > 48u * 1024u)
+            ALQ_CUDA(ctx, cudaFuncSetAttribute(bal_table_group_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(group_smem)));
+        bal_table_group_kernel<<<1, kGroupThreads, group_smem, st>>>(D->labels, D->labeled, n, c, off, grp);
+        ALQ_LAUNCH_CHECK(ctx);
+        bal_table_class_sum_kernel<<<c, kTabThreads, 0, st>>>(D->x, D->ldx, d, c, off, grp, sums0, q0);
+        ALQ_LAUNCH_CHECK(ctx);
+        return ALQ_OK;
+    }
+};
+
 }  // namespace
 
 extern "C" int alq_balancing_table_select(alq_ctx* ctx, const alq_balancing_desc* D, void* stream) {
-    static const char* const fn = "alq_balancing_table_select";
-    if (!ctx) return ALQ_ERR_INVALID;
-    int rc = alq_bal_check_desc(ctx, D, fn);
-    if (rc != ALQ_OK) return rc;
-    if (ctx->balancing_loop == 1 || ctx->balancing_loop == 2) return ALQ_OK;   // the per-step path or K11 runs
-    const int n = static_cast<int>(D->n);
-    const int c = D->c, d = D->d;
-    const bool forced = ctx->balancing_loop == 3;
-    if (n == 0 || D->budget == 0) {
-        *D->n_picks_host = 0;
-        return ALQ_OK;
-    }
-    const cudaStream_t st = static_cast<cudaStream_t>(stream);
-
-    // ---- limits that the shape decides (the same on every rank of a sharded call) -------------------------------------
-    BalShard S;
-    bool sharded = false;
-    rc = alq_bal_shard(ctx, D, n, &S, &sharded, fn);
-    if (rc != ALQ_OK) return rc;
-    const int grid = S.grid, nseg = S.world * grid;
-    const size_t smem_cap = ctx->smem_optin > 4096 ? ctx->smem_optin - 1024 : 0;   // the kernel's static shared memory
-    const size_t fixed = bal_table_smem(c, d, nseg, 0) - kBuildBytes;
-    int pend_cap = fixed < smem_cap ? static_cast<int>(std::min<size_t>(kPendMax, (smem_cap - fixed) / (static_cast<size_t>(d) * 4 + 4))) : 0;
-    while (pend_cap > 0 && bal_table_smem(c, d, nseg, pend_cap) > smem_cap) --pend_cap;
-    const size_t group_smem = static_cast<size_t>(c) * 4;
-    if (pend_cap < 1 || group_smem > smem_cap) {
-        if (!forced) return ALQ_OK;
-        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: the tables of %d classes and one pending row of %d floats need %zu bytes of shared "
-                 "memory, %zu are available (limit: class tables in shared memory)", fn, c, d,
-                 bal_table_smem(c, d, nseg, 1), smem_cap);
-    }
-    const size_t smem = bal_table_smem(c, d, nseg, pend_cap);
-    if (alq_bal_seg_rows_max(S) > kSegRowsMax) {
-        if (!forced) return ALQ_OK;
-        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: n=%d rows over %d CTAs exceed %d rows per CTA segment (limit: rows per segment)",
-                 fn, n, nseg, kSegRowsMax);
-    }
-    const size_t words = alq_bal_words_bytes(S, std::min<int64_t>(D->budget, n), sharded);
-    if (sharded && words > ctx->comm.greedy_bytes()) {
-        if (!forced) return ALQ_OK;
-        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: a budget of %lld needs %zu bytes of the peer window, %zu are usable (limit: words "
-                 "in the peer window)", fn, (long long)D->budget, words, ctx->comm.greedy_bytes());
-    }
-
-    // ---- set-up: counts, segment counts, label checks -----------------------------------------------------------
-    const size_t entries = alq_class_table_entries(n, c);
-    rc = alq_scratch_reserve(ctx, scratch_need({entries * 4, static_cast<size_t>(c) * 4, 8, static_cast<size_t>(nseg) * 4}));
-    if (rc != ALQ_OK) return rc;
-    std::vector<int32_t> counts_h(c), seg_h(nseg);
-    {
-        ScratchCursor cur(ctx->scratch);
-        int32_t* tab = cur.take<int32_t>(entries);
-        int32_t* counts = cur.take<int32_t>(c);
-        unsigned int* bad = cur.take<unsigned int>(2);
-        int32_t* seg_avail = cur.take<int32_t>(nseg);
-        rc = alq_bal_counts(ctx, D, n, c, S, tab, bad, counts, seg_avail, counts_h.data(), seg_h.data(), st, fn);
-        if (rc != ALQ_OK) return rc;
-    }
-    int64_t n_avail = 0, labeled_total = 0;
-    std::vector<int64_t> avail_of(S.world, 0);                        // available rows per rank: its table rows
-    for (int g = 0; g < nseg; ++g) {
-        n_avail += seg_h[g];
-        avail_of[g / grid] += seg_h[g];
-    }
-    for (int k = 0; k < c; ++k) labeled_total += counts_h[k];
-    const int budget = static_cast<int>(std::min<int64_t>(D->budget, n_avail));
-    if (labeled_total + budget >= (1LL << 24)) {
-        if (!forced) return ALQ_OK;
-        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: %lld labeled rows plus a budget of %d reach 2^24 (limit: counts plus budget below 2^24)",
-                 fn, (long long)labeled_total, budget);
-    }
-    if (budget == 0) {
-        *D->n_picks_host = 0;
-        return ALQ_OK;
-    }
-
-    // ---- the table and the per-CTA sums must fit the device's free memory: checked before anything is reserved ----
-    const size_t cd = static_cast<size_t>(c) * d;
-    const size_t words_b = alq_bal_words_bytes(S, budget, sharded);
-    auto need_for = [&](size_t na) {
-        return scratch_need({static_cast<size_t>(c) * 4, static_cast<size_t>(nseg) * 4, static_cast<size_t>(c + 1) * 4,
-                             static_cast<size_t>(grid) * 4, static_cast<size_t>(std::max<int64_t>(labeled_total, 1)) * 4,
-                             cd * 8, static_cast<size_t>(c) * 8, static_cast<size_t>(grid) * cd * 8, na * c * 8,
-                             na * 8, na * 4, static_cast<size_t>(n), (kMtN + 1) * 4 * 2, sharded ? 0 : words_b, 16});
-    };
-    const size_t na = static_cast<size_t>(avail_of[S.rank]);
-    const size_t need = need_for(na);
-    if (sharded) {
-        // the same decision on every rank: every rank's share against the group's least free memory (the caller's
-        // gather; this context's scratch is not counted, so the check is conservative)
-        for (int r = 0; r < S.world; ++r) {
-            const size_t nr = need_for(static_cast<size_t>(avail_of[r]));
-            const size_t want = nr + (nr >> 2) + (1u << 20);            // what alq_scratch_reserve allocates
-            if (D->group_free_bytes < 0 || want > static_cast<size_t>(D->group_free_bytes)) {
-                if (!forced) return ALQ_OK;
-                ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: rank %d's %lld x %d table (%zu bytes) and %d copies of the class sums (%zu "
-                         "bytes) need %zu bytes of device memory, the group has %lld free (limit: table in device memory)", fn,
-                         r, (long long)avail_of[r], c, static_cast<size_t>(avail_of[r]) * c * 8, grid,
-                         static_cast<size_t>(grid) * cd * 8, want, (long long)D->group_free_bytes);
-            }
-        }
-    } else if (need > ctx->scratch_bytes) {
-        size_t free_b = 0, total_b = 0;
-        ALQ_CUDA(ctx, cudaMemGetInfo(&free_b, &total_b));
-        const size_t want = need + (need >> 2) + (1u << 20);           // what alq_scratch_reserve allocates
-        if (want > free_b + ctx->scratch_bytes) {
-            if (!forced) return ALQ_OK;
-            ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: the %lld x %d table (%zu bytes) and %d copies of the class sums (%zu bytes) "
-                     "need %zu bytes of device memory, %zu are free (limit: table in device memory)", fn, (long long)n_avail, c,
-                     na * c * 8, grid, static_cast<size_t>(grid) * cd * 8, want, free_b + ctx->scratch_bytes);
-        }
-    }
-    rc = alq_scratch_reserve(ctx, need);
-    if (rc != ALQ_OK) return rc;
-    ScratchCursor cur(ctx->scratch);
-    int32_t* counts = cur.take<int32_t>(c);
-    int32_t* seg_avail = cur.take<int32_t>(nseg);
-    int32_t* off = cur.take<int32_t>(c + 1);
-    int32_t* slot_lo = cur.take<int32_t>(grid);
-    int32_t* grp = cur.take<int32_t>(static_cast<size_t>(std::max<int64_t>(labeled_total, 1)));
-    double* sums0 = cur.take<double>(cd);
-    double* q0 = cur.take<double>(c);
-    double* sums = cur.take<double>(static_cast<size_t>(grid) * cd);
-    double* table = cur.take<double>(na * c);
-    double* xn64 = cur.take<double>(na);
-    int32_t* slot_row = cur.take<int32_t>(na);
-    uint8_t* avail = cur.take<uint8_t>(n);
-    unsigned int* mt = cur.take<unsigned int>(2 * (kMtN + 1));
-    char* word_scratch = cur.take<char>(sharded ? 0 : words_b);
-    int* small = cur.take<int>(4);                                     // [0] status, [1] balancing steps
-
-    // table slots: the available rows of this rank's segments only
-    std::vector<int32_t> off_h(c + 1), slot_lo_h(grid);
-    off_h[0] = 0;
-    for (int k = 0; k < c; ++k) off_h[k + 1] = off_h[k] + counts_h[k];
-    for (int b = 0, s = 0; b < grid; ++b) { slot_lo_h[b] = s; s += seg_h[S.rank * grid + b]; }
-    ALQ_CUDA(ctx, cudaMemcpyAsync(counts, counts_h.data(), static_cast<size_t>(c) * 4, cudaMemcpyHostToDevice, st));
-    ALQ_CUDA(ctx, cudaMemcpyAsync(seg_avail, seg_h.data(), static_cast<size_t>(nseg) * 4, cudaMemcpyHostToDevice, st));
-    ALQ_CUDA(ctx, cudaMemcpyAsync(off, off_h.data(), static_cast<size_t>(c + 1) * 4, cudaMemcpyHostToDevice, st));
-    ALQ_CUDA(ctx, cudaMemcpyAsync(slot_lo, slot_lo_h.data(), static_cast<size_t>(grid) * 4, cudaMemcpyHostToDevice, st));
-
-    // ---- fp64 class sums in row order per class, and their squared norms --------------------------------------------
-    if (group_smem > 48u * 1024u)
-        ALQ_CUDA(ctx, cudaFuncSetAttribute(bal_table_group_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(group_smem)));
-    bal_table_group_kernel<<<1, kGroupThreads, group_smem, st>>>(D->labels, D->labeled, n, c, off, grp);
-    ALQ_LAUNCH_CHECK(ctx);
-    bal_table_class_sum_kernel<<<c, kTabThreads, 0, st>>>(D->x, D->ldx, d, c, off, grp, sums0, q0);
-    ALQ_LAUNCH_CHECK(ctx);
-    std::vector<unsigned int> mt_h(kMtN + 1);
-    std::copy(D->mt_key_host, D->mt_key_host + kMtN, mt_h.begin());
-    mt_h[kMtN] = static_cast<unsigned int>(*D->mt_pos_host);
-    ALQ_CUDA(ctx, cudaMemcpyAsync(mt, mt_h.data(), (kMtN + 1) * 4, cudaMemcpyHostToDevice, st));
-    ALQ_CUDA(ctx, cudaMemcpyAsync(avail, D->avail, static_cast<size_t>(n), cudaMemcpyDeviceToDevice, st));
-    ALQ_CUDA(ctx, cudaMemsetAsync(small, 0, 4 * sizeof(int), st));
-
-    // ---- the loop ---------------------------------------------------------------------------------------------------
-    TabArgs A{};
-    rc = alq_bal_words_begin(ctx, S, sharded, budget, word_scratch, &A.W, st);
-    if (rc != ALQ_OK) return rc;
-    A.x = D->x; A.ldx = D->ldx; A.d = d;
-    A.labels = D->labels; A.avail = avail;
-    A.sums0 = sums0; A.q0 = q0; A.sums = sums;
-    A.table = table; A.xn64 = xn64; A.slot_row = slot_row; A.slot_lo = slot_lo;
-    A.counts0 = counts; A.seg_avail0 = seg_avail;
-    A.mt_in = mt; A.mt_out = mt + kMtN + 1;
-    A.picks = D->picks; A.n_bal = small + 1; A.status = small;
-    A.S = S;
-    A.n = n; A.c = c; A.budget = budget; A.n_avail = static_cast<int>(n_avail); A.pend_cap = pend_cap;
-    A.timeout_cycles = static_cast<long long>(ctx->spin_timeout_ms) * ctx->clock_khz;
-    ALQ_CUDA(ctx, cudaFuncSetAttribute(balancing_table_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-    // every CTA spins on the others' words, so all of them must be resident: grid <= SMs, one CTA per SM at most
-    // (see alq_score.cu on why this is an ordinary launch and what alq_gridsync_begin/end guard against)
-    alq_gridsync_begin(ctx, st);
-    balancing_table_kernel<<<grid, kTabThreads, smem, st>>>(A);
-    const cudaError_t le = cudaGetLastError();
-    alq_gridsync_end(ctx, st);
-    ctx->launches++;
-    if (le != cudaSuccess) ALQ_FAIL(ctx, ALQ_ERR_CUDA, "%s: launch failed: %s (grid %d, %zu B shared)", fn, cudaGetErrorString(le), grid, smem);
-
-    int small_h[2] = {0, 0};
-    ALQ_CUDA(ctx, cudaMemcpyAsync(small_h, small, sizeof(small_h), cudaMemcpyDeviceToHost, st));
-    ALQ_CUDA(ctx, cudaMemcpyAsync(mt_h.data(), A.mt_out, (kMtN + 1) * 4, cudaMemcpyDeviceToHost, st));
-    ALQ_CUDA(ctx, cudaStreamSynchronize(st));
-    if (small_h[0] != 0) ALQ_FAIL(ctx, small_h[0], "%s: timed out waiting for a peer GPU or a CTA of the grid", fn);
-    std::copy(mt_h.begin(), mt_h.begin() + kMtN, D->mt_key_host);
-    *D->mt_pos_host = static_cast<int32_t>(mt_h[kMtN]);
-    *D->n_picks_host = budget;
-    *D->n_balancing_host = small_h[1];
-    return ALQ_OK;
+    return bal_select<TabLoop>(ctx, D, stream);
 }
