@@ -140,6 +140,10 @@ SIGNATURES = {
                                  C.c_void_p]),
     "alq_balancing_select": (C.c_int, [C.c_void_p, C.POINTER(BalancingDesc), C.c_void_p]),
     "alq_balancing_table_select": (C.c_int, [C.c_void_p, C.POINTER(BalancingDesc), C.c_void_p]),
+    "alq_probcover_graph": (C.c_int, [C.c_void_p, c_f32p, C.c_int64, C.c_int32, C.c_int64, C.c_void_p, c_f32p, c_i32p,
+                                      C.c_void_p, c_i32p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "alq_probcover_select": (C.c_int, [C.c_void_p, C.c_void_p, c_i32p, C.c_int64, C.c_void_p, C.c_int64, c_i32p,
+                                       C.c_void_p, C.c_void_p]),
 }
 
 

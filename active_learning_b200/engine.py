@@ -774,6 +774,74 @@ class Engine:
         np.random.set_state((sname, key, int(pos_c.value), has_gauss, cached))
         return picks[:n_picks.value].cpu().numpy().astype(np.int64), int(n_bal.value)
 
+    # -- K13 / K14: ProbCover ---------------------------------------------------------------------------
+    PROBCOVER_HEADROOM_BYTES = 1 << 30   # K14's scratch and whatever else the query holds next to the edges
+
+    @classmethod
+    def probcover_bytes(cls, nnz: int) -> int:
+        """Device memory the columns of a delta-ball graph with nnz edges need: 4 nnz plus headroom."""
+        return 4 * int(nnz) + cls.PROBCOVER_HEADROOM_BYTES
+
+    def probcover_graph(self, x: torch.Tensor, delta: float):
+        """K13: the delta-ball graph of the L2-normalised rows of x [n, d] (float32, CUDA) as CSR: (row_ptr int64 [n + 1],
+        cols int32 [nnz], recheck) with an edge (i, j) iff scipy's fp64 euclidean distance of the normalised fp32 rows is
+        < delta, every row's columns ascending, (i, j) and (j, i) both stored.  `recheck` is the number of pairs the
+        tensor-core screen left to the exact recomputation.  ValueError for n = 0, a delta that is not finite and > 0, or
+        non-finite rows, before anything runs; AlqError naming n, nnz and the bytes when the edges do not fit in the free
+        device memory, checked after the count and before the fill."""
+        delta = float(delta)
+        if not (math.isfinite(delta) and delta > 0):
+            raise ValueError(f"probcover: delta must be finite and > 0, got {delta}")
+        x = _f32c(x, "x")
+        if x.dim() != 2 or x.shape[0] == 0:
+            raise ValueError(f"probcover: need a non-empty [n, d] matrix, got {tuple(x.shape)}")
+        n, d = x.shape
+        if not bool(torch.isfinite(x).all()):
+            raise ValueError("probcover: the embeddings contain NaN or infinity")
+        dp = max(4, (d + 3) & ~3)
+        if dp != d:                                    # the tensor maps want 16-byte rows: zero columns change no distance
+            slab = torch.zeros((n, dp), dtype=torch.float32, device=x.device)
+            slab[:, :d] = x
+            x = slab
+        nt = (n + 127) // 128
+        xhat = torch.empty((n, dp), dtype=torch.float32, device=x.device)
+        tile = torch.empty(n * nt, dtype=torch.int32, device=x.device)
+        row_ptr = torch.empty(n + 1, dtype=torch.int64, device=x.device)
+        dh, nnz, rech = C.c_double(delta), C.c_int64(0), C.c_int64(0)
+        self._check(self.lib.alq_probcover_graph(self._h, _ptr(x), n, dp, _ld(x), C.byref(dh), _ptr(xhat), _ptr(tile),
+                                                 _ptr(row_ptr), None, C.byref(nnz), C.byref(rech), self._stream()),
+                    "alq_probcover_graph")
+        need, free = self.probcover_bytes(nnz.value), self._ward_free_bytes()
+        if need > free:
+            raise AlqError(f"probcover: n={n} rows at delta={delta} give nnz={nnz.value} edges, which need {need} bytes of "
+                           f"device memory (4 nnz with {self.PROBCOVER_HEADROOM_BYTES} headroom); {free} are free; use a "
+                           f"smaller delta or subset_unlabeled")
+        cols = torch.empty(max(nnz.value, 1), dtype=torch.int32, device=x.device)
+        self._check(self.lib.alq_probcover_graph(self._h, None, n, dp, dp, C.byref(dh), _ptr(xhat), _ptr(tile),
+                                                 _ptr(row_ptr), _ptr(cols), C.byref(nnz), C.byref(rech), self._stream()),
+                    "alq_probcover_graph")
+        return row_ptr, cols[:nnz.value], int(rech.value)
+
+    def probcover_select(self, row_ptr: torch.Tensor, cols: torch.Tensor, labeled: torch.Tensor, budget: int):
+        """K14: the greedy coverage picks over probcover_graph's CSR: each step takes the lowest row of the largest number
+        of uncovered rows in its ball and covers them, starting from the balls of the rows with labeled != 0 covered, and
+        stops early when nothing uncovered is left.  Returns (picks: host int64 array in pick order, greedy steps)."""
+        n = row_ptr.numel() - 1
+        if (not labeled.is_cuda or labeled.dtype not in (torch.uint8, torch.bool) or labeled.numel() != n
+                or row_ptr.dtype != torch.int64 or cols.dtype != torch.int32 or not row_ptr.is_cuda or not cols.is_cuda):
+            raise AlqError("probcover_select: row_ptr (int64), cols (int32) and labeled (uint8 or bool, one entry per row) "
+                           "must be CUDA tensors")
+        budget = int(budget)
+        row_ptr, cols = row_ptr.contiguous(), cols.contiguous()
+        lab = labeled.contiguous().view(torch.uint8).reshape(-1)
+        picks = torch.empty(max(budget, 1), dtype=torch.int32, device=row_ptr.device)
+        # an empty cols tensor has a null data pointer, which the library refuses: any device address stands in
+        cp = _ptr(cols) if cols.numel() else _ptr(row_ptr)
+        steps = C.c_int64(0)
+        self._check(self.lib.alq_probcover_select(self._h, _ptr(row_ptr), cp, n, _ptr(lab), budget,
+                                                  _ptr(picks), C.byref(steps), self._stream()), "alq_probcover_select")
+        return picks[:steps.value].cpu().numpy().astype(np.int64), int(steps.value)
+
     # -- K4 / K5 ---------------------------------------------------------------------------------------
     def leaf_bounds(self, n: int) -> np.ndarray:
         """Leaf boundaries of NumPy's float32 pairwise summation over n entries (host helper of the library)."""

@@ -20,6 +20,7 @@ from .query_strategies.balanced_random import BalancedRandomQuery
 from .query_strategies.balancing import BalancingQuery
 from .query_strategies.margin_clustering import MarginClusteringQuery
 from .query_strategies.mase import BASEQuery, MASEQuery
+from .query_strategies.probcover import ProbCoverQuery
 from .query_strategies.uncertainty import ConfidenceQuery, EntropyQuery, MarginQuery
 from .query_strategies.vaal import VAALQuery
 
@@ -36,6 +37,7 @@ _MIXINS = {
     "BalancingSampler": BalancingQuery,
     "MarginClusteringSampler": MarginClusteringQuery,
     "BalancedRandomSampler": BalancedRandomQuery,
+    "ProbCoverSampler": ProbCoverQuery,
 }
 
 

@@ -1,7 +1,8 @@
 """`--strategy` dispatch, same contract as active_learning/src/query_strategies/get_strategy.py:
 `get_strategy(name)` returns the class called `name`.  Every class name the reference dispatches is implemented: the
 thirteen accelerated samplers (the seven of the north-star path plus MASE / BASE / Balancing, SURVEY.md section 8f,
-MarginClustering, VAAL and BalancedRandom) and the default RandomSampler."""
+MarginClustering, VAAL and BalancedRandom) and the default RandomSampler.  ProbCoverSampler is this project's addition
+(no reference counterpart; it needs the sampler kwarg `delta`)."""
 from .badge_sampler import BADGESampler  # noqa: F401
 from .balanced_random_sampler import BalancedRandomSampler  # noqa: F401
 from .balancing_sampler import BalancingSampler  # noqa: F401
@@ -14,12 +15,14 @@ from .margin_sampler import MarginSampler  # noqa: F401
 from .mase_sampler import MASESampler  # noqa: F401
 from .partitioned_badge_sampler import PartitionedBADGESampler  # noqa: F401
 from .partitioned_coreset_sampler import PartitionedCoresetSampler  # noqa: F401
+from .probcover_sampler import ProbCoverSampler  # noqa: F401
 from .random_sampler import RandomSampler  # noqa: F401
 from .vaal_sampler import VAALSampler  # noqa: F401
 
 ACCELERATED = ("MarginSampler", "ConfidenceSampler", "EntropySampler", "CoresetSampler",
                "PartitionedCoresetSampler", "BADGESampler", "PartitionedBADGESampler", "MASESampler", "BASESampler",
-               "BalancingSampler", "MarginClusteringSampler", "VAALSampler", "BalancedRandomSampler")
+               "BalancingSampler", "MarginClusteringSampler", "VAALSampler", "BalancedRandomSampler",
+               "ProbCoverSampler")
 NOT_ON_THIS_PATH = ()
 
 

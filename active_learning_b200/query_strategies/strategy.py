@@ -143,7 +143,7 @@ class EngineMixin:
         # save_experiment pickles the whole Strategy every round (utils/resume_training.py:49) and
         # train() pickles it into mp.spawn workers (strategy.py:297): keep handles and caches out.
         state = dict(self.__dict__)
-        for k in ("_engine", "_shard_group", "_saved_embeddings", "_emb_cache", "_bal_cache"):
+        for k in ("_engine", "_shard_group", "_saved_embeddings", "_emb_cache", "_bal_cache", "_pc_cache"):
             state.pop(k, None)
         return state
 

@@ -496,6 +496,31 @@ int alq_balancing_select(alq_ctx* ctx, const alq_balancing_desc* desc, void* str
  * the loop: six, whatever the budget.  Synchronous.                                                               */
 int alq_balancing_table_select(alq_ctx* ctx, const alq_balancing_desc* desc, void* stream);
 
+/* ---- K13 / K14: ProbCover (Yehuda et al., NeurIPS 2022) --------------------------------------------------------------
+ * alq_probcover_graph (K13): the delta-ball graph of x[n, d] (fp32, d % 4 == 0, ldx >= d, any alignment) as CSR.  Every
+ *   row is L2-normalised into xhat[n, d] (caller-owned, 16-byte aligned): lane l of a warp sums the fp64 squares of
+ *   columns l, l + 32, .. in order, a butterfly (xor 16, 8, 4, 2, 1) adds the 32 partials, norm = sqrt, and
+ *   xhat = fl32(x / norm) in fp64 (a zero row stays zero).  There is an edge (i, j) iff scipy's fp64 euclidean distance of
+ *   xhat_i and xhat_j (K7's pair arithmetic: d = a - b, s = s + d * d, k ascending, no FMA, sqrt) is < *delta_host, so
+ *   every (i, i) is an edge.  The pairs are screened on the tensor cores (3xTF32) with a rigorous error bound (DESIGN
+ *   section 4); only pairs inside the bound's band are recomputed exactly.  Two calls, same x, d and delta:
+ *     count (cols == NULL): writes xhat, tile_cnt (caller-owned int32 [n * ceil(n / 128)], scratch of the fill), row_ptr
+ *       (int64 [n + 1]), *nnz_host = row_ptr[n] and *recheck_host = the pairs decided by the exact recomputation.
+ *     fill (cols != NULL, int32 [nnz]): reads xhat, tile_cnt and row_ptr as the count left them (x is not read) and
+ *       writes every row's columns, ascending; (i, j) and (j, i) are both stored.
+ *   The caller checks that nnz fits in memory between the two calls.  n in [1, 2^31), delta finite and > 0, otherwise
+ *   ALQ_ERR_INVALID.  Synchronous.
+ * alq_probcover_select (K14): the greedy coverage picks over that CSR.  covered[y] starts true for every y in the ball
+ *   of a row with labeled[row] != 0 and deg[x] = |{y in N(x) : y uncovered}|; each step stops if max deg = 0, else picks
+ *   c = the lowest row of the maximum and covers every uncovered y in N(c).  picks[0 .. *n_steps_host) (int32, device) in
+ *   pick order, *n_steps_host <= budget <= n.  Set-up: two launches; then ONE launch runs every step (one CTA per SM,
+ *   agreement over 8-byte LL words, every wait bounded by "spin_timeout_ms").  n / SMs <= 65 534.  Synchronous. */
+int alq_probcover_graph(alq_ctx* ctx, const float* x, int64_t n, int32_t d, int64_t ldx, const double* delta_host,
+                        float* xhat, int32_t* tile_cnt, int64_t* row_ptr, int32_t* cols, int64_t* nnz_host,
+                        int64_t* recheck_host, void* stream);
+int alq_probcover_select(alq_ctx* ctx, const int64_t* row_ptr, const int32_t* cols, int64_t n, const uint8_t* labeled,
+                         int64_t budget, int32_t* picks, int64_t* n_steps_host, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
