@@ -21,7 +21,7 @@
 // A row's dot product with a centre is a fixed function of that row: lane l accumulates the float4 chunks l, l + 32, ..
 // with fmaf in x, y, z, w order, and a butterfly folds the 32 partials (every lane ends with the same value).  Neither the
 // warp, nor the CTA, nor the grid size changes it, so the picks are bit-reproducible.
-// Sharded over a group (shard_off_host), the segments above are every rank's CTA segments (BalShard): every CTA of every
+// Sharded over a group (shard_off_host), the segments above are every rank's CTA segments (SegShard): every CTA of every
 // rank keeps all of their counts, the key words go into every rank's window and the owner of a random pick stores its
 // word there too; K12 shares the layout.
 // The host side of a call is bal_select (alq_balancing.cuh), shared with K12; this file supplies K11's part of it
@@ -49,8 +49,8 @@ struct BalArgs {
     int* picks;
     int* n_bal;
     int* status;
-    BalShard S;
-    BalWords W;                  // key words of the balancing steps (two parities), one pick word per random step
+    SegShard S;
+    LLWords W;                   // key words of the balancing steps (two parities), one pick word per random step
     int n, c, budget, n_avail;
     long long timeout_cycles;
 };
@@ -75,7 +75,7 @@ __device__ __forceinline__ float dot_fixed(const float4* x, const float4* q, int
 
 // available rows per global segment (one block each); the smallest available row with a label outside [0, c) -> *bad
 __global__ void __launch_bounds__(256) bal_seg_count_kernel(const int* __restrict__ labels, const uint8_t* __restrict__ avail,
-                                                            int c, const __grid_constant__ BalShard S, int* __restrict__ seg_avail,
+                                                            int c, const __grid_constant__ SegShard S, int* __restrict__ seg_avail,
                                                             unsigned int* __restrict__ bad) {
     __shared__ int wsum[8];
     const int lo = gseg_lo(S, blockIdx.x), hi = gseg_lo(S, blockIdx.x + 1);
@@ -182,7 +182,8 @@ __global__ void __launch_bounds__(kBalThreads, 1) balancing_loop_kernel(const __
         const float v = dot_fixed(q, q, dv, lane);
         if (lane == 0) cn[k] = v;
     }
-    bal_ready_wait(A, tid);
+    if (A.W.ready_tag != 0 && tid < A.S.world) ll_ready_wait(A.W.peer[A.S.rank], tid, A.W.ready_tag, A);
+    __syncthreads();
 
     unsigned int rnd_key = 0;
     int n_bal = 0;
@@ -236,7 +237,7 @@ __global__ void __launch_bounds__(kBalThreads, 1) balancing_loop_kernel(const __
             }
             if (lane == 0) s_key[warp] = best;
             __syncthreads();
-            bal_agree<kBalWarps>(A, s_key, &s_pick, ++rnd_key, row_lo, tid);
+            ll_agree_min_call<kBalWarps>(A, s_key, &s_pick, ++rnd_key, row_lo, tid);
         } else {
             // ===== random step (balancing_sampler.py:128): np.random.choice over the available rows =====
             if (tid == 0) {
@@ -363,7 +364,7 @@ struct BalLoop {
 
 }  // namespace
 
-int bal_seg_count(alq_ctx* ctx, const int32_t* labels, const uint8_t* avail, int c, const BalShard& S, int32_t* seg_avail,
+int bal_seg_count(alq_ctx* ctx, const int32_t* labels, const uint8_t* avail, int c, const SegShard& S, int32_t* seg_avail,
                   unsigned int* bad, cudaStream_t st) {
     bal_seg_count_kernel<<<S.world * S.grid, 256, 0, st>>>(labels, avail, c, S, seg_avail, bad);
     ALQ_LAUNCH_CHECK(ctx);

@@ -1,53 +1,22 @@
-// Shared by K11 (alq_balancing.cu) and K12 (alq_balancing_table.cu), BalancingSampler's persistent query: the CTA
-// segments, the LL-word agreement, the fp32 imbalance test, the class denominators, NumPy's MT19937 and bal_select, the
-// host driver of both entry points.
+// Shared by K11 (alq_balancing.cu) and K12 (alq_balancing_table.cu), BalancingSampler's persistent query: the segment of
+// a row, the pick words, the fp32 imbalance test, the class denominators, NumPy's MT19937 and bal_select, the host driver
+// of both entry points.  The CTA segments and the LL-word agreement: alq_ll.cuh.
 #pragma once
 #include <limits.h>
 
-#include "alq_greedy.cuh"
-
-// The rows of a call and who streams them.  Rank r owns rows [off[r], off[r + 1]) and runs `grid` CTAs on them; global
-// segment g = r * grid + b, CTA b of rank r, starts at off[r] + seg_lo(off[r + 1] - off[r], grid, b).  A single GPU is
-// world 1, rank 0, off = {0, n}: segment b starts at seg_lo(n, grid, b).  Every array stays global and replicated, so
-// every rank derives the same world * grid segments.
-struct BalShard {
-    int world, rank, grid;
-    int off[ALQ_MAX_WORLD + 1];
-};
-
-// Where the LL words of a call live.  peer[r] is rank r's window (a single GPU: peer[0] is scratch of this call); every
-// window has the same layout: u64 ready[ALQ_MAX_WORLD] (sharded calls), the key words [2 parities][world * grid] at
-// `keyw` and one pick word per step at `pickw`.  Tags carry the call's epoch (0 on a single GPU).
-struct BalWords {
-    char* peer[ALQ_MAX_WORLD];
-    unsigned int keyw, pickw;
-    unsigned int tag_base;               // 0x80000000 | (epoch & 0x7f) << 24: never 0, a zeroed word is invalid
-    unsigned long long ready_tag;        // sharded: epoch << 32, stored into every peer's ready[rank]; 0: no handshake
-};
+#include "alq_ll.cuh"
 
 // The driver's one step that lives in K11's file (alq_balancing.cu), beside its kernel: one launch counting the available
 // rows of every global segment (seg_avail[world * grid]) and the smallest available row with a label outside [0, c)
 // (atomicMin into *bad).
-int bal_seg_count(alq_ctx* ctx, const int32_t* labels, const uint8_t* avail, int c, const BalShard& S, int32_t* seg_avail,
+int bal_seg_count(alq_ctx* ctx, const int32_t* labels, const uint8_t* avail, int c, const SegShard& S, int32_t* seg_avail,
                   unsigned int* bad, cudaStream_t st);
 
 namespace {
 
 constexpr int kMtN = 624;
-constexpr int kSegRowsMax = 65535;               // the key word carries a 16-bit row offset (0xffff: empty segment)
-constexpr unsigned int kEmptyOff = 0xffffu;
-
-__host__ __device__ __forceinline__ int seg_lo(int n, int grid, int b) {
-    return static_cast<int>(static_cast<long long>(n) * b / grid);
-}
-
-__host__ __device__ __forceinline__ int gseg_lo(const BalShard& S, int g) {
-    const int r = g / S.grid;
-    if (r >= S.world) return S.off[S.world];
-    return S.off[r] + seg_lo(S.off[r + 1] - S.off[r], S.grid, g - r * S.grid);
-}
 // the global segment holding `row` (0 <= row < off[world])
-__device__ __forceinline__ int gseg_of(const BalShard& S, int row) {
+__device__ __forceinline__ int gseg_of(const SegShard& S, int row) {
     int r = 0;
     while (r + 1 < S.world && S.off[r + 1] <= row) ++r;
     const int grid = S.grid, rows = S.off[r + 1] - S.off[r], p = row - S.off[r];
@@ -57,68 +26,8 @@ __device__ __forceinline__ int gseg_of(const BalShard& S, int row) {
     return r * grid + o;
 }
 
-__device__ __forceinline__ unsigned int bal_key_tag(const BalWords& W, unsigned int round) {
-    return 0x8000u | ((W.tag_base >> 12) & 0x7000u) | (round & 0xfffu);
-}
-__device__ __forceinline__ unsigned int bal_pick_tag(const BalWords& W, int t) {   // t < 2^24: the budget limit
+__device__ __forceinline__ unsigned int bal_pick_tag(const LLWords& W, int t) {   // t < 2^24: the budget limit
     return W.tag_base | static_cast<unsigned int>(t);
-}
-
-// Sharded calls: no CTA stores into a peer's window before that peer has cleared it for this call (its ready word).
-// Called by every thread; ends with a barrier.
-template <typename Args>
-__device__ __forceinline__ void bal_ready_wait(const Args& A, int tid) {
-    if (A.W.ready_tag != 0 && tid < A.S.world) {
-        const unsigned long long* rw = reinterpret_cast<const unsigned long long*>(A.W.peer[A.S.rank]) + tid;
-        for (const long long t0 = clock64(); ld_acquire_sys(rw) != A.W.ready_tag;) {
-            if (clock64() - t0 > A.timeout_cycles) { atomicCAS(A.status, 0, ALQ_ERR_STATE); break; }
-            __nanosleep(200);
-        }
-    }
-    __syncthreads();
-}
-
-// A balancing step's agreement.  s_key[0 .. kWarps) holds each warp's smallest key (ord(ratio) << 32 | row, ~0: none)
-// and a barrier has passed.  The CTA's minimum goes as one word {tag16, row offset16, ord32} into slot rank * grid + b
-// of every rank's window; every CTA gathers all world * grid words and returns the smallest key's row (-1: none, or a
-// failed wait) to every thread.  Not inlined: K12's loop sits at the 128-register cap of its launch bounds, and the
-// exchange inlined into it spills.
-template <int kWarps, typename Args>
-__device__ __noinline__ int bal_agree(const Args& A, unsigned long long* s_key, int* s_pick, unsigned int round,
-                                         int row_lo, int tid) {
-    const BalShard& S = A.S;
-    const int nseg = S.world * S.grid, lane = tid & 31, warp = tid >> 5;
-    const unsigned int tag16 = bal_key_tag(A.W, round);
-    const size_t keyw = A.W.keyw + static_cast<size_t>(round & 1u) * nseg * 8;
-    if (tid < S.world) {
-        unsigned long long m = s_key[0];
-        for (int w = 1; w < kWarps; ++w) m = s_key[w] < m ? s_key[w] : m;
-        const unsigned long long off = m == ~0ull ? kEmptyOff : static_cast<unsigned long long>(static_cast<uint32_t>(m) - row_lo);
-        ll_store_raw(A.W.peer[tid] + keyw + static_cast<size_t>(S.rank * S.grid + blockIdx.x) * 8,
-                     (static_cast<unsigned long long>(tag16) << 48) | (off << 32) | (m >> 32));
-    }
-    unsigned long long mine = ~0ull;
-    ll_gather(A.W.peer[S.rank] + keyw, nseg, 8, tag16, 48, A, tid, [&](int i, unsigned long long w) {
-        const unsigned int off = static_cast<unsigned int>(w >> 32) & 0xffffu;
-        if (off == kEmptyOff) return;
-        const unsigned long long key = ((w & 0xffffffffull) << 32) | static_cast<uint32_t>(gseg_lo(S, i) + static_cast<int>(off));
-        mine = key < mine ? key : mine;
-    });
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        const unsigned long long w = __shfl_xor_sync(0xffffffffu, mine, o);
-        mine = w < mine ? w : mine;
-    }
-    __syncthreads();                                              // s_key is reused
-    if (lane == 0) s_key[warp] = mine;
-    __syncthreads();
-    if (tid == 0) {
-        unsigned long long m = s_key[0];
-        for (int w = 1; w < kWarps; ++w) m = s_key[w] < m ? s_key[w] : m;
-        *s_pick = m == ~0ull ? -1 : static_cast<int>(static_cast<uint32_t>(m));
-    }
-    __syncthreads();
-    return *s_pick;
 }
 
 // balancing_sampler.py:89 in fp32: fl32(count + 1e-5)
@@ -212,7 +121,7 @@ struct BalCall {
     int n, c, d;
     bool forced, sharded;
     bool declined;                               // a limit of the loop's own steps declined the call (BAL_LIMIT)
-    BalShard S;
+    SegShard S;
     int nseg;
     size_t smem_cap;                             // dynamic shared memory per CTA (the kernels' static shared memory aside)
     size_t entries;                              // K10's table pass (int32)
@@ -228,7 +137,7 @@ struct BalCall {
 size_t up128(size_t v) { return (v + 127) & ~size_t(127); }
 
 // Bytes of the LL words (from the window's start); sharded calls need them inside the window's greedy region.
-size_t bal_words_bytes(const BalShard& S, int64_t budget, bool sharded) {
+size_t bal_words_bytes(const SegShard& S, int64_t budget, bool sharded) {
     const size_t keyw = sharded ? kWordsHead : 0;
     return up128(keyw + static_cast<size_t>(2) * S.world * S.grid * 8) + static_cast<size_t>(budget) * 8;
 }
@@ -275,7 +184,7 @@ int bal_select(alq_ctx* ctx, const alq_balancing_desc* D, void* stream) {
     // The layout (S.grid from the smallest shard, the same on every rank).  A sharded call (the descriptor carries
     // shard_off_host) needs the group of alq_comm_create/connect and shard offsets that start at 0, do not decrease and
     // end at n.
-    BalShard& S = B.S;
+    SegShard& S = B.S;
     const int32_t* so = D->struct_size >= sizeof(alq_balancing_desc) ? D->shard_off_host : nullptr;
     B.sharded = so != nullptr;
     S.world = 1;
@@ -371,7 +280,7 @@ int bal_select(alq_ctx* ctx, const alq_balancing_desc* D, void* stream) {
 
     // ---- the LL words: a single GPU keeps them in scratch; a sharded call uses the group's window, bumps the epoch and,
     // after the clear in stream order, stores its ready word into every peer's window ---------------------------------
-    BalWords& W = A.W;
+    LLWords& W = A.W;
     W.keyw = static_cast<unsigned int>(B.sharded ? kWordsHead : 0);
     W.pickw = static_cast<unsigned int>(up128(W.keyw + static_cast<size_t>(2) * nseg * 8));
     W.tag_base = 0x80000000u;
@@ -397,15 +306,14 @@ int bal_select(alq_ctx* ctx, const alq_balancing_desc* D, void* stream) {
     A.picks = D->picks; A.n_bal = small + 1; A.status = small;
     A.S = S;
     A.n = n; A.c = c; A.budget = B.budget; A.n_avail = static_cast<int>(B.n_avail);
-    A.timeout_cycles = static_cast<long long>(ctx->spin_timeout_ms) * ctx->clock_khz;
+    A.timeout_cycles = ctx->spin_timeout_cycles();
     ALQ_CUDA(ctx, cudaFuncSetAttribute(K::kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(k.smem)));
     // every CTA spins on the others' words, so all of them must be resident: grid <= SMs, one CTA per SM at most
-    // (see alq_score.cu on why this is an ordinary launch and what alq_gridsync_begin/end guard against)
-    alq_gridsync_begin(ctx, st);
-    K::kernel<<<S.grid, K::kThreads, k.smem, st>>>(A);
-    const cudaError_t le = cudaGetLastError();
-    alq_gridsync_end(ctx, st);
-    ctx->launches++;
+    // (see alq_score.cu on why this is an ordinary launch)
+    const cudaError_t le = alq_gridsync_launch(ctx, st, [&] {
+        K::kernel<<<S.grid, K::kThreads, k.smem, st>>>(A);
+        return cudaGetLastError();
+    });
     if (le != cudaSuccess) ALQ_FAIL(ctx, ALQ_ERR_CUDA, "%s: launch failed: %s (grid %d, %zu B shared)", fn, cudaGetErrorString(le), S.grid, k.smem);
 
     int small_h[2] = {0, 0};

@@ -59,8 +59,8 @@ struct TabArgs {
     int* picks;
     int* n_bal;
     int* status;
-    BalShard S;
-    BalWords W;                  // key words of the balancing steps (two parities), one pick word per random step
+    SegShard S;
+    LLWords W;                   // key words of the balancing steps (two parities), one pick word per random step
     int n, c, budget, n_avail, pend_cap;
     long long timeout_cycles;
 };
@@ -183,7 +183,8 @@ __global__ void __launch_bounds__(kTabThreads, 1) balancing_table_kernel(const _
     for (int i = tid; i < kMtN; i += kTabThreads) mt[i] = A.mt_in[i];
     if (tid == 0) { s_mtpos = static_cast<int>(A.mt_in[kMtN]); s_navail = A.n_avail; }
     for (size_t i = tid; i < static_cast<size_t>(c) * d; i += kTabThreads) my_sums[i] = A.sums0[i];
-    bal_ready_wait(A, tid);
+    if (A.W.ready_tag != 0 && tid < A.S.world) ll_ready_wait(A.W.peer[A.S.rank], tid, A.W.ready_tag, A);
+    __syncthreads();
 
     // the table rows of my slots, streamed once per balancing step: apply the pending picks (in pick order) and,
     // when `score`, return the warp's smallest key (ord(fl32(near / far) + 0) << 32 | row)
@@ -376,7 +377,7 @@ __global__ void __launch_bounds__(kTabThreads, 1) balancing_table_kernel(const _
             npend = 0;
             if (lane == 0) s_key[warp] = best;
             __syncthreads();
-            bal_agree<kTabWarps>(A, s_key, &s_pick, ++rnd_key, row_lo, tid);
+            ll_agree_min_call<kTabWarps>(A, s_key, &s_pick, ++rnd_key, row_lo, tid);
         } else {
             // ===== random step (balancing_sampler.py:128): np.random.choice over the available rows =====
             if (tid == 0) {
@@ -492,7 +493,7 @@ struct TabLoop {
     // then the table slots, the fp64 class sums in row order per class and their squared norms
     int setup(alq_ctx* ctx, BalCall& B, ScratchCursor& cur, TabArgs& A) {
         const alq_balancing_desc* D = B.D;
-        const BalShard& S = B.S;
+        const SegShard& S = B.S;
         const cudaStream_t st = B.st;
         const int n = B.n, c = B.c, d = B.d, grid = S.grid, nseg = B.nseg;
         std::vector<int64_t> avail_of(S.world, 0);                    // available rows per rank: its table rows

@@ -95,6 +95,8 @@ struct alq_ctx {
     int base_impl = 0;        // 0 auto, 1 sequential class loop, 2 parallel candidate lists + in-order resolve
     int balancing_loop = 0;   // 0 auto, 1 per-step path (K11 and K12 decline), 2 K11 (error beyond its limits), 3 K12 (the same)
     std::string err;
+    // the bound of every spin on a peer or a CTA of the grid, in SM clock cycles
+    long long spin_timeout_cycles() const { return static_cast<long long>(spin_timeout_ms) * clock_khz; }
 };
 
 #define ALQ_FAIL(ctx, code, ...)                                   \
@@ -124,12 +126,22 @@ struct alq_ctx {
         }                                                                                \
     } while (0)
 
-// Device scratch: returns a 256-byte aligned pointer into the arena, growing it if needed.
-// Grid-synchronising kernels launched WITHOUT the cooperative API (see alq_score.cu) must never share the device with
-// another one of this process: every such launch is bracketed by these two (one event per device, process-wide).
+// Grid-synchronising kernels (see alq_score.cu) must never share the device with another one of this process: every
+// such launch is bracketed by these two (one event per device, process-wide).  Call them through alq_gridsync_launch.
 void alq_gridsync_begin(alq_ctx* ctx, cudaStream_t st);
 void alq_gridsync_end(alq_ctx* ctx, cudaStream_t st);
+// Runs `launch` (enqueues one grid-synchronising kernel on `st` and returns its launch error) between
+// alq_gridsync_begin and alq_gridsync_end, counts the launch and returns the launch error.
+template <typename Launch>
+cudaError_t alq_gridsync_launch(alq_ctx* ctx, cudaStream_t st, Launch&& launch) {
+    alq_gridsync_begin(ctx, st);
+    const cudaError_t e = launch();
+    alq_gridsync_end(ctx, st);
+    ctx->launches++;
+    return e;
+}
 
+// Device scratch: returns a 256-byte aligned pointer into the arena, growing it if needed.
 int alq_scratch_reserve(alq_ctx* ctx, size_t bytes);
 // The start-of-call handshake of a collective call over the group's windows (alq_comm.cu): once this rank has cleared
 // its window for the call (earlier on `st`), store `tag` into ready[rank] of every rank's window, the u64

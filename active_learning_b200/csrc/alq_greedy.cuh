@@ -1,10 +1,10 @@
 // Pieces shared by the selection-loop kernels (alq_greedy.cu: one launch per step; alq_greedy_persist.cu: one
-// persistent cooperative launch for the whole loop).
+// persistent cooperative launch for the whole loop).  The LL words of the persistent loop: alq_ll.cuh.
 #pragma once
 #include <math.h>
 #include <stdlib.h>
 
-#include "alq_common.cuh"
+#include "alq_ll.cuh"
 
 namespace {
 
@@ -127,87 +127,6 @@ private:
         return {-static_cast<int>(internal.size()), h};
     }
 };
-
-
-// ---- LL words (alq_greedy_persist.cu, alq_balancing.cu) -------------------------------------------------------
-// 8 bytes = {32-bit tag, 32-bit payload} written with one plain store (single-copy atomic, so no fence and no separate
-// flag) and polled at the destination until the tag matches.  `Args` is the kernel's argument block: it provides
-// `int* status` (sticky failure word) and `long long timeout_cycles`.
-__device__ __forceinline__ void ll_store(void* p, unsigned int tag, unsigned int payload) {
-    const unsigned long long v = (static_cast<unsigned long long>(tag) << 32) | payload;
-    asm volatile("st.relaxed.sys.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
-}
-__device__ __forceinline__ void ll_store_raw(void* p, unsigned long long v) {
-    asm volatile("st.relaxed.sys.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
-}
-__device__ __forceinline__ unsigned long long ll_load(const void* p) {
-    unsigned long long v;
-    asm volatile("ld.relaxed.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-    return v;
-}
-// Bounded spin; after a failure anywhere (sticky status) every wait returns at once, so the loop drains
-// to its end in bounded time instead of hanging the GPU on a dead peer.
-template <typename Args>
-__device__ __forceinline__ bool ll_give_up(int spin, long long t0, const Args& A) {
-    if ((spin & 63) != 63) return false;
-    if (*reinterpret_cast<volatile int*>(A.status) != 0) return true;
-    if (clock64() - t0 > A.timeout_cycles) { atomicCAS(A.status, 0, ALQ_ERR_STATE); return true; }
-    return false;
-}
-template <typename Args>
-__device__ __forceinline__ unsigned int ll_wait(const void* p, unsigned int tag, const Args& A) {
-    unsigned long long v = ll_load(p);
-    if (static_cast<unsigned int>(v >> 32) == tag) return static_cast<unsigned int>(v);
-    const long long t0 = clock64();
-    for (int spin = 0;; ++spin) {
-        v = ll_load(p);
-        if (static_cast<unsigned int>(v >> 32) == tag || ll_give_up(spin, t0, A)) break;
-    }
-    return static_cast<unsigned int>(v);
-}
-// Collect `nwords` LL words at `base` (stride `stride` bytes) whose top (64 - shift) bits equal `tag`.
-// Polling is what floods L2 when 75 000 threads spin on words that are not there yet (measured: it slows the CTAs
-// that still stream and every store behind it), so it is rationed: only the first kPollers threads (`ct`) poll;
-// (1) one warp spins on 32 sentinel words spread over the range -- one load per lane per round -- and only when
-// those have arrived (2) every poller loads its up-to-kBatch words as one batch (one L2 round trip), re-loading just
-// the few still missing.  Called by every thread with ct < kPollers (named barrier 2); the caller follows it with a
-// barrier of its own.
-constexpr int kPollers = 320;
-constexpr int kBatch = 8;
-template <typename Args, typename Sink>
-__device__ __forceinline__ void ll_gather(const char* base, int nwords, int stride, unsigned long long tag, int shift,
-                                          const Args& A, int ct, Sink&& sink) {
-    if (ct >= kPollers) return;
-    if (ct < 32 && nwords > 0) {
-        const char* sp = base + static_cast<size_t>(static_cast<long long>(ct) * nwords / 32) * stride;
-        const long long t0 = clock64();
-        for (int spin = 0; (ll_load(sp) >> shift) != tag; ++spin) {
-            if (ll_give_up(spin, t0, A)) break;
-            __nanosleep(40);
-        }
-    }
-    asm volatile("bar.sync 2, %0;" ::"n"(kPollers) : "memory");
-    for (int chunk = 0; chunk < nwords; chunk += kPollers * kBatch) {
-        unsigned int pend = 0;
-#pragma unroll
-        for (int q = 0; q < kBatch; ++q)
-            if (chunk + ct + q * kPollers < nwords) pend |= 1u << q;
-        const long long t0 = clock64();
-        for (int spin = 0; pend; ++spin) {
-            unsigned long long w[kBatch];
-#pragma unroll
-            for (int q = 0; q < kBatch; ++q)
-                if (pend & (1u << q)) w[q] = ll_load(base + static_cast<size_t>(chunk + ct + q * kPollers) * stride);
-#pragma unroll
-            for (int q = 0; q < kBatch; ++q)
-                if ((pend & (1u << q)) && (w[q] >> shift) == tag) {
-                    sink(chunk + ct + q * kPollers, w[q]);
-                    pend &= ~(1u << q);
-                }
-            if (pend && ll_give_up(spin, t0, A)) break;
-        }
-    }
-}
 
 }  // namespace
 

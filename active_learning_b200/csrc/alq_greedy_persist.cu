@@ -78,7 +78,7 @@ struct PersistArgs {
     long long timeout_cycles;
 };
 
-// LL words (ll_store, ll_load, ll_wait, ll_gather): alq_greedy.cuh
+// LL words (ll_store, ll_load, ll_wait, ll_gather): alq_ll.cuh
 
 __device__ __forceinline__ void cons_bar() { asm volatile("bar.sync 1, %0;" ::"n"(kConsThreads) : "memory"); }
 __device__ __forceinline__ unsigned long long gtime_ns() {
@@ -534,12 +534,7 @@ greedy_persist_kernel(const __grid_constant__ PersistArgs A, const PipeCfg cfg, 
         }
     }
 
-    if (A.world > 1 && ct < A.world)          // peers may still be clearing their windows for this call
-        for (long long t0 = clock64();;) {
-            if (ld_acquire_sys(reinterpret_cast<const unsigned long long*>(win + A.ready_off) + ct) == A.ready_tag) break;
-            if (clock64() - t0 > A.timeout_cycles) { atomicCAS(A.status, 0, ALQ_ERR_STATE); break; }
-            __nanosleep(200);
-        }
+    if (A.world > 1 && ct < A.world) ll_ready_wait(win + A.ready_off, ct, A.ready_tag, A);   // peers may still be clearing theirs
     cons_bar();
 
     // per-warp position in the tile stream (global over all steps): tiles cw, cw + C, cw + 2C, ...
@@ -816,13 +811,6 @@ __global__ void persist_posinv_kernel(const int* __restrict__ vpos, const int* _
     int p = 0;
     while (p + 1 < P && row >= part_off[p + 1]) ++p;
     posinv[cfull_off[p] + vpos[row]] = row;
-}
-
-__global__ void persist_ready_kernel(PersistArgs A) {
-    if (blockIdx.x == 0 && threadIdx.x < A.world) {
-        __threadfence_system();
-        st_release_sys(reinterpret_cast<unsigned long long*>(A.peer[threadIdx.x] + A.ready_off) + A.rank, A.ready_tag);
-    }
 }
 
 template <bool FACTORED, bool SAMPLE>
@@ -1105,8 +1093,7 @@ int alq_greedy_persist(alq_ctx* ctx, const alq_greedy_desc* D, void* stream) {
     ctx->comm.epoch += 1;
     A.ready_tag = ctx->comm.epoch << 32;
     A.tag_base = static_cast<unsigned int>(ctx->comm.epoch & 0x7fu) << 24 | 0x80000000u;   // never 0: a zeroed word is invalid
-    const int clock_khz = ctx->clock_khz;
-    A.timeout_cycles = static_cast<long long>(ctx->spin_timeout_ms) * clock_khz;
+    A.timeout_cycles = ctx->spin_timeout_cycles();
     {   // L2 residency: keep `l2_resident_mb` of the rows this GPU streams in L2 across the steps (evict_last), split evenly over the CTAs
         const long long mb = ctx->l2_resident_mb;
         A.resident_rows = mb > 0 ? static_cast<int>(std::min<long long>((mb << 20) / static_cast<long long>(row_bytes) / std::max(grid, 1), 1 << 30)) : 0;
@@ -1114,19 +1101,17 @@ int alq_greedy_persist(alq_ctx* ctx, const alq_greedy_desc* D, void* stream) {
     A.fast_path = ctx->d2_fast_path;
 
     if (comm) {
-        persist_ready_kernel<<<1, 32, 0, st>>>(A);       // after the clears above, in stream order
-        ALQ_LAUNCH_CHECK(ctx);
+        rc = alq_comm_ready(ctx, A.ready_tag, st);       // after the clears above, in stream order
+        if (rc) return rc;
     }
-    alq_gridsync_begin(ctx, st);
-    cudaError_t le;
-    if (factored) le = sample ? launch_persist<true, true>(grid, smem, st, A, cfg, k_max, lc_max, ne_max, rm_max) : launch_persist<true, false>(grid, smem, st, A, cfg, k_max, lc_max, ne_max, rm_max);
-    else le = sample ? launch_persist<false, true>(grid, smem, st, A, cfg, k_max, lc_max, ne_max, rm_max) : launch_persist<false, false>(grid, smem, st, A, cfg, k_max, lc_max, ne_max, rm_max);
-    alq_gridsync_end(ctx, st);
+    const cudaError_t le = alq_gridsync_launch(ctx, st, [&] {
+        if (factored) return sample ? launch_persist<true, true>(grid, smem, st, A, cfg, k_max, lc_max, ne_max, rm_max) : launch_persist<true, false>(grid, smem, st, A, cfg, k_max, lc_max, ne_max, rm_max);
+        return sample ? launch_persist<false, true>(grid, smem, st, A, cfg, k_max, lc_max, ne_max, rm_max) : launch_persist<false, false>(grid, smem, st, A, cfg, k_max, lc_max, ne_max, rm_max);
+    });
     if (le != cudaSuccess) {
         cudaGetLastError();
         ALQ_FAIL(ctx, ALQ_ERR_CUDA, "alq_greedy_select: cooperative launch failed: %s (grid %d, %zu B shared)", cudaGetErrorString(le), grid, smem);
     }
-    ALQ_LAUNCH_CHECK(ctx);
 
     int status = 0;
     unsigned long long prof[8] = {};

@@ -22,13 +22,13 @@
 // K14 alq_probcover_select  the greedy coverage picks.  Two set-up launches mark every row in a labeled row's ball
 //              covered and count deg[x] = |{y in N(x) : y uncovered}|.  Then ONE ordinary launch, one CTA per SM
 //              (bracketed by alq_gridsync_begin/end, every wait bounded by "spin_timeout_ms"), runs every pick: each CTA
-//              reduces its row segment to (deg, lowest row) and the grid agrees over 8-byte LL words (ll_gather); the
+//              reduces its row segment to (deg, lowest row) and the grid agrees over 8-byte LL words (ll_agree_min); the
 //              ball of the pick is split over every thread of the grid, a newly covered y subtracts one from deg[x] of
 //              every x in N(y) (atomicSub), and a second round of LL words is the grid barrier before the next step.
 //              Work per query: O(B n / SMs + nnz).
 #include <math.h>
 
-#include "alq_greedy.cuh"
+#include "alq_ll.cuh"
 #include "alq_wgmma.cuh"
 
 namespace pc {
@@ -315,11 +315,6 @@ __global__ void __launch_bounds__(SCAN_THREADS) pc_ptr_scan_kernel(long long* __
 // ---- K14 --------------------------------------------------------------------------------------------------------------
 constexpr int SEL_THREADS = 512;                 // >= kPollers: every poller of ll_gather is a thread of the CTA
 constexpr int SEL_WARPS = SEL_THREADS / 32;
-constexpr int SEG_ROWS_MAX = 65534;              // the key word carries a 16-bit row offset (0xffff: no row)
-
-__host__ __device__ __forceinline__ int seg_lo(int n, int grid, int b) {
-    return static_cast<int>(static_cast<long long>(n) * b / grid);
-}
 
 // every row in a labeled row's ball is covered (one warp per row)
 __global__ void __launch_bounds__(256) pc_cover_kernel(const long long* __restrict__ row_ptr, const int* __restrict__ cols, int n,
@@ -346,7 +341,9 @@ struct SelArgs {
     int n, budget;
     int* deg;
     uint8_t* covered;
-    char* words;                 // [2 parities][grid] key words, then [2 parities][grid] barrier words
+    SegShard S;                  // world 1: off = {0, n}
+    LLWords W;                   // [2 parities][grid] key words at keyw = 0 of peer[0] (scratch)
+    char* barw;                  // [2 parities][grid] barrier words, behind the key words
     int* picks;
     int* steps;
     int* status;
@@ -358,50 +355,26 @@ __global__ void __launch_bounds__(SEL_THREADS, 1) pc_greedy_kernel(const __grid_
     __shared__ int s_pick;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int b = blockIdx.x, G = gridDim.x;
-    const int lo = seg_lo(A.n, G, b), hi = seg_lo(A.n, G, b + 1);
+    const int lo = gseg_lo(A.S, b), hi = gseg_lo(A.S, b + 1);
     int steps = 0;
     for (int t = 0; t < A.budget; ++t) {
-        const unsigned long long tag = 0x8000u | (static_cast<unsigned int>(t) & 0x7fffu);
-        // ---- this segment's (largest deg, lowest row): key = deg << 32 | ~row, the largest key wins
-        unsigned long long best = 0;
+        // ---- the grid agrees on (largest deg, lowest row): the smallest key (0xffffffff - deg) << 32 | row, deg > 0
+        unsigned long long best = ~0ull;
         for (int row = lo + tid; row < hi; row += SEL_THREADS) {
             const int dg = __ldcg(A.deg + row);
             if (dg > 0) {
-                const unsigned long long key = (static_cast<unsigned long long>(dg) << 32) | (0xffffffffu - static_cast<uint32_t>(row));
-                best = key > best ? key : best;
+                const unsigned long long key = (static_cast<unsigned long long>(0xffffffffu - static_cast<uint32_t>(dg)) << 32) | static_cast<uint32_t>(row);
+                best = key < best ? key : best;
             }
         }
-        best = warp_max_u64(best);
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const unsigned long long w = __shfl_xor_sync(0xffffffffu, best, o);
+            best = w < best ? w : best;
+        }
         if (lane == 0) s_key[warp] = best;
         __syncthreads();
-        char* keyw = A.words + static_cast<size_t>(t & 1) * G * 8;
-        if (tid == 0) {
-            unsigned long long m = s_key[0];
-            for (int w = 1; w < SEL_WARPS; ++w) m = s_key[w] > m ? s_key[w] : m;
-            const unsigned long long off = m ? static_cast<unsigned long long>((0xffffffffu - static_cast<uint32_t>(m)) - lo) : 0xffffull;
-            ll_store_raw(keyw + static_cast<size_t>(b) * 8, (tag << 48) | (off << 32) | (m >> 32));
-        }
-        // ---- the grid's agreement on the pick
-        unsigned long long mine = 0;
-        ll_gather(keyw, G, 8, tag, 48, A, tid, [&](int i, unsigned long long w) {
-            const unsigned int off = static_cast<unsigned int>(w >> 32) & 0xffffu;
-            const unsigned int dg = static_cast<unsigned int>(w);
-            if (off == 0xffffu || dg == 0) return;
-            const uint32_t row = static_cast<uint32_t>(seg_lo(A.n, G, i)) + off;
-            const unsigned long long key = (static_cast<unsigned long long>(dg) << 32) | (0xffffffffu - row);
-            mine = key > mine ? key : mine;
-        });
-        mine = warp_max_u64(mine);
-        __syncthreads();                                              // s_key is reused
-        if (lane == 0) s_key[warp] = mine;
-        __syncthreads();
-        if (tid == 0) {
-            unsigned long long m = s_key[0];
-            for (int w = 1; w < SEL_WARPS; ++w) m = s_key[w] > m ? s_key[w] : m;
-            s_pick = m ? static_cast<int>(0xffffffffu - static_cast<uint32_t>(m)) : -1;
-        }
-        __syncthreads();
-        const int pick = s_pick;
+        const int pick = ll_agree_min<SEL_WARPS>(A, s_key, &s_pick, static_cast<unsigned int>(t), lo, tid);
         if (pick < 0 || pick >= A.n) break;                           // max deg = 0: full coverage (or a failed wait)
         if (b == 0 && tid == 0) A.picks[t] = pick;
         steps = t + 1;
@@ -417,7 +390,8 @@ __global__ void __launch_bounds__(SEL_THREADS, 1) pc_greedy_kernel(const __grid_
         }
         // ---- grid barrier: every deg and covered update of this step is visible before the next arg-max
         __syncthreads();
-        char* barw = A.words + static_cast<size_t>(2 + (t & 1)) * G * 8;
+        const unsigned long long tag = ll_key_tag(A.W, static_cast<unsigned int>(t));
+        char* barw = A.barw + static_cast<size_t>(t & 1) * G * 8;
         if (tid == 0) {
             __threadfence();
             ll_store_raw(barw + static_cast<size_t>(b) * 8, tag << 48);
@@ -510,9 +484,9 @@ extern "C" int alq_probcover_select(alq_ctx* ctx, const int64_t* row_ptr, const 
     const cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int ni = static_cast<int>(n);
     const int grid = std::max(1, std::min(ctx->sm_count, (ni + 255) / 256));
-    if ((ni + grid - 1) / grid > SEG_ROWS_MAX)
+    if ((ni + grid - 1) / grid > kSegRowsMax)
         ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_probcover_select: n=%d rows over %d CTAs exceed %d rows per CTA segment", ni, grid,
-                 SEG_ROWS_MAX);
+                 kSegRowsMax);
     int rc = alq_scratch_reserve(ctx, scratch_need({static_cast<size_t>(n) * 4, static_cast<size_t>(n),
                                                     static_cast<size_t>(4) * grid * 8, 16}));
     if (rc) return rc;
@@ -531,15 +505,19 @@ extern "C" int alq_probcover_select(alq_ctx* ctx, const int64_t* row_ptr, const 
     ALQ_LAUNCH_CHECK(ctx);
     SelArgs A{};
     A.row_ptr = rp; A.cols = cols; A.n = ni; A.budget = static_cast<int>(budget);
-    A.deg = deg; A.covered = covered; A.words = words;
+    A.deg = deg; A.covered = covered;
+    A.S.world = 1; A.S.rank = 0; A.S.grid = grid;
+    A.S.off[0] = 0; A.S.off[1] = ni;
+    A.W.peer[0] = words;
+    A.W.tag_base = 0x80000000u;
+    A.barw = words + static_cast<size_t>(2) * grid * 8;
     A.picks = picks; A.steps = small + 1; A.status = small;
-    A.timeout_cycles = static_cast<long long>(ctx->spin_timeout_ms) * ctx->clock_khz;
+    A.timeout_cycles = ctx->spin_timeout_cycles();
     // every CTA spins on the others' words, so all of them must be resident: grid <= SMs, one CTA per SM
-    alq_gridsync_begin(ctx, st);
-    pc_greedy_kernel<<<grid, SEL_THREADS, 0, st>>>(A);
-    const cudaError_t le = cudaGetLastError();
-    alq_gridsync_end(ctx, st);
-    ctx->launches++;
+    const cudaError_t le = alq_gridsync_launch(ctx, st, [&] {
+        pc_greedy_kernel<<<grid, SEL_THREADS, 0, st>>>(A);
+        return cudaGetLastError();
+    });
     if (le != cudaSuccess) ALQ_FAIL(ctx, ALQ_ERR_CUDA, "alq_probcover_select: launch failed: %s", cudaGetErrorString(le));
     int small_h[2] = {0, 0};
     ALQ_CUDA(ctx, cudaMemcpyAsync(small_h, small, sizeof(small_h), cudaMemcpyDeviceToHost, st));

@@ -7,7 +7,7 @@
 #include <initializer_list>
 #include <stdlib.h>
 
-#include "alq_common.cuh"
+#include "alq_ll.cuh"
 #include "alq_mase_rows.cuh"
 
 namespace {
@@ -548,10 +548,6 @@ __device__ __noinline__ void select_epilogue(const SelArgs& S, uint32_t* s_hist,
     sel_stamp(S.g_ctr, 2);
 }
 
-__device__ __forceinline__ void sel_ll_store(void* p, unsigned int tag, unsigned int payload) {
-    const unsigned long long v = (static_cast<unsigned long long>(tag) << 32) | payload;
-    asm volatile("st.relaxed.sys.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
-}
 // Bounded spin.  The sticky failure flag that lets every other wait of this launch return at once lives in DEVICE
 // memory (g_ctr[12]); the host-visible status word is mapped host memory and is only WRITTEN, once, on a timeout --
 // polling it from thousands of spinning threads is a PCIe read storm that delays the very launches being waited for
@@ -600,8 +596,8 @@ __device__ __noinline__ void select_epilogue_mgpu(const SelArgs& S, uint32_t* s_
         // this CTA's slice of the rank histogram -> every rank; then the same slice summed over the ranks
         for (int i = tid; i < (b_hi - b_lo) * W; i += nthr) {
             const int bin = b_lo + i / W, p = i % W;
-            sel_ll_store(S.peer[p] + S.hist_off + (static_cast<size_t>(level * W + S.rank) * 2048 + bin) * 8, S.tag,
-                         __ldcg(S.g_hist + level * 2048 + bin));
+            ll_store(S.peer[p] + S.hist_off + (static_cast<size_t>(level * W + S.rank) * 2048 + bin) * 8, S.tag,
+                     __ldcg(S.g_hist + level * 2048 + bin));
         }
         uint32_t* s_sum = reinterpret_cast<uint32_t*>(s_misc + 16);           // [per <= 32] (find_bin's scratch, free here)
         if (tid < 32) s_sum[tid] = 0;
@@ -637,7 +633,7 @@ __device__ __noinline__ void select_epilogue_mgpu(const SelArgs& S, uint32_t* s_
     if (tid == 0) {
         __threadfence_system();               // the candidate words are visible in every window before the count is
         for (int p = 0; p < W; ++p)
-            sel_ll_store(S.peer[p] + S.cnt_off + (static_cast<size_t>(S.rank) * S.stride + blockIdx.x) * 8, S.tag, static_cast<unsigned int>(nc));
+            ll_store(S.peer[p] + S.cnt_off + (static_cast<size_t>(S.rank) * S.stride + blockIdx.x) * 8, S.tag, static_cast<unsigned int>(nc));
     }
     // ---- counts of every CTA of every rank -> per-rank totals ----
     uint32_t* s_tot = reinterpret_cast<uint32_t*>(s_misc + 24);      // [8]
@@ -1152,12 +1148,11 @@ cudaError_t launch_rows_pipe(alq_ctx* ctx, cudaStream_t st, const RowPipeCfg& cf
         // share the device at the same time: they are chained through one event per device (other kernels merely delay the
         // moment the last CTA becomes resident; they never wait for ours).
         if (grid > ctx->sm_count) return cudaErrorInvalidConfiguration;
-        alq_gridsync_begin(ctx, st);
-        rows_pipe_kernel<NV, MODE><<<grid, 32 * (1 + cfg.consumers), smem, st>>>(logits, n, c, cfg, scores, bs, row0, n_total, a, lda,
-                                                                              counter, mase, sel);
-        const cudaError_t le = cudaGetLastError();
-        alq_gridsync_end(ctx, st);
-        return le;
+        return alq_gridsync_launch(ctx, st, [&] {
+            rows_pipe_kernel<NV, MODE><<<grid, 32 * (1 + cfg.consumers), smem, st>>>(logits, n, c, cfg, scores, bs, row0, n_total,
+                                                                                  a, lda, counter, mase, sel);
+            return cudaGetLastError();
+        });
     }
     rows_pipe_kernel<NV, MODE><<<grid, 32 * (1 + cfg.consumers), smem, st>>>(logits, n, c, cfg, scores, bs, row0, n_total, a, lda,
                                                                           counter, mase, sel);
@@ -1357,14 +1352,13 @@ static int uncertainty_tail_impl(alq_ctx* ctx, const float* logits, int64_t n, i
         sel.cnt_off = base + hist_bytes;
         sel.cand_off = sel.cnt_off + cnt_bytes;
         sel.tag = 0x80000000u | static_cast<unsigned int>(G.epoch & 0x7fffffffu);
-        sel.timeout_cycles = static_cast<long long>(ctx->spin_timeout_ms) * ctx->clock_khz;
+        sel.timeout_cycles = ctx->spin_timeout_cycles();
         sel.status = ctx->xchg_status_dev;
     }
     cudaError_t e;
     if (mode == ALQ_MODE_MARGIN) e = launch_rows_pipe_nv<ALQ_MODE_MARGIN>(ctx, st, cfg, smem, logits, n, c, scores, 1, 0, n, nullptr, 0, MaseArgs{}, sel);
     else if (mode == ALQ_MODE_LEAST_CONFIDENCE) e = launch_rows_pipe_nv<ALQ_MODE_LEAST_CONFIDENCE>(ctx, st, cfg, smem, logits, n, c, scores, 1, 0, n, nullptr, 0, MaseArgs{}, sel);
     else e = launch_rows_pipe_nv<ALQ_MODE_ENTROPY>(ctx, st, cfg, smem, logits, n, c, scores, 1, 0, n, nullptr, 0, MaseArgs{}, sel);
-    ctx->launches++;
     if (e != cudaSuccess) {
         cudaGetLastError();
         ALQ_FAIL(ctx, ALQ_ERR_CUDA, "alq_uncertainty_tail: cooperative launch failed: %s", cudaGetErrorString(e));

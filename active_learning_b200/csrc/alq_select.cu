@@ -594,8 +594,7 @@ extern "C" int alq_topb_exchange(alq_ctx* ctx, const float* scores, const int32_
     X.flags_off = base + static_cast<size_t>(G.world) * AlqComm::kTopbWords * 8;
     X.tag = G.epoch << 32;
     X.ticket = ticket; X.status = status;
-    const int clock_khz = ctx->clock_khz;
-    X.timeout_cycles = static_cast<long long>(ctx->spin_timeout_ms) * clock_khz;
+    X.timeout_cycles = ctx->spin_timeout_cycles();
     const int blocks = static_cast<int>((b + 255) / 256);
     topb_push_kernel<<<blocks, 256, 0, st>>>(scores, pos, k, row_lo, b, X);
     ALQ_LAUNCH_CHECK(ctx);

@@ -514,7 +514,8 @@ int alq_balancing_table_select(alq_ctx* ctx, const alq_balancing_desc* desc, voi
  *   of a row with labeled[row] != 0 and deg[x] = |{y in N(x) : y uncovered}|; each step stops if max deg = 0, else picks
  *   c = the lowest row of the maximum and covers every uncovered y in N(c).  picks[0 .. *n_steps_host) (int32, device) in
  *   pick order, *n_steps_host <= budget <= n.  Set-up: two launches; then ONE launch runs every step (one CTA per SM,
- *   agreement over 8-byte LL words, every wait bounded by "spin_timeout_ms").  n / SMs <= 65 534.  Synchronous. */
+ *   agreement over 8-byte LL words, every wait bounded by "spin_timeout_ms"); at most 65 535 rows per CTA segment.
+ *   Synchronous. */
 int alq_probcover_graph(alq_ctx* ctx, const float* x, int64_t n, int32_t d, int64_t ldx, const double* delta_host,
                         float* xhat, int32_t* tile_cnt, int64_t* row_ptr, int32_t* cols, int64_t* nnz_host,
                         int64_t* recheck_host, void* stream);
