@@ -8,13 +8,20 @@ written from the algorithm of Yehuda et al., "Active Learning Through a Covering
   greedy     covered = the balls of the labeled rows; deg[x] = uncovered rows in N(x); each step stops if max deg = 0,
              else takes the lowest position c of the maximum and covers N(c);
   fill       the rest of the budget is np.random.choice(available-and-unpicked positions ascending, rest, replace=False).
+
+The tensor-core screen's pieces (DESIGN section 4) follow: its bound E, its band decision in the epilogue's fp64
+order, emulations of the 3xTF32 chain under three adder models, and rows that stress E.
 """
+import math
+
 import numpy as np
 
 LANES = 32
 
 
-def normalize(x):
+def lane_sum_sq(x):
+    """K13's fp64 sum of squares of each fp32 row: lane l of 32 adds the squares of columns l, l + 32, .. in order, then a
+    butterfly (xor 16, 8, 4, 2, 1) adds the 32 partials."""
     x = np.asarray(x, dtype=np.float32)
     n, d = x.shape
     dp = -(-max(d, 1) // LANES) * LANES
@@ -27,7 +34,18 @@ def normalize(x):
     lanes = np.arange(LANES)
     for o in (16, 8, 4, 2, 1):
         s = s + s[:, lanes ^ o]
-    norm = np.sqrt(s[:, 0])
+    return s[:, 0]
+
+
+def nrm2(xhat):
+    """K13's nrm2_i = |xhat_i|^2 in fp64, the order of lane_sum_sq."""
+    return lane_sum_sq(xhat)
+
+
+def normalize(x):
+    x = np.asarray(x, dtype=np.float32)
+    n, d = x.shape
+    norm = np.sqrt(lane_sum_sq(x))
     out = np.zeros((n, d), dtype=np.float32)
     nz = norm > 0
     out[nz] = (x[nz].astype(np.float64) / norm[nz, None]).astype(np.float32)
@@ -148,25 +166,95 @@ def tf32_rna(v):
     return ((b + np.uint32(0x1000)) & np.uint32(0xFFFFE000)).view(np.float32)
 
 
-def emulate_3xtf32(a, b, truncate=False):
+EDGE, NONE, RECHECK = 1, 0, 2
+
+
+def screen_decide(d, ni, nj, g, delta):
+    """The epilogue's decision for fp32 dot products g of rows with nrm2 ni, nj at width d (K13's padded width), in fp64
+    and in the kernel's operation order: EDGE, NONE, or RECHECK (inside the band: the exact recomputation decides)."""
+    coef = 2.0 * screen_bound(d, 1.0, 1.0) * (1.0 + 1e-6)
+    delta2 = float(delta) * float(delta)
+    slack = 1e-9 * delta2 + 1e-10
+    ni, nj = np.asarray(ni, dtype=np.float64), np.asarray(nj, dtype=np.float64)
+    d2 = (ni + nj) - 2.0 * np.asarray(g, dtype=np.float32).astype(np.float64)
+    bnd = coef * np.sqrt(ni * nj) + slack
+    return np.where(d2 < delta2 - bnd, EDGE, np.where(d2 > delta2 + bnd, NONE, RECHECK))
+
+
+def _to_f32_toward_zero(v):
+    f = v.astype(np.float32)
+    over = np.abs(f.astype(np.float64)) > np.abs(v)
+    return np.where(over, np.nextafter(f, np.float32(0)), f)
+
+
+def emulate_3xtf32(a, b, adder="nearest", bits=24):
     """g for row pairs (a[p], b[p]) as the wgmma chain forms it: hi = rna(x), lo = rna(x - hi); per k-block of 8 three
-    MMAs (hi hi', hi lo', lo hi') each adding its 8 exact products to the fp32 accumulator with one rounding (to nearest,
-    or toward zero with truncate=True)."""
+    MMAs (hi hi', hi lo', lo hi'), each adding its 8 exact products to the fp32 accumulator.  The adder of one MMA:
+      "nearest"  the exact sum rounded once to nearest;
+      "zero"     the exact sum rounded once toward zero;
+      "align"    the accumulator and the 8 products aligned to the largest exponent among them, each truncated to `bits`
+                 bits below and including that exponent's leading bit, summed exactly, the sum truncated to fp32."""
     a, b = np.asarray(a, dtype=np.float32), np.asarray(b, dtype=np.float32)
     ah, bh = tf32_rna(a), tf32_rna(b)
     al, bl = tf32_rna(a - ah), tf32_rna(b - bh)
     d = a.shape[1]
     acc = np.zeros(a.shape[0], dtype=np.float32)
-
-    def rnd(v):
-        f = v.astype(np.float32)
-        if truncate:
-            over = np.abs(f.astype(np.float64)) > np.abs(v)
-            f = np.where(over, np.nextafter(f, np.float32(0)), f)
-        return f
-
     for k0 in range(0, d, 8):
         sl = slice(k0, min(d, k0 + 8))
         for x, y in ((ah, bh), (ah, bl), (al, bh)):
-            acc = rnd(acc.astype(np.float64) + (x[:, sl].astype(np.float64) * y[:, sl].astype(np.float64)).sum(axis=1))
+            prods = x[:, sl].astype(np.float64) * y[:, sl].astype(np.float64)
+            if adder == "align":
+                terms = np.concatenate([acc.astype(np.float64)[:, None], prods], axis=1)
+                _, ex = np.frexp(np.max(np.abs(terms), axis=1))        # largest |term| in [2^(ex - 1), 2^ex)
+                q = np.ldexp(1.0, ex - bits)[:, None]
+                acc = _to_f32_toward_zero((np.trunc(terms / q) * q).sum(axis=1))    # exact: < 2^53 units of q
+            else:
+                s = acc.astype(np.float64) + prods.sum(axis=1)
+                acc = s.astype(np.float32) if adder == "nearest" else _to_f32_toward_zero(s)
     return acc
+
+
+# ---- rows that stress the bound -------------------------------------------------------------------------------------
+def _low_bits(x, pattern):
+    """x with the low 13 mantissa bits (those TF32 drops) set to `pattern`."""
+    u = np.asarray(x, dtype=np.float32).view(np.uint32)
+    return ((u & np.uint32(0xFFFFE000)) | np.uint32(pattern)).view(np.float32)
+
+
+def bound_families(rng, d, instances=3):
+    """{family: [m, d] float32 rows} of near-unit rows (normalize'd) at which the 3xTF32 chain's error is largest relative
+    to E.  The TF32 bit patterns are imposed after normalisation, which moves |x|^2 by at most 2^-10."""
+    k = np.arange(d)
+    u = lambda: rng.random(d)                                              # noqa: E731
+    sign = lambda: rng.choice([-1.0, 1.0], d)                              # noqa: E731
+    raw = {
+        "equal": [np.ones(d), -np.ones(d)],
+        "full_mantissa": [1.0 + u() for _ in range(instances)],            # same sign: the accumulator dwarfs a product
+        "midpoint": [1.0 + u() for _ in range(instances)],
+        "below_midpoint": [(1.0 + u()) * sign() for _ in range(instances)],
+        "spike_first": [], "spike_last": [],
+        "alternating": [(-1.0) ** (k >> s) * (1.0 + 1e-3 * u()) for s in range(instances)],   # Walsh signs: S >> |g|
+        "ramp": [2.0 ** (-4.0 * ((k + s) % 8) - 3.0 * k / max(d - 1, 1)) * (1.0 + u()) * sign() for s in range(instances)],
+        "normal": [rng.normal(size=d) for _ in range(instances)],
+        "abs_normal": [np.abs(rng.normal(size=d)) for _ in range(instances)],
+    }
+    for _ in range(instances):
+        tiny = 1e-4 * (1.0 + u()) * sign()
+        first, last = tiny.copy(), tiny.copy()
+        first[0], last[-1] = 1.0, -1.0
+        raw["spike_first"].append(first)
+        raw["spike_last"].append(last)
+    fam = {name: normalize(np.stack(rows).astype(np.float32)) for name, rows in raw.items()}
+    fam["midpoint"] = _low_bits(fam["midpoint"], 0x1000)                  # on a midpoint: |lo| = half a TF32 ulp ...
+    fam["below_midpoint"] = _low_bits(fam["below_midpoint"], 0x0FFF)      # ... just below: lo, and lo lo', at their largest
+    base = np.concatenate(list(fam.values()))
+    noise = (rng.normal(size=base.shape) * 1e-4).astype(np.float32)
+    fam["near_duplicate"] = normalize(base + noise * np.abs(base).max(axis=1, keepdims=True))   # d^2 next to 0
+    fam["antipode"] = -base
+    return fam
+
+
+def exact_dots(a, b):
+    """<a_p, b_p> of fp32 rows correctly rounded to fp64: the products are exact in fp64, math.fsum adds them exactly."""
+    a, b = np.asarray(a, dtype=np.float32).astype(np.float64), np.asarray(b, dtype=np.float32).astype(np.float64)
+    return np.array([math.fsum(p) for p in a * b])

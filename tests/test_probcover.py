@@ -76,17 +76,50 @@ def test_screen_bound_holds_against_fp64_truth_on_adversarial_rows(d):
     nrm = (x64 * x64).sum(axis=1)
     truth = (x64[i] * x64[j]).sum(axis=1)
     bound = P.screen_bound(d, nrm[i], nrm[j])
-    for truncate in (False, True):
-        g = P.emulate_3xtf32(xh[i], xh[j], truncate=truncate).astype(np.float64)
-        assert (np.abs(g - truth) <= bound).all(), np.max(np.abs(g - truth) / bound)
+    for adder in ("nearest", "zero", "align"):
+        g = P.emulate_3xtf32(xh[i], xh[j], adder=adder).astype(np.float64)
+        assert (np.abs(g - truth) <= bound).all(), (adder, np.max(np.abs(g - truth) / bound))
         # every certified decision is the exact one, for radii placed on the pairs' own distances
-        d2 = nrm[i] + nrm[j] - 2 * g
         exact = P.exact_d2(xh[i], xh[j])
+        n2 = P.nrm2(xh)
         for delta in np.sqrt(np.clip(exact[::7], 1e-12, None)).tolist() + [0.5, 1.0, 1.9]:
-            bnd = 2 * bound * (1 + 1e-6) + 1e-9 * delta * delta + 1e-10
-            inside, outside = d2 < delta * delta - bnd, d2 > delta * delta + bnd
+            dec = P.screen_decide(d, n2[i], n2[j], g, delta)
             truth_edge = np.sqrt(exact) < delta
-            assert truth_edge[inside].all() and not truth_edge[outside].any()
+            assert truth_edge[dec == P.EDGE].all() and not truth_edge[dec == P.NONE].any()
+
+
+@pytest.mark.parametrize("d", [4, 28, 36, 64, 520, 2048])
+def test_screen_bound_holds_on_the_bound_families_under_every_adder_model(d):
+    """The rows the H100 probe (test_gpu_tf32_bound.py) measures, every pair within and across families, under the
+    three adder models; the align-and-truncate adder keeps 24 bits.  An align adder of 21 bits breaks E on these rows
+    from d = 28 on, so they are adversarial enough to tell the two apart."""
+    fam = P.bound_families(np.random.default_rng(100 + d), d)
+    xh = np.concatenate(list(fam.values()))
+    i, j = np.triu_indices(len(xh))
+    truth = P.exact_dots(xh[i], xh[j])
+    nrm = P.nrm2(xh)
+    bound = P.screen_bound(d, nrm[i], nrm[j])
+
+    def worst(adder, bits=24):
+        return np.max(np.abs(P.emulate_3xtf32(xh[i], xh[j], adder=adder, bits=bits).astype(np.float64) - truth) / bound)
+
+    for adder in ("nearest", "zero", "align"):
+        assert worst(adder) <= 1.0, (adder, d, worst(adder))
+    if d >= 28:
+        assert worst("align", bits=21) > 1.0
+
+
+def test_the_adder_models_are_exact_on_tf32_integers_and_differ_elsewhere():
+    rng = np.random.default_rng(4)
+    a = rng.integers(-8, 9, size=(64, 520)).astype(np.float32)
+    b = rng.integers(-8, 9, size=(64, 520)).astype(np.float32)
+    want = (a.astype(np.float64) * b).sum(axis=1)
+    for adder in ("nearest", "zero", "align"):
+        assert (P.emulate_3xtf32(a, b, adder=adder).astype(np.float64) == want).all()
+    fam = P.bound_families(np.random.default_rng(5), 2048)["full_mantissa"]
+    g = {ad: P.emulate_3xtf32(fam, fam[::-1], adder=ad) for ad in ("nearest", "zero", "align")}
+    assert (g["align"] != g["nearest"]).any() and (g["align"] != g["zero"]).any()
+    assert (P.emulate_3xtf32(fam, fam[::-1], adder="align", bits=21) != g["align"]).any()
 
 
 # ---- the sampler's host logic ------------------------------------------------------------------------------------------
