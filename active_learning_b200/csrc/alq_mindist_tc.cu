@@ -9,14 +9,11 @@
 // The dropped lo*lo' and r terms are <= 2^-21 |x||y| per product.  Small integers (the exact-arithmetic
 // parity fixtures) have lo == 0 and give bit-identical results to fp32.
 //
-// Structure (one CTA per SM, persistent over a host-built work list, 3 warpgroups):
-//   warpgroup 0   TMA producer (one thread): 4 tensor maps (X_hi, X_lo, Y_hi, Y_lo), boxes of 32 fp32
-//                 (=128 B, SWIZZLE_128B) x 128 rows into a 3-stage shared-memory ring, mbarrier complete_tx.
-//   warpgroups 1-2 consumers: each owns 64 of the tile's 128 rows and issues
-//                 wgmma.mma_async.m64n128k8.f32.tf32.tf32 from shared memory (12 per stage, one stage kept
-//                 in flight), then the distance + running row min on its register accumulators; one float
-//                 atomic per row at the end of a work item.  The factored/BADGE form keeps two accumulators
-//                 (<h,h'> and <a,a'>) and multiplies them in the epilogue.
+// Structure: the ring of alq_wgmma.cuh (one CTA per SM, a TMA producer warpgroup, two consumer warpgroups issuing
+// tc::ring_mma), persistent over a host-built work list of (row block, column-tile range).  The producer loads
+// 4 tensor maps (X_hi, X_lo, Y_hi, Y_lo); the consumers compute the distance + running row min on their register
+// accumulators and issue one float atomic per row at the end of a work item.  The factored/BADGE form keeps two
+// accumulators (<h,h'> and <a,a'>) in the same ring, k-blocks of h first, and multiplies them in the epilogue.
 // Every CTA sweeps the column tiles in the same order, so a Y tile is fetched from HBM once and
 // served to the other CTAs from L2.
 #include <stdlib.h>
@@ -24,14 +21,6 @@
 #include "alq_wgmma.cuh"
 
 namespace tc {
-
-constexpr int BM = 128;          // rows per tile (two m64 warpgroups)
-constexpr int BN = 128;          // cols per tile (wgmma N)
-constexpr int STAGES = 3;
-constexpr int A_BYTES = BM * BK * 4;              // 16 KB
-constexpr int B_BYTES = BN * BK * 4;              // 16 KB
-constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;   // hi + lo of both operands = 64 KB
-constexpr int THREADS = 384;
 
 struct WorkItem {
     int m_blk, n_begin, n_end, pad;   // row block, [first, last) column tile
@@ -55,102 +44,55 @@ min_dist_tc_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_cons
                    const __grid_constant__ CUtensorMap map_yah, const __grid_constant__ CUtensorMap map_yal,
                    Params P) {
     extern __shared__ unsigned char smem_dyn[];
-    // SWIZZLE_128B tiles must sit on 1024-byte boundaries: align by hand (1 KB of slack is allocated)
-    unsigned char* smem_raw = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
-    unsigned char* stage_base = smem_raw;
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem_raw + STAGES * STAGE_BYTES);
-    uint64_t* empty = full + STAGES;
-
-    const int wg = threadIdx.x >> 7;
+    const Role me = ring_role();
     const int n_items = P.item_count[blockIdx.x];
     const WorkItem* items = P.items + static_cast<size_t>(blockIdx.x) * P.items_per_cta;
     const int kb_total = P.kblocks_h + (FACTORED ? P.kblocks_a : 0);
+    const Ring ring = ring_init(smem_dyn);
 
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-
-    if (wg == 0) {
-        // ================= TMA producer =================
-        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (me.wg == 0) {
+        producer_regs();
         if (threadIdx.x == 0) {
             uint32_t it = 0;
             for (int w = 0; w < n_items; ++w) {
                 const WorkItem wi = items[w];
                 for (int nt = wi.n_begin; nt < wi.n_end; ++nt) {
                     for (int kb = 0; kb < kb_total; ++kb, ++it) {
-                        const int s = it % STAGES;
-                        const uint32_t round = it / STAGES;
-                        if (round > 0) mbar_wait(&empty[s], (round - 1) & 1u);
-                        unsigned char* st = stage_base + static_cast<size_t>(s) * STAGE_BYTES;
-                        mbar_expect_tx(&full[s], STAGE_BYTES);
                         const bool apart = FACTORED && kb >= P.kblocks_h;
-                        const int k0 = (apart ? kb - P.kblocks_h : kb) * BK;
-                        tma_load_2d(st, apart ? &map_xah : &map_xh, k0, wi.m_blk * BM, &full[s]);
-                        tma_load_2d(st + A_BYTES, apart ? &map_xal : &map_xl, k0, wi.m_blk * BM, &full[s]);
-                        tma_load_2d(st + 2 * A_BYTES, apart ? &map_yah : &map_yh, k0, nt * BN, &full[s]);
-                        tma_load_2d(st + 2 * A_BYTES + B_BYTES, apart ? &map_yal : &map_yl, k0, nt * BN, &full[s]);
+                        ring_load(ring, it, apart ? &map_xah : &map_xh, apart ? &map_xal : &map_xl, wi.m_blk * BM,
+                                  apart ? &map_yah : &map_yh, apart ? &map_yal : &map_yl, nt * BN,
+                                  (apart ? kb - P.kblocks_h : kb) * BK);
                     }
                 }
             }
         }
     } else {
-        // ================= consumers: warpgroup wg - 1 owns rows [64 (wg - 1), 64 wg) of the tile =================
-        asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
-        const int t = threadIdx.x & 127, warp = t >> 5, lane = t & 31;
-        const uint32_t a_off = static_cast<uint32_t>(wg - 1) * 64 * BK * 4;     // 8 KB: a whole number of swizzle atoms
-        // m64nN fp32 fragment: d[4j + {0,1}] = (r, 8j + 2 (lane % 4) + {0,1}), d[4j + {2,3}] = (r + 8, same cols),
-        // r = 16 warp + lane / 4
-        const int r_in_tile = (wg - 1) * 64 + warp * 16 + (lane >> 2);
-        const int c_in_tile = 2 * (lane & 3);
+        consumer_regs();
         uint32_t it = 0;
         for (int w = 0; w < n_items; ++w) {
             const WorkItem wi = items[w];
-            const int row0 = wi.m_blk * BM + r_in_tile, row1 = row0 + 8;
+            const int row0 = wi.m_blk * BM + me.r_in_tile, row1 = row0 + 8;
             const float rn0 = row0 < P.n ? P.xn[row0] : 0.f, rn1 = row1 < P.n ? P.xn[row1] : 0.f;
             float best0 = RED_MAX ? ALQ_NEG_INF : ALQ_POS_INF, best1 = best0;
             for (int nt = wi.n_begin; nt < wi.n_end; ++nt) {
                 float acc[64];
                 float acc_a[FACTORED ? 64 : 1];
                 int prev = -1;
+                // one pipeline for both contractions: a k-block of the a-part goes into acc_a, and the stage hand-back
+                // runs across the boundary
                 for (int kb = 0; kb < kb_total; ++kb, ++it) {
-                    const int s = it % STAGES;
-                    mbar_wait(&full[s], (it / STAGES) & 1u);
-                    const bool apart = FACTORED && kb >= P.kblocks_h;
-                    const bool first_kb = apart ? (kb == P.kblocks_h) : (kb == 0);
-                    const uint32_t a_hi = smem_u32(stage_base + static_cast<size_t>(s) * STAGE_BYTES) + a_off;
-                    const uint32_t a_lo = a_hi + A_BYTES, b_hi = a_hi - a_off + 2 * A_BYTES, b_lo = b_hi + B_BYTES;
-                    wgmma_fence();
-#pragma unroll
-                    for (int k = 0; k < BK / UK; ++k) {
-                        const uint32_t off = k * UK * 4;    // bytes along K inside the 128-byte swizzle span
-                        const uint64_t dah = make_desc(a_hi + off), dal = make_desc(a_lo + off);
-                        const uint64_t dbh = make_desc(b_hi + off), dbl = make_desc(b_lo + off);
-                        const uint32_t sc = (first_kb && k == 0) ? 0u : 1u;
-                        if constexpr (FACTORED) {
-                            if (apart) {
-                                wgmma_tf32(acc_a, dah, dbh, sc);
-                                wgmma_tf32(acc_a, dah, dbl, 1u);
-                                wgmma_tf32(acc_a, dal, dbh, 1u);
-                                continue;
-                            }
+                    if constexpr (FACTORED) {
+                        if (kb >= P.kblocks_h) {
+                            ring_mma(ring, it, me.a_off, acc_a, kb == P.kblocks_h, prev, me.t);
+                            continue;
                         }
-                        wgmma_tf32(acc, dah, dbh, sc);
-                        wgmma_tf32(acc, dah, dbl, 1u);
-                        wgmma_tf32(acc, dal, dbh, 1u);
                     }
-                    wgmma_commit();
-                    wgmma_wait<1>();                          // the previous stage's MMAs have retired: hand it back
-                    if (prev >= 0 && t == 0) mbar_arrive(&empty[prev]);
-                    prev = s;
+                    ring_mma(ring, it, me.a_off, acc, kb == 0, prev, me.t);
                 }
-                wgmma_wait<0>();
-                if (prev >= 0 && t == 0) mbar_arrive(&empty[prev]);
+                ring_drain(ring, prev, me.t);
 #pragma unroll
                 for (int j = 0; j < 16; ++j) {
-                    const int col = nt * BN + 8 * j + c_in_tile;
+                    const int col = nt * BN + 8 * j + me.c_in_tile;
                     const float pad = RED_MAX ? ALQ_NEG_INF : ALQ_POS_INF;
                     const float cn0 = col < P.m ? __ldg(P.yn + col) : pad;
                     const float cn1 = col + 1 < P.m ? __ldg(P.yn + col + 1) : pad;
@@ -172,7 +114,7 @@ min_dist_tc_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_cons
                 best0 = RED_MAX ? fmaxf(best0, b0) : fminf(best0, b0);
                 best1 = RED_MAX ? fmaxf(best1, b1) : fminf(best1, b1);
             }
-            if ((lane & 3) == 0 && wi.n_end > wi.n_begin) {
+            if ((me.lane & 3) == 0 && wi.n_end > wi.n_begin) {
                 if (row0 < P.n) { if (RED_MAX) atomic_max_float(P.out + row0, best0); else atomic_min_float(P.out + row0, best0); }
                 if (row1 < P.n) { if (RED_MAX) atomic_max_float(P.out + row1, best1); else atomic_min_float(P.out + row1, best1); }
             }
@@ -305,7 +247,7 @@ int alq_min_dist_tc(alq_ctx* ctx, const float* x, int64_t ldx, const float* xn, 
     P.xn = xn_use; P.yn = yn_use; P.out = out; P.items = d_items; P.item_count = d_counts; P.items_per_cta = items_per_cta;
     P.n = static_cast<int>(n); P.m = static_cast<int>(m);
     P.kblocks_h = (d + BK - 1) / BK; P.kblocks_a = factored ? (c + BK - 1) / BK : 0;
-    const size_t smem = static_cast<size_t>(STAGES) * STAGE_BYTES + 256 + 1024;
+    const size_t smem = ring_smem_bytes(0);
     auto launch = [&](auto kern) -> cudaError_t {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
         if (e != cudaSuccess) return e;

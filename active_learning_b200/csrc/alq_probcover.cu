@@ -5,9 +5,10 @@
 //   normalise  one warp per row: lane-strided fp64 sum of squares, a butterfly, norm = sqrt, xhat = fl32(x / norm)
 //              (a zero row stays zero); the same kernel splits xhat into TF32 hi / lo (alq_wgmma.cuh) and stores
 //              nrm2 = |xhat|^2 in fp64.
-//   screen     one CTA per SM, persistent over the upper-triangle 128 x 128 tiles of xhat xhat^T, K3's layout:
-//              warpgroup 0 is the TMA producer (3-stage ring), warpgroups 1-2 issue the 3xTF32 wgmma chain.  The epilogue
-//              decides each pair from d2 = nrm2_i + nrm2_j - 2 g (g the tensor-core dot product) against the bound
+//   screen     one CTA per SM, persistent over the upper-triangle 128 x 128 tiles of xhat xhat^T, on the ring of
+//              alq_wgmma.cuh that K3 and K9 use: warpgroup 0 is the TMA producer (3-stage ring), warpgroups 1-2 issue
+//              the 3xTF32 chain tc::ring_mma.  The epilogue decides each pair from d2 = nrm2_i + nrm2_j - 2 g
+//              (g the tensor-core dot product) against the bound
 //              |g - <xhat_i, xhat_j>| <= E_ij of DESIGN section 4: clearly inside delta^2 is an edge, clearly outside is
 //              not, and a pair inside the band is recomputed exactly with K7's arithmetic.  A pair is decided once per
 //              tile, so (i, j) and (j, i) of an off-diagonal tile share one decision; on a diagonal tile both orders are
@@ -34,13 +35,9 @@
 namespace pc {
 
 using tc::BK;
-using tc::UK;
-constexpr int BM = 128;                       // rows and columns of a tile (two m64 warpgroups x wgmma N = 128)
-constexpr int STAGES = 3;
-constexpr int OP_BYTES = BM * BK * 4;         // 16 KB: one operand's k-block
-constexpr int STAGE_BYTES = 4 * OP_BYTES;     // hi + lo of the row block and of the column block
-constexpr int THREADS = 384;
+using tc::BM;                                 // rows and columns of a tile
 constexpr int NORM_WARPS = 8;
+constexpr int BITS_BYTES = BM * 4 * 4;        // the screen's tile bitmap: [128 rows][4 words]
 
 // ---- normalise + split ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(NORM_WARPS * 32)
@@ -126,53 +123,30 @@ __device__ __forceinline__ uint32_t decide(const GraphParams& P, float g, double
     return exact_edge(P.xhat, P.d, i, j, P.delta) ? 1u : 0u;
 }
 
-__global__ void __launch_bounds__(THREADS, 1)
+__global__ void __launch_bounds__(tc::THREADS, 1)
 pc_graph_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ CUtensorMap map_lo,
                 const GraphParams P) {
     extern __shared__ unsigned char smem_dyn[];
-    unsigned char* stage_base = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);   // SWIZZLE_128B: 1 KB
-    uint64_t* full = reinterpret_cast<uint64_t*>(stage_base + STAGES * STAGE_BYTES);
-    uint64_t* empty = full + STAGES;
-    uint32_t* bits = reinterpret_cast<uint32_t*>(empty + STAGES);          // [128 rows][4 words]: the tile's edges
-
-    const int wg = threadIdx.x >> 7;
+    const tc::Role me = tc::ring_role();
     const int nt = P.ntiles;
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
+    const tc::Ring ring = tc::ring_init(smem_dyn);
+    uint32_t* bits = reinterpret_cast<uint32_t*>(ring.tail);              // [128 rows][4 words]: the tile's edges
 
-    if (wg == 0) {
-        // ================= TMA producer =================
-        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (me.wg == 0) {
+        tc::producer_regs();
         if (threadIdx.x == 0) {
             uint32_t it = 0;
             for (long long idx = blockIdx.x; idx < P.tile_pairs; idx += gridDim.x) {
                 int ti, tj;
                 tile_of(idx, nt, ti, tj);
-                for (int kb = 0; kb < P.kblocks; ++kb, ++it) {
-                    const int s = it % STAGES;
-                    const uint32_t round = it / STAGES;
-                    if (round > 0) mbar_wait(&empty[s], (round - 1) & 1u);
-                    unsigned char* st = stage_base + static_cast<size_t>(s) * STAGE_BYTES;
-                    mbar_expect_tx(&full[s], STAGE_BYTES);
-                    tc::tma_load_2d(st, &map_hi, kb * BK, ti * BM, &full[s]);
-                    tc::tma_load_2d(st + OP_BYTES, &map_lo, kb * BK, ti * BM, &full[s]);
-                    tc::tma_load_2d(st + 2 * OP_BYTES, &map_hi, kb * BK, tj * BM, &full[s]);
-                    tc::tma_load_2d(st + 3 * OP_BYTES, &map_lo, kb * BK, tj * BM, &full[s]);
-                }
+                for (int kb = 0; kb < P.kblocks; ++kb, ++it)
+                    tc::ring_load(ring, it, &map_hi, &map_lo, ti * BM, &map_hi, &map_lo, tj * BM, kb * BK);
             }
         }
         return;
     }
-    // ================= consumers: warpgroup wg - 1 owns rows [64 (wg - 1), 64 wg) of the tile =================
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
-    const int t = threadIdx.x & 127, warp = t >> 5, lane = t & 31, ct = threadIdx.x - 128;
-    const uint32_t a_off = static_cast<uint32_t>(wg - 1) * 64 * BK * 4;
-    // m64nN fp32 fragment: d[4j + {0,1}] = (r, 8j + 2 (lane % 4) + {0,1}), d[4j + {2,3}] = (r + 8, same cols)
-    const int r_in_tile = (wg - 1) * 64 + warp * 16 + (lane >> 2);
-    const int c_in_tile = 2 * (lane & 3);
+    tc::consumer_regs();
+    const int ct = threadIdx.x - 128;
     unsigned int rech = 0;
     uint32_t it = 0;
     for (long long idx = blockIdx.x; idx < P.tile_pairs; idx += gridDim.x) {
@@ -180,38 +154,18 @@ pc_graph_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constan
         tile_of(idx, nt, ti, tj);
         float acc[64];
         int prev = -1;
-        for (int kb = 0; kb < P.kblocks; ++kb, ++it) {
-            const int s = it % STAGES;
-            mbar_wait(&full[s], (it / STAGES) & 1u);
-            const uint32_t a_hi = smem_u32(stage_base + static_cast<size_t>(s) * STAGE_BYTES) + a_off;
-            const uint32_t a_lo = a_hi + OP_BYTES, b_hi = a_hi - a_off + 2 * OP_BYTES, b_lo = b_hi + OP_BYTES;
-            tc::wgmma_fence();
-#pragma unroll
-            for (int k = 0; k < BK / UK; ++k) {
-                const uint32_t off = k * UK * 4;
-                const uint64_t dah = tc::make_desc(a_hi + off), dal = tc::make_desc(a_lo + off);
-                const uint64_t dbh = tc::make_desc(b_hi + off), dbl = tc::make_desc(b_lo + off);
-                tc::wgmma_tf32(acc, dah, dbh, (kb == 0 && k == 0) ? 0u : 1u);
-                tc::wgmma_tf32(acc, dah, dbl, 1u);
-                tc::wgmma_tf32(acc, dal, dbh, 1u);
-            }
-            tc::wgmma_commit();
-            tc::wgmma_wait<1>();
-            if (prev >= 0 && t == 0) mbar_arrive(&empty[prev]);
-            prev = s;
-        }
-        tc::wgmma_wait<0>();
-        if (prev >= 0 && t == 0) mbar_arrive(&empty[prev]);
+        for (int kb = 0; kb < P.kblocks; ++kb, ++it) tc::ring_mma(ring, it, me.a_off, acc, kb == 0, prev, me.t);
+        tc::ring_drain(ring, prev, me.t);
 
         // ---- epilogue: the decisions of this thread's 2 x 32 pairs as canonical column masks of its two rows
-        const int row0 = ti * BM + r_in_tile, row1 = row0 + 8;
+        const int row0 = ti * BM + me.r_in_tile, row1 = row0 + 8;
         const double n0 = row0 < P.n ? __ldg(P.nrm2 + row0) : 0.0, n1 = row1 < P.n ? __ldg(P.nrm2 + row1) : 0.0;
         uint32_t m0[4] = {0u, 0u, 0u, 0u}, m1[4] = {0u, 0u, 0u, 0u};
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
-                const int cl = 8 * j + c_in_tile + e, col = tj * BM + cl;
+                const int cl = 8 * j + me.c_in_tile + e, col = tj * BM + cl;
                 if (col >= P.n) continue;
                 const double nc = __ldg(P.nrm2 + col);
                 if (row0 < P.n) m0[cl >> 5] |= decide(P, acc[4 * j + e], n0, nc, row0, col, rech) << (cl & 31);
@@ -225,11 +179,11 @@ pc_graph_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constan
                 m0[w] |= __shfl_xor_sync(0xffffffffu, m0[w], o);
                 m1[w] |= __shfl_xor_sync(0xffffffffu, m1[w], o);
             }
-        if ((lane & 3) == 0)
+        if ((me.lane & 3) == 0)
 #pragma unroll
             for (int w = 0; w < 4; ++w) {
-                bits[r_in_tile * 4 + w] = m0[w];
-                bits[(r_in_tile + 8) * 4 + w] = m1[w];
+                bits[me.r_in_tile * 4 + w] = m0[w];
+                bits[(me.r_in_tile + 8) * 4 + w] = m1[w];
             }
         asm volatile("bar.sync 1, 256;" ::: "memory");
         if (ct < BM) {
@@ -448,10 +402,10 @@ extern "C" int alq_probcover_graph(alq_ctx* ctx, const float* x, int64_t n, int3
     P.slack = 1e-9 * P.delta2 + 1e-10;
     P.tile_cnt = tile_cnt; P.row_ptr = reinterpret_cast<const long long*>(row_ptr); P.cols = cols;
     P.recheck = rech; P.fill = fill ? 1 : 0;
-    const size_t smem = static_cast<size_t>(STAGES) * STAGE_BYTES + 1024 + 2 * STAGES * 8 + BM * 4 * 4;
+    const size_t smem = tc::ring_smem_bytes(BITS_BYTES);
     ALQ_CUDA(ctx, cudaFuncSetAttribute(pc_graph_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
     const int grid = static_cast<int>(std::min<long long>(ctx->sm_count, P.tile_pairs));
-    pc_graph_kernel<<<grid, THREADS, smem, st>>>(mhi, mlo, P);
+    pc_graph_kernel<<<grid, tc::THREADS, smem, st>>>(mhi, mlo, P);
     ALQ_LAUNCH_CHECK(ctx);
     if (fill) {
         ALQ_CUDA(ctx, cudaStreamSynchronize(st));

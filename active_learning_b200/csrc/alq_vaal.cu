@@ -1,9 +1,9 @@
 // K9: the VAAL discriminator on the Hopper tensor cores (vaal_sampler.py:57-58 and vaal_discriminator.py of the
 // reference's query_strategies):  p[i] = sigmoid(w3 . relu(W2 relu(W1 mu_i + b1) + b2) + b3),  hidden width 512.
 //
-// Two launches of one kernel template per pool slice of at most SLICE_ROWS rows, both on K3's pipeline
-// (alq_wgmma.cuh): a one-thread TMA producer warpgroup feeding a 3-stage SWIZZLE_128B ring, two consumer
-// warpgroups issuing wgmma m64n128k8 3xTF32 (hi*hi' + hi*lo' + lo*hi', operands split ahead of time).
+// Two launches of one kernel template per pool slice of at most SLICE_ROWS rows, both on the ring of alq_wgmma.cuh
+// that K3 and K13 use: a one-thread TMA producer warpgroup feeding a 3-stage SWIZZLE_128B ring, two consumer
+// warpgroups issuing the 3xTF32 chain tc::ring_mma (hi*hi' + hi*lo' + lo*hi', operands split ahead of time).
 //   layer 1  X = mu [rows, z] (z zero-padded to a multiple of 32), Y = W1 [512, z].  Epilogue: relu(acc + b1),
 //            stored as the TF32 hi/lo pair layer 2 reads, so the [rows, 512] intermediate needs no split pass.
 //   layer 2  X = H1 [rows, 512], Y = W2 [512, 512].  Epilogue: relu(acc + b2_j) * w3_j summed over all 512
@@ -18,12 +18,7 @@ namespace vaal {
 using namespace tc;
 
 constexpr int HID = 512;                          // the reference's only hidden width
-constexpr int BM = 128, BN = 128, NT = HID / BN;
-constexpr int STAGES = 3;
-constexpr int A_BYTES = BM * BK * 4;              // 16 KB
-constexpr int B_BYTES = BN * BK * 4;              // 16 KB
-constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;
-constexpr int THREADS = 384;
+constexpr int NT = HID / BN;
 constexpr int64_t SLICE_ROWS = 131072;            // bounds the hi + lo intermediate at 512 MB
 
 struct Params {
@@ -40,79 +35,33 @@ __global__ void __launch_bounds__(THREADS, 1)
 vaal_layer_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_constant__ CUtensorMap map_xl,
                   const __grid_constant__ CUtensorMap map_yh, const __grid_constant__ CUtensorMap map_yl, Params P) {
     extern __shared__ unsigned char smem_dyn[];
-    unsigned char* smem_raw = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);   // SWIZZLE_128B alignment
-    unsigned char* stage_base = smem_raw;
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem_raw + STAGES * STAGE_BYTES);
-    uint64_t* empty = full + STAGES;
-
-    const int wg = threadIdx.x >> 7;
+    const Role me = ring_role();
     const int m_blocks = (P.rows + BM - 1) / BM;
+    const Ring ring = ring_init(smem_dyn);
 
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-
-    if (wg == 0) {
-        // ================= TMA producer =================
-        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (me.wg == 0) {
+        producer_regs();
         if (threadIdx.x == 0) {
             uint32_t it = 0;
             for (int mb = blockIdx.x; mb < m_blocks; mb += gridDim.x)
                 for (int nt = 0; nt < NT; ++nt)
-                    for (int kb = 0; kb < P.kblocks; ++kb, ++it) {
-                        const int s = it % STAGES;
-                        const uint32_t round = it / STAGES;
-                        if (round > 0) mbar_wait(&empty[s], (round - 1) & 1u);
-                        unsigned char* st = stage_base + static_cast<size_t>(s) * STAGE_BYTES;
-                        mbar_expect_tx(&full[s], STAGE_BYTES);
-                        tma_load_2d(st, &map_xh, kb * BK, mb * BM, &full[s]);
-                        tma_load_2d(st + A_BYTES, &map_xl, kb * BK, mb * BM, &full[s]);
-                        tma_load_2d(st + 2 * A_BYTES, &map_yh, kb * BK, nt * BN, &full[s]);
-                        tma_load_2d(st + 2 * A_BYTES + B_BYTES, &map_yl, kb * BK, nt * BN, &full[s]);
-                    }
+                    for (int kb = 0; kb < P.kblocks; ++kb, ++it)
+                        ring_load(ring, it, &map_xh, &map_xl, mb * BM, &map_yh, &map_yl, nt * BN, kb * BK);
         }
     } else {
-        // ================= consumers: warpgroup wg - 1 owns rows [64 (wg - 1), 64 wg) of the tile =================
-        asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
-        const int t = threadIdx.x & 127, warp = t >> 5, lane = t & 31;
-        const uint32_t a_off = static_cast<uint32_t>(wg - 1) * 64 * BK * 4;
-        // m64nN fp32 fragment: d[4j + {0,1}] = (r, 8j + 2 (lane % 4) + {0,1}), d[4j + {2,3}] = (r + 8, same cols)
-        const int r_in_tile = (wg - 1) * 64 + warp * 16 + (lane >> 2);
-        const int c_in_tile = 2 * (lane & 3);
+        consumer_regs();
         uint32_t it = 0;
         for (int mb = blockIdx.x; mb < m_blocks; mb += gridDim.x) {
-            const int row0 = mb * BM + r_in_tile, row1 = row0 + 8;
+            const int row0 = mb * BM + me.r_in_tile, row1 = row0 + 8;
             float s0 = 0.f, s1 = 0.f;                 // layer 2: this thread's share of the w3 dot product
             for (int nt = 0; nt < NT; ++nt) {
                 float acc[64];
                 int prev = -1;
-                for (int kb = 0; kb < P.kblocks; ++kb, ++it) {
-                    const int s = it % STAGES;
-                    mbar_wait(&full[s], (it / STAGES) & 1u);
-                    const uint32_t a_hi = smem_u32(stage_base + static_cast<size_t>(s) * STAGE_BYTES) + a_off;
-                    const uint32_t a_lo = a_hi + A_BYTES, b_hi = a_hi - a_off + 2 * A_BYTES, b_lo = b_hi + B_BYTES;
-                    wgmma_fence();
-#pragma unroll
-                    for (int k = 0; k < BK / UK; ++k) {
-                        const uint32_t off = k * UK * 4;
-                        const uint64_t dah = make_desc(a_hi + off), dal = make_desc(a_lo + off);
-                        const uint64_t dbh = make_desc(b_hi + off), dbl = make_desc(b_lo + off);
-                        wgmma_tf32(acc, dah, dbh, (kb == 0 && k == 0) ? 0u : 1u);
-                        wgmma_tf32(acc, dah, dbl, 1u);
-                        wgmma_tf32(acc, dal, dbh, 1u);
-                    }
-                    wgmma_commit();
-                    wgmma_wait<1>();                          // the previous stage's MMAs have retired: hand it back
-                    if (prev >= 0 && t == 0) mbar_arrive(&empty[prev]);
-                    prev = s;
-                }
-                wgmma_wait<0>();
-                if (prev >= 0 && t == 0) mbar_arrive(&empty[prev]);
+                for (int kb = 0; kb < P.kblocks; ++kb, ++it) ring_mma(ring, it, me.a_off, acc, kb == 0, prev, me.t);
+                ring_drain(ring, prev, me.t);
 #pragma unroll
                 for (int j = 0; j < 16; ++j) {
-                    const int col = nt * BN + 8 * j + c_in_tile;
+                    const int col = nt * BN + 8 * j + me.c_in_tile;
                     const float bb0 = __ldg(P.bias + col), bb1 = __ldg(P.bias + col + 1);
                     const float h00 = fmaxf(acc[4 * j] + bb0, 0.f), h01 = fmaxf(acc[4 * j + 1] + bb1, 0.f);
                     const float h10 = fmaxf(acc[4 * j + 2] + bb0, 0.f), h11 = fmaxf(acc[4 * j + 3] + bb1, 0.f);
@@ -141,7 +90,7 @@ vaal_layer_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_const
                 // the four lanes of a quad hold the same two rows, 128 columns each
                 s0 += __shfl_xor_sync(0xffffffffu, s0, 1); s1 += __shfl_xor_sync(0xffffffffu, s1, 1);
                 s0 += __shfl_xor_sync(0xffffffffu, s0, 2); s1 += __shfl_xor_sync(0xffffffffu, s1, 2);
-                if ((lane & 3) == 0) {
+                if ((me.lane & 3) == 0) {
                     const float b3 = __ldg(P.b3);
                     if (row0 < P.rows) {
                         const float x = s0 + b3;
@@ -222,7 +171,7 @@ extern "C" int alq_vaal_scores(alq_ctx* ctx, const float* mu, int64_t n, int32_t
     if (!(make_map(&mw1h, w1h, HID, kp, BN) && make_map(&mw1l, w1l, HID, kp, BN) && make_map(&mw2h, w2h, HID, HID, BN) &&
           make_map(&mw2l, w2l, HID, HID, BN)))
         ALQ_FAIL(ctx, ALQ_ERR_CUDA, "alq_vaal_scores: cuTensorMapEncodeTiled failed");
-    const size_t smem = static_cast<size_t>(STAGES) * STAGE_BYTES + 256 + 1024;
+    const size_t smem = ring_smem_bytes(0);
     ALQ_CUDA(ctx, cudaFuncSetAttribute(vaal_layer_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
     ALQ_CUDA(ctx, cudaFuncSetAttribute(vaal_layer_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
 

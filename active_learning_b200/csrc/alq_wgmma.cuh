@@ -1,7 +1,17 @@
-// Hopper tensor-core building blocks shared by the wgmma kernels (K3 in alq_mindist_tc.cu, K9 in alq_vaal.cu):
-// TMA tile loads, SWIZZLE_128B shared-memory descriptors, the m64n128k8 TF32 MMA and the host-side tensor-map
-// encoder.  Operands are fp32 rows already split into TF32 hi/lo pairs; a stage row is BK = 32 fp32 = 128 bytes,
-// one swizzle span.
+// The Hopper 3xTF32 tile pipeline of the wgmma kernels (K3 in alq_mindist_tc.cu, K9 in alq_vaal.cu, K13 in
+// alq_probcover.cu): TMA tile loads, SWIZZLE_128B shared-memory descriptors, the m64n128k8 TF32 MMA, the host-side
+// tensor-map encoder, and the ring that connects them.  Operands are fp32 rows already split into TF32 hi/lo pairs; a
+// stage row is BK = 32 fp32 = 128 bytes, one swizzle span.
+//
+// The ring (one CTA per SM, 3 warpgroups):
+//   warpgroup 0    TMA producer (one thread): per k-block, the hi and lo boxes of a 128-row block of X and of a
+//                  128-row block of Y into one of 3 shared-memory stages (ring_load), mbarrier complete_tx on `full`.
+//   warpgroups 1-2 consumers: each owns 64 of the tile's 128 rows and issues hi*hi' + hi*lo' + lo*hi' per 8-wide
+//                  k-step, k ascending, into one m64n128 fp32 register fragment (ring_mma), keeping one stage in
+//                  flight and handing the previous one back on `empty`.
+// Each kernel keeps its own work schedule and epilogue; the producer and the consumers walk the same sequence of
+// k-blocks, counted by `it`.  K3, K9 and K13 all issue this one chain, so the 3xTF32 error bound of DESIGN section 4,
+// measured through K3, holds for all three.
 #pragma once
 #include <cuda.h>
 
@@ -11,6 +21,19 @@ namespace tc {
 
 constexpr int BK = 32;           // fp32 per stage row = 128 bytes = one swizzle span
 constexpr int UK = 8;            // wgmma K for tf32
+constexpr int BM = 128;          // rows per tile (two m64 consumer warpgroups)
+constexpr int BN = 128;          // columns per tile (wgmma N)
+constexpr int STAGES = 3;
+constexpr int OP_BYTES = BM * BK * 4;             // 16 KB: one operand's k-block (BM == BN)
+constexpr int STAGE_BYTES = 4 * OP_BYTES;         // hi + lo of the row block and of the column block = 64 KB
+constexpr int THREADS = 384;
+static_assert(BM == BN, "the four operand boxes of a stage share OP_BYTES");
+
+// dynamic shared memory of a ring kernel: the stages, the 1 KB SWIZZLE_128B alignment slack, the full / empty
+// barriers, and `extra` bytes the kernel places after them (Ring::tail)
+__host__ __device__ constexpr size_t ring_smem_bytes(size_t extra) {
+    return static_cast<size_t>(STAGES) * STAGE_BYTES + 1024 + 2 * STAGES * sizeof(uint64_t) + extra;
+}
 
 __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
     asm volatile(
@@ -60,6 +83,97 @@ __device__ __forceinline__ void split_tf32(float v, float& hi, float& lo) {
     hi = __uint_as_float(hb);
     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(lb) : "f"(v - hi));
     lo = __uint_as_float(lb);
+}
+
+// ---- the ring ----------------------------------------------------------------------------------------------------------
+struct Ring {
+    unsigned char* stage;        // STAGES x STAGE_BYTES, 1 KB aligned: [X hi | X lo | Y hi | Y lo] per stage
+    uint64_t* full;              // [STAGES] the producer's TMA bytes have landed
+    uint64_t* empty;             // [STAGES] both consumer warpgroups have retired the stage's MMAs
+    unsigned char* tail;         // the first byte after the barriers (ring_smem_bytes' `extra`)
+};
+
+// every thread of the CTA, before the role split
+__device__ __forceinline__ Ring ring_init(unsigned char* smem_dyn) {
+    Ring r;
+    // SWIZZLE_128B tiles must sit on 1024-byte boundaries: align by hand (ring_smem_bytes allocates 1 KB of slack)
+    r.stage = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
+    r.full = reinterpret_cast<uint64_t*>(r.stage + STAGES * STAGE_BYTES);
+    r.empty = r.full + STAGES;
+    r.tail = reinterpret_cast<unsigned char*>(r.empty + STAGES);
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < STAGES; ++s) { mbar_init(&r.full[s], 1); mbar_init(&r.empty[s], 2); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    return r;
+}
+
+// A thread's role.  Warpgroup 0 produces, warpgroups 1-2 consume; warpgroup wg - 1 owns rows [64 (wg - 1), 64 wg) of the
+// tile.  m64nN fp32 fragment: d[4j + {0,1}] = (r, 8j + 2 (lane % 4) + {0,1}), d[4j + {2,3}] = (r + 8, same cols),
+// r = 16 warp + lane / 4 inside the warpgroup's 64 rows.
+struct Role {
+    int wg, t, lane;
+    uint32_t a_off;              // the warpgroup's 64 rows inside an X box: 8 KB, a whole number of swizzle atoms
+    int r_in_tile, c_in_tile;    // the fragment's first row and first column inside the 128 x 128 tile
+};
+__device__ __forceinline__ Role ring_role() {
+    Role r;
+    r.wg = threadIdx.x >> 7;
+    r.t = threadIdx.x & 127;
+    r.lane = threadIdx.x & 31;
+    r.a_off = static_cast<uint32_t>(r.wg - 1) * 64 * BK * 4;
+    r.r_in_tile = (r.wg - 1) * 64 + (r.t >> 5) * 16 + (r.lane >> 2);
+    r.c_in_tile = 2 * (r.lane & 3);
+    return r;
+}
+// the producer warpgroup gives its registers to the consumers: 40 + 2 x 232 = 3 x 168, the launch's budget per thread
+__device__ __forceinline__ void producer_regs() { asm volatile("setmaxnreg.dec.sync.aligned.u32 40;"); }
+__device__ __forceinline__ void consumer_regs() { asm volatile("setmaxnreg.inc.sync.aligned.u32 232;"); }
+
+// Producer, k-block `it` of the CTA's sequence: columns [k0, k0 + 32) of rows [a_row, a_row + 128) of X (a_hi, a_lo) and
+// of rows [b_row, b_row + 128) of Y (b_hi, b_lo) into stage it % STAGES, once the consumers have handed it back.
+__device__ __forceinline__ void ring_load(const Ring& r, uint32_t it, const CUtensorMap* a_hi, const CUtensorMap* a_lo,
+                                          int a_row, const CUtensorMap* b_hi, const CUtensorMap* b_lo, int b_row, int k0) {
+    const int s = it % STAGES;
+    const uint32_t round = it / STAGES;
+    if (round > 0) mbar_wait(&r.empty[s], (round - 1) & 1u);
+    unsigned char* st = r.stage + static_cast<size_t>(s) * STAGE_BYTES;
+    mbar_expect_tx(&r.full[s], STAGE_BYTES);
+    tma_load_2d(st, a_hi, k0, a_row, &r.full[s]);
+    tma_load_2d(st + OP_BYTES, a_lo, k0, a_row, &r.full[s]);
+    tma_load_2d(st + 2 * OP_BYTES, b_hi, k0, b_row, &r.full[s]);
+    tma_load_2d(st + 3 * OP_BYTES, b_lo, k0, b_row, &r.full[s]);
+}
+
+// Consumer, k-block `it`: acc (+)= X Y^T over the stage's 32 columns as 4 k-steps of hi*hi' + hi*lo' + lo*hi'; `first`
+// overwrites acc on the first MMA.  The MMAs stay in flight; the previous stage (`prev`, -1 for none) is handed back
+// once its own have retired, and `prev` becomes this stage.  After a tile's last k-block, ring_drain.
+__device__ __forceinline__ void ring_mma(const Ring& r, uint32_t it, uint32_t a_off, float (&acc)[64], bool first,
+                                         int& prev, int t) {
+    const int s = it % STAGES;
+    mbar_wait(&r.full[s], (it / STAGES) & 1u);
+    const uint32_t a_hi = smem_u32(r.stage + static_cast<size_t>(s) * STAGE_BYTES) + a_off;
+    const uint32_t a_lo = a_hi + OP_BYTES, b_hi = a_hi - a_off + 2 * OP_BYTES, b_lo = b_hi + OP_BYTES;
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < BK / UK; ++k) {
+        const uint32_t off = k * UK * 4;    // bytes along K inside the 128-byte swizzle span
+        const uint64_t dah = make_desc(a_hi + off), dal = make_desc(a_lo + off);
+        const uint64_t dbh = make_desc(b_hi + off), dbl = make_desc(b_lo + off);
+        wgmma_tf32(acc, dah, dbh, (first && k == 0) ? 0u : 1u);
+        wgmma_tf32(acc, dah, dbl, 1u);
+        wgmma_tf32(acc, dal, dbh, 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<1>();
+    if (prev >= 0 && t == 0) mbar_arrive(&r.empty[prev]);
+    prev = s;
+}
+// every MMA of the tile has retired: the accumulators are readable and the last stage goes back
+__device__ __forceinline__ void ring_drain(const Ring& r, int prev, int t) {
+    wgmma_wait<0>();
+    if (prev >= 0 && t == 0) mbar_arrive(&r.empty[prev]);
 }
 
 using EncodeFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,

@@ -1,10 +1,10 @@
 """The 3xTF32 bound of DESIGN section 4 measured on the H100's own tensor cores, K13's rechecks predicted pair by pair,
 and K14 at its segment limit.
 
-K3 (alq_mindist_tc.cu) and K13 (alq_probcover.cu) issue the same wgmma chain: the same split_tf32, per 8-wide k-step
-hi hi', hi lo', lo hi', k ascending, into one m64n128 fp32 fragment.  With zero norms and one column row, K3 returns
-fl(fl(0 + 0) - 2 acc) = -2 g exactly, so g_hw(X, y) = -0.5 K3(X, 0, y, 0) reads the tensor core's fp32 dot product g of
-any operand pair through the public API.  The probe is established first (exact where it must be, on the tensor path,
+K3 (alq_mindist_tc.cu) and K13 (alq_probcover.cu) issue the same wgmma chain, tc::ring_mma of alq_wgmma.cuh: the same
+split_tf32, per 8-wide k-step hi hi', hi lo', lo hi', k ascending, into one m64n128 fp32 fragment.  With zero norms and
+one column row, K3 returns fl(fl(0 + 0) - 2 acc) = -2 g exactly, so g_hw(X, y) = -0.5 K3(X, 0, y, 0) reads the tensor
+core's fp32 dot product g of any operand pair through the public API.  The probe is established first (exact where it must be, on the tensor path,
 independent of the pair's place in the tile); then it holds E against fp64 truth and predicts K13's band decisions.
 """
 import contextlib

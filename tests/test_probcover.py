@@ -1,6 +1,7 @@
 """ProbCoverSampler without a GPU: the oracle's greedy against the authors' loop, the tensor-core screen's bound against
 fp64 truth, and the sampler's host logic (RNG draws, budget clamp, cache, pickling) through a fake engine built on the
 oracle."""
+import os
 import pickle
 
 import numpy as np
@@ -120,6 +121,18 @@ def test_the_adder_models_are_exact_on_tf32_integers_and_differ_elsewhere():
     g = {ad: P.emulate_3xtf32(fam, fam[::-1], adder=ad) for ad in ("nearest", "zero", "align")}
     assert (g["align"] != g["nearest"]).any() and (g["align"] != g["zero"]).any()
     assert (P.emulate_3xtf32(fam, fam[::-1], adder="align", bits=21) != g["align"]).any()
+
+
+def test_the_tensor_core_kernels_issue_only_the_rings_chain():
+    """test_gpu_tf32_bound.py measures the bound through K3 and applies it to K13 (and DESIGN section 4 to K9) because all
+    three issue one chain: alq_wgmma.cuh's tc::ring_mma.  None of them may issue MMAs, TMA loads or barriers of its own."""
+    csrc = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "active_learning_b200", "csrc")
+    for name in ("alq_mindist_tc.cu", "alq_vaal.cu", "alq_probcover.cu"):
+        with open(os.path.join(csrc, name)) as f:
+            src = f.read()
+        assert "ring_mma(" in src, name
+        for own in ("wgmma_tf32(", "tma_load_2d(", "mbar_init("):
+            assert own not in src, (name, own)
 
 
 # ---- the sampler's host logic ------------------------------------------------------------------------------------------
