@@ -637,14 +637,19 @@ extern "C" int alq_greedy_select(alq_ctx* ctx, const alq_greedy_desc* D, void* s
         ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_greedy_select: D^2 sampling needs vpos and full_n");
     if (D->part_off_host[0] != 0 || D->part_off_host[P] != n)
         ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_greedy_select: part_off must span [0, n]");
-    // ---- multi-GPU group? (every array is global and replicated; rank r streams its shard: include/alq.h) ----
-    const bool comm = D->shard_off_host != nullptr && ctx->comm.world > 1;
+    // ---- group path? shard_off on a context with a peer-memory group, of any size (a group of one rank included):
+    //      every array is global and replicated, rank r streams its shard (include/alq.h) ----
     const AlqComm& G = ctx->comm;
-    if (D->shard_off_host && ctx->comm.world <= 1 && D->shard_off_host[1] != n)
+    const bool comm = D->shard_off_host != nullptr && G.window != nullptr;
+    if (D->shard_off_host && !comm && D->shard_off_host[1] != n)
         ALQ_FAIL(ctx, ALQ_ERR_STATE, "alq_greedy_select: shard_off given but no multi-GPU group (alq_comm_create/connect)");
     if (comm) {
         if (!G.connected) ALQ_FAIL(ctx, ALQ_ERR_STATE, "alq_greedy_select: alq_comm_connect has not been called");
         if (P != 1) ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_greedy_select: the multi-GPU loop is for one global partition");
+        const int v = D->variant ? D->variant : ctx->greedy_variant;
+        if (v == 1 || v == 2)
+            ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_greedy_select: variant %d with shard_off: the multi-GPU loop has no other variant "
+                                           "than the persistent one", v);
         if (D->shard_off_host[0] != 0 || D->shard_off_host[G.world] != n)
             ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_greedy_select: shard_off must span the n global candidate rows");
         for (int r = 0; r < G.world; ++r)

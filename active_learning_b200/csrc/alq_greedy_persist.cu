@@ -67,10 +67,10 @@ struct PersistArgs {
     int* status;
     unsigned long long* prof;      // [8] ns: streaming, selection, steps, then selection sub-phases
     int world, rank;
-    char* peer[ALQ_MAX_WORLD];     // windows (world == 1: peer[0] = local scratch)
+    char* peer[ALQ_MAX_WORLD];     // windows (one GPU without a group: peer[0] = local scratch)
     int leaf_bound[ALQ_MAX_WORLD + 1];   // multi-GPU D^2: rank r sums leaves [leaf_bound[r], leaf_bound[r+1])
     unsigned int ready_off;        // u64 ready[world] at the head of every window
-    unsigned long long ready_tag;
+    unsigned long long ready_tag;  // group path: epoch << 32, stored into every peer's ready[rank]; 0: no handshake
     unsigned int tag_base;         // 0x80000000 | (epoch & 0x7f) << 24
     int resident_rows;             // rows at the head of every CTA's segment fetched L2::evict_last (they stay in L2 across
                                    // steps; the rest is fetched evict_first).  0: no hints
@@ -534,7 +534,7 @@ greedy_persist_kernel(const __grid_constant__ PersistArgs A, const PipeCfg cfg, 
         }
     }
 
-    if (A.world > 1 && ct < A.world) ll_ready_wait(win + A.ready_off, ct, A.ready_tag, A);   // peers may still be clearing theirs
+    if (A.ready_tag != 0 && ct < A.world) ll_ready_wait(win + A.ready_off, ct, A.ready_tag, A);   // peers may still be clearing theirs
     cons_bar();
 
     // per-warp position in the tile stream (global over all steps): tiles cw, cw + C, cw + 2C, ...
@@ -840,7 +840,7 @@ int alq_greedy_persist(alq_ctx* ctx, const alq_greedy_desc* D, void* stream) {
     const bool sample = D->uniforms_host != nullptr;
     const int d = D->d, c = factored ? D->c : 0;
     const AlqComm& Gc = ctx->comm;
-    const bool comm = D->shard_off_host != nullptr && Gc.world > 1;
+    const bool comm = D->shard_off_host != nullptr && Gc.window != nullptr && Gc.connected;   // the group path (alq_greedy_select)
     const int world = comm ? Gc.world : 1, rank = comm ? Gc.rank : 0;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
 
@@ -1091,7 +1091,7 @@ int alq_greedy_persist(alq_ctx* ctx, const alq_greedy_desc* D, void* stream) {
     for (int r = 0; r <= ALQ_MAX_WORLD; ++r) A.leaf_bound[r] = leaf_bound[std::min(r, world)];
     A.ready_off = 0;
     ctx->comm.epoch += 1;
-    A.ready_tag = ctx->comm.epoch << 32;
+    A.ready_tag = comm ? ctx->comm.epoch << 32 : 0;   // 0: no handshake (one GPU, the window is scratch)
     A.tag_base = static_cast<unsigned int>(ctx->comm.epoch & 0x7fu) << 24 | 0x80000000u;   // never 0: a zeroed word is invalid
     A.timeout_cycles = ctx->spin_timeout_cycles();
     {   // L2 residency: keep `l2_resident_mb` of the rows this GPU streams in L2 across the steps (evict_last), split evenly over the CTAs

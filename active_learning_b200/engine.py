@@ -866,7 +866,9 @@ class Engine:
 
         Multi-GPU (comm_init): every tensor is the GLOBAL, replicated array; `shard_off` [world + 1] says which
         rows each rank streams and, for D^2 sampling, `shard_pos` [world + 1] the matching leaf-aligned position
-        ranges of the full array (sharding.plan_shards)."""
+        ranges of the full array (sharding.plan_shards).  After comm_init a call with `shard_off` takes the group path
+        whatever the group's size: a group of one rank runs the group path (the window, its ready handshake and tags)
+        on this GPU.  Without comm_init, `shard_off=[0, n]` is ignored and any other split is an AlqError."""
         x = _f32c(x, "x")
         n, d = x.shape
         part_off_h = np.ascontiguousarray(part_off, dtype=np.int32)

@@ -240,7 +240,10 @@ typedef struct alq_greedy_desc {
        by GLOBAL candidate row and REPLICATED on every rank (x/a/xn/an/vpos: n rows each; a few hundred MB next to
        180 GB of HBM), so a new centre is announced as a row id and read locally -- no row payload crosses NVLink.
        Rank r streams rows [shard_off[r], shard_off[r+1]) only and owns that range of `mind` (the rest of `mind` is
-       not touched).  picks are global row ids, identical on every rank.  NULL => single GPU.
+       not touched).  picks are global row ids, identical on every rank.  NULL => single GPU.  Given on a context with
+       a group, whatever its size, the call takes the group path: a group of one rank runs the group path too (the
+       window, its ready handshake and tags, on this GPU's own memory).  Given without a group, shard_off = {0, n} is
+       ignored and anything else is ALQ_ERR_STATE.  An explicit variant 1 or 2 (or the option) is ALQ_ERR_INVALID.
        D^2 sampling additionally needs the shards aligned to the leaves of NumPy's pairwise-sum tree over the
        partition's full array: rank r's rows are exactly the candidates with vpos in
        [shard_pos[r], shard_pos[r+1]), every shard_pos a leaf boundary (alq_pairwise_leaf_bounds), shard_pos[0] = 0,

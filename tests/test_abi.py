@@ -125,3 +125,25 @@ def test_pairwise_leaf_bounds_is_numpys_tree_and_matches_the_host_twin():
             assert abs(len(seg) - len(cand) / world) < 200
     off, pos = plan_shards(cand, 130000, 4, leaf_aligned=False)
     assert pos is None and off.tolist() == [0, 20000, 40000, 60000, 80000]
+
+
+def test_leaf_aligned_shards_cut_on_the_librarys_leaf_bounds():
+    """plan_shards(..., leaf_aligned=True) for 1..8 ranks: every shard_pos is a leaf boundary of the library's own
+    alq_pairwise_leaf_bounds (the one the selection loop checks them against), and shard_off is where each position
+    range starts among the candidates, searchsorted(cand_pos, shard_pos)."""
+    import numpy as np
+    from active_learning_b200 import _lib
+    from active_learning_b200.sharding import plan_shards
+    lib = _lib.load()
+    rng = np.random.default_rng(3)
+    for full_n in (1, 2, 128, 129, 1000, 13007, 130000):
+        out = np.empty(full_n // 64 + 8, dtype=np.int32)
+        k = lib.alq_pairwise_leaf_bounds(full_n, ctypes.c_void_p(out.ctypes.data), len(out))
+        bounds = out[:k + 1]
+        for n_cand in sorted({1, max(1, full_n // 7), full_n}):
+            cand = np.sort(rng.choice(full_n, n_cand, replace=False))
+            for world in range(1, 9):
+                off, pos = plan_shards(cand, full_n, world, leaf_aligned=True)
+                assert len(pos) == world + 1 and pos[0] == 0 and pos[-1] == full_n
+                assert np.isin(pos, bounds).all() and (np.diff(pos) >= 0).all(), (full_n, n_cand, world)
+                assert off.tolist() == np.searchsorted(cand, pos).tolist(), (full_n, n_cand, world)
