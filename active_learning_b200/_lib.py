@@ -144,6 +144,13 @@ SIGNATURES = {
                                       C.c_void_p, c_i32p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "alq_probcover_select": (C.c_int, [C.c_void_p, C.c_void_p, c_i32p, C.c_int64, C.c_void_p, C.c_int64, c_i32p,
                                        C.c_void_p, C.c_void_p]),
+    "alq_kmeans_rows": (C.c_int, [C.c_void_p, c_f32p, C.c_int64, C.c_int32, C.c_int64, C.c_int32, c_f32p, c_f32p, c_f32p,
+                                  C.c_void_p, C.c_void_p]),
+    "alq_kmeans_assign": (C.c_int, [C.c_void_p, c_f32p, c_f32p, c_f32p, C.c_void_p, C.c_int64, C.c_int32, c_f32p, C.c_int32,
+                                    c_i32p, C.c_void_p, C.c_void_p]),
+    "alq_kmeans_update": (C.c_int, [C.c_void_p, c_f32p, C.c_int64, C.c_int32, c_i32p, C.c_int32, c_f32p, C.c_void_p]),
+    "alq_typicality": (C.c_int, [C.c_void_p, c_f32p, C.c_int32, c_i32p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p,
+                                 c_i32p, C.c_void_p]),
 }
 
 

@@ -2,9 +2,9 @@
 //
 // K13 alq_probcover_graph   the delta-ball graph of the L2-normalised pool rows as CSR.  There is an edge (i, j) iff
 //                           scipy's fp64 euclidean distance of the fp32 rows (K7's per-pair arithmetic) is < delta.
-//   normalise  one warp per row: lane-strided fp64 sum of squares, a butterfly, norm = sqrt, xhat = fl32(x / norm)
-//              (a zero row stays zero); the same kernel splits xhat into TF32 hi / lo (alq_wgmma.cuh) and stores
-//              nrm2 = |xhat|^2 in fp64.
+//   normalise  one warp per row (alq_rows_split.cuh, shared with K15): lane-strided fp64 sum of squares, a butterfly,
+//              norm = sqrt, xhat = fl32(x / norm) (a zero row stays zero); the same kernel splits xhat into TF32 hi / lo
+//              (alq_wgmma.cuh) and stores nrm2 = |xhat|^2 in fp64.
 //   screen     one CTA per SM, persistent over the upper-triangle 128 x 128 tiles of xhat xhat^T, on the ring of
 //              alq_wgmma.cuh that K3 and K9 use: warpgroup 0 is the TMA producer (3-stage ring), warpgroups 1-2 issue
 //              the 3xTF32 chain tc::ring_mma.  The epilogue decides each pair from d2 = nrm2_i + nrm2_j - 2 g
@@ -30,49 +30,15 @@
 #include <math.h>
 
 #include "alq_ll.cuh"
+#include "alq_rows_split.cuh"
 #include "alq_wgmma.cuh"
 
 namespace pc {
 
 using tc::BK;
 using tc::BM;                                 // rows and columns of a tile
-constexpr int NORM_WARPS = 8;
+using rs::NORM_WARPS;
 constexpr int BITS_BYTES = BM * 4 * 4;        // the screen's tile bitmap: [128 rows][4 words]
-
-// ---- normalise + split ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(NORM_WARPS * 32)
-pc_normalize_kernel(const float* __restrict__ x, int n, int d, long long ldx, float* __restrict__ xhat,
-                    float* __restrict__ hi, float* __restrict__ lo, double* __restrict__ nrm2, int normalise) {
-    const int lane = threadIdx.x & 31;
-    const int row = blockIdx.x * NORM_WARPS + (threadIdx.x >> 5);
-    if (row >= n) return;
-    float* xr = xhat + static_cast<size_t>(row) * d;
-    if (normalise) {
-        const float* src = x + static_cast<size_t>(row) * ldx;
-        double s = 0.0;
-        for (int k = lane; k < d; k += 32) {
-            const double v = static_cast<double>(src[k]);
-            s = __dadd_rn(s, __dmul_rn(v, v));
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) s = __dadd_rn(s, __shfl_xor_sync(0xffffffffu, s, o));
-        const double norm = __dsqrt_rn(s);
-        for (int k = lane; k < d; k += 32)
-            xr[k] = norm > 0.0 ? __double2float_rn(__ddiv_rn(static_cast<double>(src[k]), norm)) : 0.f;
-    }
-    double t = 0.0;
-    for (int k = lane; k < d; k += 32) {            // the lane reads back what it wrote
-        const float v = xr[k];
-        float h, l;
-        tc::split_tf32(v, h, l);
-        hi[static_cast<size_t>(row) * d + k] = h;
-        lo[static_cast<size_t>(row) * d + k] = l;
-        t = __dadd_rn(t, __dmul_rn(static_cast<double>(v), static_cast<double>(v)));
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) t = __dadd_rn(t, __shfl_xor_sync(0xffffffffu, t, o));
-    if (lane == 0) nrm2[row] = t;
-}
 
 struct GraphParams {
     const float* xhat;                 // [n, d]
@@ -384,7 +350,7 @@ extern "C" int alq_probcover_graph(alq_ctx* ctx, const float* x, int64_t n, int3
     double* nrm2 = cur.take<double>(n);
     unsigned long long* rech = cur.take<unsigned long long>(1);
 
-    pc_normalize_kernel<<<(ni + NORM_WARPS - 1) / NORM_WARPS, NORM_WARPS * 32, 0, st>>>(x, ni, d, ldx, xhat, hi, lo, nrm2, fill ? 0 : 1);
+    rs::normalize_split_kernel<<<(ni + NORM_WARPS - 1) / NORM_WARPS, NORM_WARPS * 32, 0, st>>>(x, ni, d, ldx, xhat, hi, lo, nrm2, fill ? 0 : 1);
     ALQ_LAUNCH_CHECK(ctx);
     if (!fill) ALQ_CUDA(ctx, cudaMemsetAsync(rech, 0, 8, st));
 

@@ -842,6 +842,135 @@ class Engine:
                                                   _ptr(picks), C.byref(steps), self._stream()), "alq_probcover_select")
         return picks[:steps.value].cpu().numpy().astype(np.int64), int(steps.value)
 
+    # -- K15 / K16 / K17: TypiClust ----------------------------------------------------------------------
+    KMEANS_MAX_ITER = 100
+
+    @staticmethod
+    def _pad4(x: torch.Tensor) -> torch.Tensor:
+        """x with zero columns up to a multiple of 4 (the tensor maps want 16-byte rows; a zero column changes no
+        distance, norm or dot product)."""
+        n, d = x.shape
+        dp = max(4, (d + 3) & ~3)
+        if dp == d:
+            return x
+        slab = torch.zeros((n, dp), dtype=torch.float32, device=x.device)
+        slab[:, :d] = x
+        return slab
+
+    def normalize(self, x: torch.Tensor) -> torch.Tensor:
+        """The rows of x [n, d] L2-normalised exactly as probcover_graph normalises them, padded with zero columns to a
+        multiple of 4: xhat [n, dp] float32.  ValueError for n = 0 or non-finite rows."""
+        x = _f32c(x, "x")
+        if x.dim() != 2 or x.shape[0] == 0:
+            raise ValueError(f"normalize: need a non-empty [n, d] matrix, got {tuple(x.shape)}")
+        if not bool(torch.isfinite(x).all()):
+            raise ValueError("normalize: the embeddings contain NaN or infinity")
+        return self._kmeans_rows(self._pad4(x), True)[0]
+
+    def _kmeans_rows(self, x: torch.Tensor, normalise: bool):
+        """(xhat, hi, lo, nrm2): K15's row operands; with normalise, xhat = the normalised rows of x."""
+        n, d = x.shape
+        xhat = torch.empty((n, d), dtype=torch.float32, device=x.device) if normalise else x
+        hi, lo = torch.empty_like(xhat), torch.empty_like(xhat)
+        nrm2 = torch.empty(n, dtype=torch.float64, device=x.device)
+        self._check(self.lib.alq_kmeans_rows(self._h, _ptr(x) if normalise else None, n, d, _ld(x), int(normalise),
+                                             _ptr(xhat), _ptr(hi), _ptr(lo), _ptr(nrm2), self._stream()),
+                    "alq_kmeans_rows")
+        return xhat, hi, lo, nrm2
+
+    @staticmethod
+    def _kmeans_inputs(xhat: torch.Tensor, centres: torch.Tensor):
+        xhat, centres = _f32c(xhat, "xhat").contiguous(), _f32c(centres, "centres").contiguous()
+        if xhat.dim() != 2 or centres.dim() != 2 or xhat.shape[1] != centres.shape[1] or xhat.shape[1] % 4:
+            raise AlqError(f"kmeans: xhat [n, d] and centres [K, d] with d % 4 == 0, got {tuple(xhat.shape)} and "
+                           f"{tuple(centres.shape)}")
+        return xhat, centres
+
+    def _assign(self, rows, centres: torch.Tensor, labels: torch.Tensor):
+        xhat, hi, lo, nrm2 = rows
+        n, d = xhat.shape
+        counts = (C.c_int64 * 2)()
+        self._check(self.lib.alq_kmeans_assign(self._h, _ptr(xhat), _ptr(hi), _ptr(lo), _ptr(nrm2), n, d, _ptr(centres),
+                                               centres.shape[0], _ptr(labels), counts, self._stream()),
+                    "alq_kmeans_assign")
+        return int(counts[0]), int(counts[1])
+
+    def kmeans_assign(self, xhat: torch.Tensor, centres: torch.Tensor, labels: Optional[torch.Tensor] = None):
+        """K15: labels[i] = the lowest c of the minimum of the exact fp64 d2(xhat_i, centres_c) (K7's pair arithmetic).
+        `labels` (int32, CUDA) holds the previous labels and is updated in place; None starts from -1.  Returns
+        (labels, rows whose label changed, rows the tensor-core screen left to the exact recheck)."""
+        xhat, centres = self._kmeans_inputs(xhat, centres)
+        if labels is None:
+            labels = torch.full((xhat.shape[0],), -1, dtype=torch.int32, device=xhat.device)
+        elif labels.dtype != torch.int32 or not labels.is_cuda or labels.numel() != xhat.shape[0] or not labels.is_contiguous():
+            raise AlqError("kmeans_assign: labels must be a contiguous int32 CUDA tensor with one entry per row")
+        changed, rech = self._assign(self._kmeans_rows(xhat, False), centres, labels)
+        return labels, changed, rech
+
+    def kmeans_update(self, xhat: torch.Tensor, labels: torch.Tensor, centres: torch.Tensor) -> torch.Tensor:
+        """K16: centres[c] = fl32(fp64 sum of the rows with label c in ascending row order / their count), in place;
+        a cluster with no row keeps its centre.  `centres` must be a contiguous float32 CUDA tensor."""
+        xhat = _f32c(xhat, "xhat").contiguous()
+        if (centres.dtype != torch.float32 or not centres.is_cuda or not centres.is_contiguous()
+                or centres.dim() != 2 or centres.shape[1] != xhat.shape[1]):
+            raise AlqError("kmeans_update: centres must be a contiguous float32 CUDA tensor [K, d]")
+        if labels.dtype != torch.int32 or not labels.is_cuda or labels.numel() != xhat.shape[0]:
+            raise AlqError("kmeans_update: labels must be an int32 CUDA tensor with one entry per row")
+        n, d = xhat.shape
+        self._check(self.lib.alq_kmeans_update(self._h, _ptr(xhat), n, d, _ptr(labels.contiguous()), centres.shape[0],
+                                               _ptr(centres), self._stream()), "alq_kmeans_update")
+        return centres
+
+    def kmeans(self, xhat: torch.Tensor, first_pick: int, uniforms, K: int, max_iter: int = KMEANS_MAX_ITER):
+        """k-means of the rows of xhat [n, d] (d % 4 == 0) into K clusters.  Seeding: k-means++ with nothing labeled,
+        CoresetQuery's D^2 cold start through greedy_select (centre 0 = row first_pick, then one D^2 draw per uniform,
+        K - 1 of them).  Then Lloyd: assign (K15), and while some label changed and fewer than max_iter assignments
+        ran, update (K16) and assign again; one 8-byte copy per assignment.  Returns (labels int32 CUDA [n], centres
+        [K, d], assignments run, seed rows)."""
+        xhat = _f32c(xhat, "xhat").contiguous()
+        n, d = xhat.shape
+        K = int(K)
+        if not 1 <= K <= n:
+            raise ValueError(f"kmeans: K={K} outside [1, n={n}]")
+        u = np.zeros(K, dtype=np.float64)
+        u[1:] = np.asarray(uniforms, dtype=np.float64).reshape(-1)[:K - 1]
+        if np.asarray(uniforms).size != K - 1:
+            raise ValueError(f"kmeans: need K - 1 = {K - 1} uniforms, got {np.asarray(uniforms).size}")
+        mind = torch.full((n,), float("inf"), dtype=torch.float32, device=xhat.device)
+        seeds = self.greedy_select(xhat, self.row_norm2(xhat), mind, [0, n], [K], uniforms=u,
+                                   vpos=torch.arange(n, dtype=torch.int32, device=xhat.device), full_n=[n],
+                                   first_pick=[int(first_pick)]).astype(np.int64)
+        centres = xhat.index_select(0, torch.as_tensor(seeds, device=xhat.device)).contiguous()
+        rows = self._kmeans_rows(self._kmeans_inputs(xhat, centres)[0], False)
+        labels = torch.full((n,), -1, dtype=torch.int32, device=xhat.device)
+        it = 0
+        while True:
+            changed, _ = self._assign(rows, centres, labels)
+            it += 1
+            if changed == 0 or it >= int(max_iter):
+                return labels, centres, it, seeds
+            self.kmeans_update(xhat, labels, centres)
+
+    def typicality(self, xhat: torch.Tensor, rows: torch.Tensor, group_off: Sequence[int], k: int = 20):
+        """K17: rows[group_off[g]:group_off[g + 1]] (int32 CUDA row ids of xhat) form group g.  Per listed row, with
+        k' = min(k, group size // 2): typicality = 1 / (mean + 1e-5), mean = the ascending fp64 sum of its k' smallest
+        exact squared distances to the other rows of its group / k' (0 for a group of one row).  Returns (typicality
+        float64 CUDA [len(rows)], host int64 [groups]: the position in rows of each group's largest, lowest on ties).
+        k must lie in [1, 32] (AlqError otherwise)."""
+        xhat = _f32c(xhat, "xhat").contiguous()
+        if rows.dtype != torch.int32 or not rows.is_cuda:
+            raise AlqError("typicality: rows must be an int32 CUDA tensor")
+        rows = rows.contiguous()
+        goff = np.ascontiguousarray(group_off, dtype=np.int64)
+        if goff.ndim != 1 or len(goff) < 2 or goff[-1] != rows.numel():
+            raise AlqError("typicality: group_off must run from 0 to len(rows)")
+        g = len(goff) - 1
+        typ = torch.empty(max(rows.numel(), 1), dtype=torch.float64, device=xhat.device)
+        best = torch.empty(g, dtype=torch.int32, device=xhat.device)
+        self._check(self.lib.alq_typicality(self._h, _ptr(xhat), xhat.shape[1], _ptr(rows), C.c_void_p(goff.ctypes.data),
+                                            g, int(k), _ptr(typ), _ptr(best), self._stream()), "alq_typicality")
+        return typ[:rows.numel()], best.cpu().numpy().astype(np.int64)
+
     # -- K4 / K5 ---------------------------------------------------------------------------------------
     def leaf_bounds(self, n: int) -> np.ndarray:
         """Leaf boundaries of NumPy's float32 pairwise summation over n entries (host helper of the library)."""

@@ -21,6 +21,7 @@ from .query_strategies.balancing import BalancingQuery
 from .query_strategies.margin_clustering import MarginClusteringQuery
 from .query_strategies.mase import BASEQuery, MASEQuery
 from .query_strategies.probcover import ProbCoverQuery
+from .query_strategies.typiclust import TypiClustQuery
 from .query_strategies.uncertainty import ConfidenceQuery, EntropyQuery, MarginQuery
 from .query_strategies.vaal import VAALQuery
 
@@ -38,6 +39,7 @@ _MIXINS = {
     "MarginClusteringSampler": MarginClusteringQuery,
     "BalancedRandomSampler": BalancedRandomQuery,
     "ProbCoverSampler": ProbCoverQuery,
+    "TypiClustSampler": TypiClustQuery,
 }
 
 

@@ -525,6 +525,33 @@ int alq_probcover_graph(alq_ctx* ctx, const float* x, int64_t n, int32_t d, int6
 int alq_probcover_select(alq_ctx* ctx, const int64_t* row_ptr, const int32_t* cols, int64_t n, const uint8_t* labeled,
                          int64_t budget, int32_t* picks, int64_t* n_steps_host, void* stream);
 
+/* ---- K15 / K16 / K17: TypiClust (Hacohen, Dekel & Weinshall, ICML 2022) ----------------------------------------------
+ * alq_kmeans_rows: normalise != 0: xhat = x's rows L2-normalised exactly as alq_probcover_graph does; normalise == 0: xhat
+ *   is the input.  Then hi / lo = the TF32 split of xhat and nrm2 = |xhat|^2 in fp64, the operands of alq_kmeans_assign.
+ *   x[n, d] (fp32, ldx >= d), xhat, hi, lo [n, d] (16-byte aligned), d % 4 == 0.  Asynchronous on `stream`.
+ * alq_kmeans_assign (K15): labels[i] = the lowest c of the minimum over c < K of the exact fp64 d2(xhat_i, centres_c)
+ *   (K7's pair arithmetic: d = a - b, s = s + d * d, k ascending, no FMA).  The pairs are screened on the tensor cores
+ *   (3xTF32) with a rigorous band (DESIGN section 4); a row whose nearest centre the band cannot isolate is recomputed
+ *   exactly against every centre.  labels is read (the previous labels; any value outside [0, K) counts as a change)
+ *   and written.  counts_host[0] = rows whose label changed, counts_host[1] = rows rechecked.  K in [1, 8192].
+ *   Synchronous (one 8-byte copy).
+ * alq_kmeans_update (K16): for every c < K with m_c = |{i : labels[i] == c}| > 0, centres[c] = fl32(S_c / m_c), S_c the
+ *   fp64 sum of the member rows of xhat in ascending row order (one sequential chain per column).  Clusters with no
+ *   member, and rows whose label is outside [0, K), are left alone.  K in [1, 8192].  Asynchronous on `stream`.
+ * alq_typicality (K17): rows[group_off_host[g] .. group_off_host[g + 1]) (int32 row ids of xhat[., d], device) form group
+ *   g, every group non-empty.  For each listed row, k = min(k_max, m_g / 2) and mean = the ascending fp64 sum of the k
+ *   smallest exact fp64 d2 (K7's arithmetic) to the other rows of its group (itself excluded by position) divided by k;
+ *   typ = 1 / (mean + 1e-5) (fp64, device, one per listed row; 0 for a group of one row).  best[g] = the position in
+ *   rows of the group's largest typ, the lowest on ties.  k_max in [1, 32].  Synchronous. */
+int alq_kmeans_rows(alq_ctx* ctx, const float* x, int64_t n, int32_t d, int64_t ldx, int32_t normalise, float* xhat,
+                    float* hi, float* lo, double* nrm2, void* stream);
+int alq_kmeans_assign(alq_ctx* ctx, const float* xhat, const float* hi, const float* lo, const double* nrm2, int64_t n,
+                      int32_t d, const float* centres, int32_t k, int32_t* labels, int64_t* counts_host, void* stream);
+int alq_kmeans_update(alq_ctx* ctx, const float* xhat, int64_t n, int32_t d, const int32_t* labels, int32_t k,
+                      float* centres, void* stream);
+int alq_typicality(alq_ctx* ctx, const float* xhat, int32_t d, const int32_t* rows, const int64_t* group_off_host,
+                   int32_t groups, int32_t k_max, double* typ, int32_t* best, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
