@@ -971,6 +971,41 @@ class Engine:
                                             g, int(k), _ptr(typ), _ptr(best), self._stream()), "alq_typicality")
         return typ[:rows.numel()], best.cpu().numpy().astype(np.int64)
 
+    # -- K18 / K19: CAL ------------------------------------------------------------------------------
+    def knn(self, x: torch.Tensor, y: torch.Tensor, k: int):
+        """K18: the k nearest rows of y [m, d] for every row of x [n, d] (float32 CUDA, d % 4 == 0) by the exact fp64
+        squared distance of the raw rows (K7's pair arithmetic), ascending (d2, row of y).  Returns (idx int32 CUDA
+        [n, k], d2 float64 CUDA [n, k], rows that took the exact fallback scan); past m entries are -1 / +inf.  AlqError
+        for k outside [1, 32], d % 4 != 0, an empty x or y, or a squared row norm that is not finite or above 2^100."""
+        x, y = _f32c(x, "x").contiguous(), _f32c(y, "y").contiguous()
+        if x.dim() != 2 or y.dim() != 2 or x.shape[1] != y.shape[1]:
+            raise AlqError(f"knn: need x [n, d] and y [m, d], got {tuple(x.shape)} and {tuple(y.shape)}")
+        n, k = x.shape[0], int(k)
+        idx = torch.empty((n, max(k, 1)), dtype=torch.int32, device=x.device)
+        d2 = torch.empty((n, max(k, 1)), dtype=torch.float64, device=x.device)
+        fallback = C.c_int64(0)
+        self._check(self.lib.alq_knn(self._h, _ptr(x), n, _ptr(y), y.shape[0], x.shape[1], k, _ptr(idx), _ptr(d2),
+                                     C.byref(fallback), self._stream()), "alq_knn")
+        return idx, d2, int(fallback.value)
+
+    def cal_scores(self, cand_logits: torch.Tensor, ref_logits: torch.Tensor, idx: torch.Tensor):
+        """K19: CAL's score of every candidate row against its neighbours idx [n, k] (int32 CUDA rows of ref_logits,
+        entries outside [0, m) skipped): the mean over the neighbours of KL(softmax(ref) || softmax(cand)) in fp64 (spec:
+        tests/cal_oracle.py).  Returns (score float64 CUDA [n], key float32 CUDA [n]), key = -fl32(score) with +0.0 for a
+        zero and +NaN for a NaN score, so that select_smallest(key, b) takes the b largest scores, lowest row on ties."""
+        zc, zr = _f32c(cand_logits, "cand_logits").contiguous(), _f32c(ref_logits, "ref_logits").contiguous()
+        if zc.dim() != 2 or zr.dim() != 2 or zc.shape[1] != zr.shape[1]:
+            raise AlqError(f"cal_scores: need logits [n, C] and [m, C], got {tuple(zc.shape)} and {tuple(zr.shape)}")
+        if idx.dtype != torch.int32 or not idx.is_cuda or idx.dim() != 2 or idx.shape[0] != zc.shape[0]:
+            raise AlqError("cal_scores: idx must be an int32 CUDA tensor [n, k]")
+        idx = idx.contiguous()
+        n = zc.shape[0]
+        score = torch.empty(n, dtype=torch.float64, device=zc.device)
+        key = torch.empty(n, dtype=torch.float32, device=zc.device)
+        self._check(self.lib.alq_cal_scores(self._h, _ptr(zc), n, _ptr(zr), zr.shape[0], zc.shape[1], _ptr(idx),
+                                            idx.shape[1], _ptr(score), _ptr(key), self._stream()), "alq_cal_scores")
+        return score, key
+
     # -- K4 / K5 ---------------------------------------------------------------------------------------
     def leaf_bounds(self, n: int) -> np.ndarray:
         """Leaf boundaries of NumPy's float32 pairwise summation over n entries (host helper of the library)."""

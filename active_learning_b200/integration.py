@@ -17,6 +17,7 @@ from __future__ import annotations
 from .query_strategies.coreset import (BADGEQuery, CoresetQuery, PartitionedBADGEQuery,
                                        PartitionedCoresetQuery)
 from .query_strategies.balanced_random import BalancedRandomQuery
+from .query_strategies.cal import CALQuery
 from .query_strategies.balancing import BalancingQuery
 from .query_strategies.margin_clustering import MarginClusteringQuery
 from .query_strategies.mase import BASEQuery, MASEQuery
@@ -40,6 +41,7 @@ _MIXINS = {
     "BalancedRandomSampler": BalancedRandomQuery,
     "ProbCoverSampler": ProbCoverQuery,
     "TypiClustSampler": TypiClustQuery,
+    "CALSampler": CALQuery,
 }
 
 

@@ -1,12 +1,13 @@
 """`--strategy` dispatch, same contract as active_learning/src/query_strategies/get_strategy.py:
 `get_strategy(name)` returns the class called `name`.  Every class name the reference dispatches is implemented: the
 thirteen accelerated samplers (the seven of the north-star path plus MASE / BASE / Balancing, SURVEY.md section 8f,
-MarginClustering, VAAL and BalancedRandom) and the default RandomSampler.  ProbCoverSampler and TypiClustSampler are this
-project's additions (no reference counterpart; ProbCoverSampler needs the sampler kwarg `delta`)."""
+MarginClustering, VAAL and BalancedRandom) and the default RandomSampler.  ProbCoverSampler, TypiClustSampler and
+CALSampler are this project's additions (no reference counterpart; ProbCoverSampler needs the sampler kwarg `delta`)."""
 from .badge_sampler import BADGESampler  # noqa: F401
 from .balanced_random_sampler import BalancedRandomSampler  # noqa: F401
 from .balancing_sampler import BalancingSampler  # noqa: F401
 from .base_sampler import BASESampler  # noqa: F401
+from .cal_sampler import CALSampler  # noqa: F401
 from .confidence_sampler import ConfidenceSampler  # noqa: F401
 from .coreset_sampler import CoresetSampler  # noqa: F401
 from .entropy_sampler import EntropySampler  # noqa: F401
@@ -23,7 +24,7 @@ from .vaal_sampler import VAALSampler  # noqa: F401
 ACCELERATED = ("MarginSampler", "ConfidenceSampler", "EntropySampler", "CoresetSampler",
                "PartitionedCoresetSampler", "BADGESampler", "PartitionedBADGESampler", "MASESampler", "BASESampler",
                "BalancingSampler", "MarginClusteringSampler", "VAALSampler", "BalancedRandomSampler",
-               "ProbCoverSampler", "TypiClustSampler")
+               "ProbCoverSampler", "TypiClustSampler", "CALSampler")
 NOT_ON_THIS_PATH = ()
 
 

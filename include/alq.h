@@ -552,6 +552,27 @@ int alq_kmeans_update(alq_ctx* ctx, const float* xhat, int64_t n, int32_t d, con
 int alq_typicality(alq_ctx* ctx, const float* xhat, int32_t d, const int32_t* rows, const int64_t* group_off_host,
                    int32_t groups, int32_t k_max, double* typ, int32_t* best, void* stream);
 
+/* ---- K18 / K19: CAL (Margatina, Vernikos, Barrault & Aletras, EMNLP 2021) ---------------------------------------------
+ * alq_knn (K18): for every row i of x[n, d], idx[i][0..k) = the k rows j of y[m, d] with the smallest exact fp64
+ *   d2(x_i, y_j) (K7's pair arithmetic on the raw rows: d = a - b, s = s + d * d, k ascending, no FMA), in ascending
+ *   (d2, j) order, and d2[i][0..k) their values.  When m < k the last k - m entries of a row are idx -1, d2 +inf.  The
+ *   pairs are screened on the tensor cores (3xTF32) with a rigorous band (DESIGN section 4); each row keeps 32 candidate
+ *   columns and takes an exact scan of all m rows when they cannot certify its k nearest.  x, y: fp32, contiguous rows
+ *   (pitch d), 16-byte aligned, d % 4 == 0; every squared row norm finite and at most 2^100 (ALQ_ERR_INVALID otherwise).
+ *   idx int32 [n, k], d2 fp64 [n, k], device.  k in [1, 32].  *fallback_rows_host = the rows that took the exact scan.
+ *   Synchronous (two 4-byte copies).
+ * alq_cal_scores (K19): per row r of cand_logits[n, C] and ref_logits[m, C] (fp32, contiguous rows), in fp64:
+ *   lse_r = mx_r + log(sum_c exp(z_rc - mx_r)) (c ascending, mx_r = max_c z_rc), lp_rc = z_rc - lse_r, p_rc = exp(lp_rc).
+ *   For candidate i and each idx[i][j] in [0, m) (other entries are skipped): KL_j = sum_c p_nc (lp_nc - lp_ic),
+ *   c ascending; score[i] = (sum of the KL_j in list order) / (their number), 0 when there is none.  key[i] =
+ *   -fl32(score[i]), +0.0 when fl32(score[i]) is zero and +NaN when score[i] is NaN: alq_select_smallest on key takes the
+ *   largest scores first, the lowest row on ties.  idx int32 [n, k], score fp64 [n], key fp32 [n], device.  k in
+ *   [1, 32].  Asynchronous on `stream`. */
+int alq_knn(alq_ctx* ctx, const float* x, int64_t n, const float* y, int64_t m, int32_t d, int32_t k, int32_t* idx,
+            double* d2, int64_t* fallback_rows_host, void* stream);
+int alq_cal_scores(alq_ctx* ctx, const float* cand_logits, int64_t n, const float* ref_logits, int64_t m, int32_t c,
+                   const int32_t* idx, int32_t k, double* score, float* key, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
