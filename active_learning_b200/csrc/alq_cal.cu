@@ -1,12 +1,12 @@
 // K18 / K19: CALSampler (Margatina, Vernikos, Barrault & Aletras, "Active Learning by Acquiring Contrastive Examples",
 // EMNLP 2021) on the device.
 //
-// K18 alq_knn        idx[i][0..k) = the k rows j of y with the smallest exact fp64 d2(x_i, y_j) in K7's pair arithmetic
-//                    (d = a - b, s = s + d * d, k ascending, no FMA), ascending (d2, j); the raw rows, not normalised.
+// K18 alq_knn        idx[i][0..k) = the k rows j of y with the smallest exact fp64 d2(x_i, y_j) = exact_d2 (K7's pair
+//                    arithmetic, alq_common.cuh), ascending (d2, j) = pair_less; the raw rows, not normalised.
 //   split      x and y through alq_rows_split.cuh's kernel without normalisation: TF32 hi / lo and nrm2 = |row|^2 in fp64;
 //              knn_norms_kernel refuses a squared norm that is not finite or above NRM2_MAX and writes sqrt(nrm2).
 //   screen     one CTA per SM, persistent over 128-row blocks of x; for each, every 128-column tile of y on the ring of
-//              alq_wgmma.cuh (warpgroup 0 the TMA producer, warpgroups 1-2 issue tc::ring_mma).  The epilogue forms
+//              alq_wgmma.cuh (warpgroup 0 runs tc::ring_produce_rows, warpgroups 1-2 tc::ring_tile).  The epilogue forms
 //              d2~ = nrm2_i + nrm2_j - 2 g in fp64 and the band b of DESIGN section 4 (relative to |x_i||y_j| and to
 //              (|x_i| + |y_j|)^2), and each row keeps in shared memory the S smallest lower bounds L = d2~ - b (rounded
 //              down to fp32) with their columns, and L* = the smallest lower bound it dropped.  The four lanes holding a
@@ -119,13 +119,7 @@ knn_screen_kernel(const __grid_constant__ CUtensorMap map_xhi, const __grid_cons
 
     if (me.wg == 0) {
         tc::producer_regs();
-        if (threadIdx.x == 0) {
-            uint32_t it = 0;
-            for (int rb = blockIdx.x; rb < P.rblocks; rb += gridDim.x)
-                for (int ct = 0; ct < P.ctiles; ++ct)
-                    for (int kb = 0; kb < P.kblocks; ++kb, ++it)
-                        tc::ring_load(ring, it, &map_xhi, &map_xlo, rb * BM, &map_yhi, &map_ylo, ct * BM, kb * BK);
-        }
+        if (threadIdx.x == 0) tc::ring_produce_rows(ring, &map_xhi, &map_xlo, &map_yhi, &map_ylo, P.rblocks, P.ctiles, P.kblocks);
         return;
     }
     tc::consumer_regs();
@@ -152,9 +146,7 @@ knn_screen_kernel(const __grid_constant__ CUtensorMap map_xhi, const __grid_cons
         float ls[2] = {INFINITY, INFINITY};
         for (int ct = 0; ct < P.ctiles; ++ct) {
             float acc[64];
-            int prev = -1;
-            for (int kb = 0; kb < P.kblocks; ++kb, ++it) tc::ring_mma(ring, it, me.a_off, acc, kb == 0, prev, me.t);
-            tc::ring_drain(ring, prev, me.t);
+            tc::ring_tile(ring, it, me, acc, P.kblocks);
             // acc becomes the lower bounds L, rounded down to fp32; columns past m get +inf and are never kept
             float lo = INFINITY;
 #pragma unroll
@@ -226,29 +218,6 @@ knn_screen_kernel(const __grid_constant__ CUtensorMap map_xhi, const __grid_cons
         }
         __syncwarp();
     }
-}
-
-__device__ __forceinline__ bool pair_less(double a, int ca, double b, int cb) {
-    return a < b || (a == b && ca < cb);
-}
-
-// the exact d2 of rows a and b (16-byte aligned, d % 4 == 0): K7's sequential chain
-__device__ __forceinline__ double exact_d2(const float* __restrict__ a, const float* __restrict__ b, int d) {
-    const float4* a4 = reinterpret_cast<const float4*>(a);
-    const float4* b4 = reinterpret_cast<const float4*>(b);
-    double s = 0.0;
-    for (int k = 0; k < d / 4; ++k) {
-        const float4 u = __ldg(a4 + k), v = __ldg(b4 + k);
-        double df = __dsub_rn(static_cast<double>(u.x), static_cast<double>(v.x));
-        s = __dadd_rn(s, __dmul_rn(df, df));
-        df = __dsub_rn(static_cast<double>(u.y), static_cast<double>(v.y));
-        s = __dadd_rn(s, __dmul_rn(df, df));
-        df = __dsub_rn(static_cast<double>(u.z), static_cast<double>(v.z));
-        s = __dadd_rn(s, __dmul_rn(df, df));
-        df = __dsub_rn(static_cast<double>(u.w), static_cast<double>(v.w));
-        s = __dadd_rn(s, __dmul_rn(df, df));
-    }
-    return s;
 }
 
 constexpr int RECHECK_WARPS = 8;
@@ -472,11 +441,10 @@ extern "C" int alq_knn(alq_ctx* ctx, const float* x, int64_t n, const float* y, 
     ScreenParams P{};
     P.nx = nx; P.sx = sx; P.ny = ny; P.sy = sy;
     P.n = ni; P.m = mi; P.ctiles = (mi + BM - 1) / BM; P.kblocks = (d + BK - 1) / BK; P.rblocks = (ni + BM - 1) / BM;
-    // DESIGN section 4: |g - <x, y>| <= (1 + 3 ceil(d / 8)) 2^-20 |x||y|, d2~ carries twice that (the 1e-6 covers the fp64
-    // |x| |y|); the fp64 roundings of the norms, of the epilogue and of the exact sum are < (2d + 13) 2^-53 (|x| + |y|)^2,
-    // of which the band takes twice; flushed or underflowing TF32 operands and products move 2g by < 2^-118 d (1 + |x| +
-    // |y|), of which it takes 2^18 times.
-    P.coef = 2.0 * (1.0 + 3.0 * ((d + 7) / 8)) * ldexp(1.0, -20) * (1.0 + 1e-6);
+    // DESIGN section 4: the fp64 roundings of the norms, of the epilogue and of the exact sum are < (2d + 13) 2^-53
+    // (|x| + |y|)^2, of which the band takes twice; flushed or underflowing TF32 operands and products move 2g by
+    // < 2^-118 d (1 + |x| + |y|), of which it takes 2^18 times.
+    P.coef = tc::band_coef(d);
     P.rel = (4.0 * d + 32.0) * ldexp(1.0, -53);
     P.abs_ = d * ldexp(1.0, -100);
     P.cand = cand; P.lstar = lstar;

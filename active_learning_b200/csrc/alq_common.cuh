@@ -367,4 +367,30 @@ __device__ __forceinline__ void alq_bitonic_sort_smem(unsigned long long* sk, in
     }
 }
 
+// ---- K7's pair arithmetic: scipy's euclidean on fp32 rows, the exact d2 of every kernel that certifies distances ----
+// (K7, K13's recheck, K15's recheck, K17, K18's recheck and fallback; the NumPy statement is probcover_oracle.exact_d2)
+// one step: the fp32 entries widened to fp64 (exact), d = a - b, s + d * d, each operation rounded on its own (no FMA)
+__device__ __forceinline__ double d2_step(double s, double a, double b) {
+    const double df = __dsub_rn(a, b);
+    return __dadd_rn(s, __dmul_rn(df, df));
+}
+// the whole chain over rows a and b, k ascending (16-byte aligned, d % 4 == 0)
+__device__ __forceinline__ double exact_d2(const float* __restrict__ a, const float* __restrict__ b, int d) {
+    const float4* a4 = reinterpret_cast<const float4*>(a);
+    const float4* b4 = reinterpret_cast<const float4*>(b);
+    double s = 0.0;
+    for (int k = 0; k < d / 4; ++k) {
+        const float4 u = __ldg(a4 + k), v = __ldg(b4 + k);
+        s = d2_step(s, u.x, v.x);
+        s = d2_step(s, u.y, v.y);
+        s = d2_step(s, u.z, v.z);
+        s = d2_step(s, u.w, v.w);
+    }
+    return s;
+}
+// the ascending (d2, index) order: ties to the lower index
+__device__ __forceinline__ bool pair_less(double a, int ca, double b, int cb) {
+    return a < b || (a == b && ca < cb);
+}
+
 static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }

@@ -1,18 +1,18 @@
 // K13 / K14: ProbCoverSampler (Yehuda et al., "Active Learning Through a Covering Lens", NeurIPS 2022) on the device.
 //
 // K13 alq_probcover_graph   the delta-ball graph of the L2-normalised pool rows as CSR.  There is an edge (i, j) iff
-//                           scipy's fp64 euclidean distance of the fp32 rows (K7's per-pair arithmetic) is < delta.
+//                           scipy's fp64 euclidean distance of the fp32 rows (d2_step, K7's pair arithmetic) is < delta.
 //   normalise  one warp per row (alq_rows_split.cuh, shared with K15): lane-strided fp64 sum of squares, a butterfly,
 //              norm = sqrt, xhat = fl32(x / norm) (a zero row stays zero); the same kernel splits xhat into TF32 hi / lo
 //              (alq_wgmma.cuh) and stores nrm2 = |xhat|^2 in fp64.
 //   screen     one CTA per SM, persistent over the upper-triangle 128 x 128 tiles of xhat xhat^T, on the ring of
-//              alq_wgmma.cuh that K3 and K9 use: warpgroup 0 is the TMA producer (3-stage ring), warpgroups 1-2 issue
-//              the 3xTF32 chain tc::ring_mma.  The epilogue decides each pair from d2 = nrm2_i + nrm2_j - 2 g
-//              (g the tensor-core dot product) against the bound
+//              alq_wgmma.cuh: warpgroup 0 is the TMA producer (3-stage ring, its own loop over the triangle), warpgroups
+//              1-2 issue the 3xTF32 chain tile by tile (tc::ring_tile).  The epilogue decides each pair from
+//              d2 = nrm2_i + nrm2_j - 2 g (g the tensor-core dot product) against the bound
 //              |g - <xhat_i, xhat_j>| <= E_ij of DESIGN section 4: clearly inside delta^2 is an edge, clearly outside is
-//              not, and a pair inside the band is recomputed exactly with K7's arithmetic.  A pair is decided once per
-//              tile, so (i, j) and (j, i) of an off-diagonal tile share one decision; on a diagonal tile both orders are
-//              decided separately and agree because every decision equals the exact one.
+//              not, and a pair inside the band is recomputed exactly with d2_step (K7's pair arithmetic).  A pair is
+//              decided once per tile, so (i, j) and (j, i) of an off-diagonal tile share one decision; on a diagonal
+//              tile both orders are decided separately and agree because every decision equals the exact one.
 //   CSR        the tile's decisions go into a 128 x 128 bitmap in shared memory.  Thread t of the consumers then owns
 //              tile row t (the edges (i, j), j in the column block) and, on an off-diagonal tile, thread 128 + t owns
 //              tile column t (the mirrored edges (j, i)).  Count pass: the number of edges of every (row, column block)
@@ -67,15 +67,14 @@ __device__ __forceinline__ void tile_of(long long idx, int nt, int& ti, int& tj)
     tj = static_cast<int>(t + (idx - tri_off(t, nt)));
 }
 
-// K7's pair arithmetic (scipy's euclidean on fp32 rows): d = a - b in fp64, s = s + d * d, k ascending, no FMA
+// scipy's euclidean on the fp32 rows: d2_step (K7's pair arithmetic), k ascending.  Out of line, because the screen's
+// epilogue sits at the 168-register cap; scalar loads, because ptxas allocates the caller around this function's
+// registers, and exact_d2's float4 loads would re-lay out the whole screen.
 __device__ __noinline__ bool exact_edge(const float* __restrict__ xhat, int d, int i, int j, double delta) {
     const float* a = xhat + static_cast<size_t>(i) * d;
     const float* b = xhat + static_cast<size_t>(j) * d;
     double s = 0.0;
-    for (int k = 0; k < d; ++k) {
-        const double df = __dsub_rn(static_cast<double>(__ldg(a + k)), static_cast<double>(__ldg(b + k)));
-        s = __dadd_rn(s, __dmul_rn(df, df));
-    }
+    for (int k = 0; k < d; ++k) s = d2_step(s, __ldg(a + k), __ldg(b + k));
     return __dsqrt_rn(s) < delta;
 }
 
@@ -119,9 +118,7 @@ pc_graph_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constan
         int ti, tj;
         tile_of(idx, nt, ti, tj);
         float acc[64];
-        int prev = -1;
-        for (int kb = 0; kb < P.kblocks; ++kb, ++it) tc::ring_mma(ring, it, me.a_off, acc, kb == 0, prev, me.t);
-        tc::ring_drain(ring, prev, me.t);
+        tc::ring_tile(ring, it, me, acc, P.kblocks);
 
         // ---- epilogue: the decisions of this thread's 2 x 32 pairs as canonical column masks of its two rows
         const int row0 = ti * BM + me.r_in_tile, row1 = row0 + 8;
@@ -363,8 +360,7 @@ extern "C" int alq_probcover_graph(alq_ctx* ctx, const float* x, int64_t n, int3
     P.tile_pairs = static_cast<long long>(nt) * (nt + 1) / 2;
     P.delta = *delta_host;
     P.delta2 = P.delta * P.delta;
-    // DESIGN section 4: |g - <xhat_i, xhat_j>| <= (1 + 3 ceil(d / 8)) 2^-20 sqrt(nrm2_i nrm2_j); d2 carries twice that
-    P.coef = 2.0 * (1.0 + 3.0 * ((d + 7) / 8)) * ldexp(1.0, -20) * (1.0 + 1e-6);
+    P.coef = tc::band_coef(d);
     P.slack = 1e-9 * P.delta2 + 1e-10;
     P.tile_cnt = tile_cnt; P.row_ptr = reinterpret_cast<const long long*>(row_ptr); P.cols = cols;
     P.recheck = rech; P.fill = fill ? 1 : 0;

@@ -2,18 +2,18 @@
 //
 // alq_kmeans_rows       the pool rows L2-normalised (K13's normalise, alq_rows_split.cuh) and split into TF32 hi / lo
 //                       with their fp64 squared norms, once per k-means.
-// K15 alq_kmeans_assign label_i = the exact fp64 argmin over the centres c of d2(xhat_i, c) in K7's pair arithmetic
-//                       (d = a - b, s = s + d * d, k ascending, no FMA), ties to the lowest centre.
+// K15 alq_kmeans_assign label_i = the exact fp64 argmin over the centres c of d2(xhat_i, c) = exact_d2 (K7's pair
+//                       arithmetic, alq_common.cuh), ties to the lowest centre.
 //   split      the centres [K, d] through the same kernel (no normalisation): hi / lo and cn = |c|^2 in fp64.
 //   screen     one CTA per SM, persistent over 128-row blocks; for each, every 128-centre tile on the ring of
-//              alq_wgmma.cuh (warpgroup 0 the TMA producer, warpgroups 1-2 issue tc::ring_mma).  The epilogue forms
-//              d2~ = nrm2_i + cn_c - 2 g in fp64 and the band b = coef sqrt(nrm2_i) sqrt(cn_c) + slack of DESIGN
-//              section 4, and keeps per row U = min_c (d2~ + b) and the two smallest lower bounds L1 (at c1) <= L2 of
-//              d2~ - b.  The four lanes holding a row's columns merge their states; if L2 > U every other centre is
+//              alq_wgmma.cuh (warpgroup 0 runs tc::ring_produce_rows, warpgroups 1-2 tc::ring_tile).  The epilogue
+//              forms d2~ = nrm2_i + cn_c - 2 g in fp64 and the band b = band_coef(d) sqrt(nrm2_i) sqrt(cn_c) + slack of
+//              DESIGN section 4, and keeps per row U = min_c (d2~ + b) and the two smallest lower bounds L1 (at c1) <= L2
+//              of d2~ - b.  The four lanes holding a row's columns merge their states; if L2 > U every other centre is
 //              strictly farther than c1 and the label is c1, otherwise the row goes on the recheck list.  n x K is never
 //              formed.
-//   recheck    a warp per listed row: the exact fp64 d2 to ALL K centres, lane-strided over the centres, the (d2,
-//              centre) minimum over the warp.
+//   recheck    a warp per listed row: exact_d2 to ALL K centres, lane-strided over the centres, the (d2, centre)
+//              minimum (pair_less) over the warp.
 //   Returns the rows whose label changed and the rows rechecked, in one 8-byte copy.
 // K16 alq_kmeans_update centre_c = fl32(S_c / m_c), S_c the fp64 sum of the member rows in ascending row order, one
 //              sequential chain per column.  A stable counting sort of the rows by label (per-chunk histograms, a scan,
@@ -23,8 +23,7 @@
 //              per row the k = min(k_max, m / 2) smallest exact fp64 d2 to the OTHER rows of its group (excluded by
 //              position, so a duplicate row counts with d2 = 0), their ascending fp64 sum / k = mean, typicality =
 //              1 / (mean + 1e-5), and per group the argmax (lowest position on ties).  64 x 64 block-diagonal tiles of
-//              K7's arithmetic; each warp keeps the sorted 32 smallest of its rows across the lanes.  m x m is never
-//              formed.
+//              d2_step; each warp keeps the sorted 32 smallest of its rows across the lanes.  m x m is never formed.
 #include <math.h>
 
 #include <algorithm>
@@ -80,13 +79,7 @@ km_assign_kernel(const __grid_constant__ CUtensorMap map_xhi, const __grid_const
 
     if (me.wg == 0) {
         tc::producer_regs();
-        if (threadIdx.x == 0) {
-            uint32_t it = 0;
-            for (int rb = blockIdx.x; rb < P.rblocks; rb += gridDim.x)
-                for (int ct = 0; ct < P.ctiles; ++ct)
-                    for (int kb = 0; kb < P.kblocks; ++kb, ++it)
-                        tc::ring_load(ring, it, &map_xhi, &map_xlo, rb * BM, &map_chi, &map_clo, ct * BM, kb * BK);
-        }
+        if (threadIdx.x == 0) tc::ring_produce_rows(ring, &map_xhi, &map_xlo, &map_chi, &map_clo, P.rblocks, P.ctiles, P.kblocks);
         return;
     }
     tc::consumer_regs();
@@ -99,9 +92,7 @@ km_assign_kernel(const __grid_constant__ CUtensorMap map_xhi, const __grid_const
         Near a{INFINITY, INFINITY, INFINITY, 0x7fffffff}, b{INFINITY, INFINITY, INFINITY, 0x7fffffff};
         for (int ct = 0; ct < P.ctiles; ++ct) {
             float acc[64];
-            int prev = -1;
-            for (int kb = 0; kb < P.kblocks; ++kb, ++it) tc::ring_mma(ring, it, me.a_off, acc, kb == 0, prev, me.t);
-            tc::ring_drain(ring, prev, me.t);
+            tc::ring_tile(ring, it, me, acc, P.kblocks);
 #pragma unroll
             for (int j = 0; j < 16; ++j) {
 #pragma unroll
@@ -154,19 +145,14 @@ km_recheck_kernel(const float* __restrict__ xhat, const float* __restrict__ cen,
         double best = INFINITY;
         int bc = 0x7fffffff;
         for (int c = lane; c < K; c += 32) {            // ascending per lane: a strict < keeps the lowest centre
-            const float* q = cen + static_cast<size_t>(c) * d;
-            double s = 0.0;
-            for (int k = 0; k < d; ++k) {
-                const double df = __dsub_rn(static_cast<double>(__ldg(a + k)), static_cast<double>(__ldg(q + k)));
-                s = __dadd_rn(s, __dmul_rn(df, df));
-            }
+            const double s = exact_d2(a, cen + static_cast<size_t>(c) * d, d);
             if (s < best) { best = s; bc = c; }
         }
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) {
             const double ob = __shfl_xor_sync(0xffffffffu, best, o);
             const int oc = __shfl_xor_sync(0xffffffffu, bc, o);
-            if (ob < best || (ob == best && oc < bc)) { best = ob; bc = oc; }
+            if (pair_less(ob, oc, best, bc)) { best = ob; bc = oc; }
         }
         if (lane == 0 && labels[row] != bc) {
             labels[row] = bc;
@@ -332,10 +318,7 @@ __global__ void __launch_bounds__(TYP_THREADS) km_typ_kernel(const TypArgs A) {
 #pragma unroll
                 for (int q = 0; q < 4; ++q)
 #pragma unroll
-                    for (int r = 0; r < 4; ++r) {
-                        const double df = __dsub_rn(a[q], b[r]);
-                        acc[q][r] = __dadd_rn(acc[q][r], __dmul_rn(df, df));
-                    }
+                    for (int r = 0; r < 4; ++r) acc[q][r] = d2_step(acc[q][r], a[q], b[r]);
             }
             __syncthreads();
         }
@@ -426,8 +409,9 @@ extern "C" int alq_kmeans_assign(alq_ctx* ctx, const float* xhat, const float* h
     if (n < 1 || n >= (1LL << 31)) ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_kmeans_assign: n=%lld outside [1, 2^31)", (long long)n);
     if (d < 4 || d % 4) ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_kmeans_assign: d=%d must be a positive multiple of 4", d);
     if (k < 1 || k > K_MAX) ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_kmeans_assign: K=%d outside [1, %d]", k, K_MAX);
-    if (!xhat || !hi || !lo || !nrm2 || !centres || !labels || !counts_host || !aligned16(hi) || !aligned16(lo))
-        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_kmeans_assign: null pointer or hi / lo not 16-byte aligned");
+    if (!xhat || !hi || !lo || !nrm2 || !centres || !labels || !counts_host || !aligned16(xhat) || !aligned16(hi) ||
+        !aligned16(lo))
+        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_kmeans_assign: null pointer or xhat / hi / lo not 16-byte aligned");
     if (!tc::get_encode()) ALQ_FAIL(ctx, ALQ_ERR_CUDA, "alq_kmeans_assign: cuTensorMapEncodeTiled is unavailable");
     const cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int ni = static_cast<int>(n);
@@ -455,10 +439,9 @@ extern "C" int alq_kmeans_assign(alq_ctx* ctx, const float* xhat, const float* h
     AssignParams P{};
     P.nrm2 = nrm2; P.cn = cn;
     P.n = ni; P.K = k; P.ctiles = (k + BM - 1) / BM; P.kblocks = (d + BK - 1) / BK; P.rblocks = (ni + BM - 1) / BM;
-    // DESIGN section 4: |g - <xhat_i, c>| <= (1 + 3 ceil(d / 8)) 2^-20 |xhat_i| |c|; d2 carries twice that.  The 1e-6
-    // covers sqrt(nrm2_i) sqrt(cn_c) in place of sqrt(nrm2_i cn_c); the slack the fp64 epilogue (d2 <= 4) and the
-    // exact sum's own rounding (d 2^-53 of at most 4).
-    P.coef = 2.0 * (1.0 + 3.0 * ((d + 7) / 8)) * ldexp(1.0, -20) * (1.0 + 1e-6);
+    // DESIGN section 4: the slack covers the fp64 epilogue (d2 <= 4) and the exact sum's own rounding (d 2^-53 of at
+    // most 4)
+    P.coef = tc::band_coef(d);
     P.slack = 1e-9;
     P.labels = labels; P.list = list; P.counts = cnt;
     const size_t smem = tc::ring_smem_bytes(0);

@@ -2,8 +2,9 @@
 // reference's query_strategies):  p[i] = sigmoid(w3 . relu(W2 relu(W1 mu_i + b1) + b2) + b3),  hidden width 512.
 //
 // Two launches of one kernel template per pool slice of at most SLICE_ROWS rows, both on the ring of alq_wgmma.cuh
-// that K3 and K13 use: a one-thread TMA producer warpgroup feeding a 3-stage SWIZZLE_128B ring, two consumer
-// warpgroups issuing the 3xTF32 chain tc::ring_mma (hi*hi' + hi*lo' + lo*hi', operands split ahead of time).
+// that K3, K13, K15 and K18 use: a one-thread TMA producer warpgroup (tc::ring_produce_rows) feeding a 3-stage
+// SWIZZLE_128B ring, two consumer warpgroups issuing the 3xTF32 chain tile by tile (tc::ring_tile: hi*hi' + hi*lo' +
+// lo*hi', operands split ahead of time).
 //   layer 1  X = mu [rows, z] (z zero-padded to a multiple of 32), Y = W1 [512, z].  Epilogue: relu(acc + b1),
 //            stored as the TF32 hi/lo pair layer 2 reads, so the [rows, 512] intermediate needs no split pass.
 //   layer 2  X = H1 [rows, 512], Y = W2 [512, 512].  Epilogue: relu(acc + b2_j) * w3_j summed over all 512
@@ -41,13 +42,7 @@ vaal_layer_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_const
 
     if (me.wg == 0) {
         producer_regs();
-        if (threadIdx.x == 0) {
-            uint32_t it = 0;
-            for (int mb = blockIdx.x; mb < m_blocks; mb += gridDim.x)
-                for (int nt = 0; nt < NT; ++nt)
-                    for (int kb = 0; kb < P.kblocks; ++kb, ++it)
-                        ring_load(ring, it, &map_xh, &map_xl, mb * BM, &map_yh, &map_yl, nt * BN, kb * BK);
-        }
+        if (threadIdx.x == 0) ring_produce_rows(ring, &map_xh, &map_xl, &map_yh, &map_yl, m_blocks, NT, P.kblocks);
     } else {
         consumer_regs();
         uint32_t it = 0;
@@ -56,9 +51,7 @@ vaal_layer_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_const
             float s0 = 0.f, s1 = 0.f;                 // layer 2: this thread's share of the w3 dot product
             for (int nt = 0; nt < NT; ++nt) {
                 float acc[64];
-                int prev = -1;
-                for (int kb = 0; kb < P.kblocks; ++kb, ++it) ring_mma(ring, it, me.a_off, acc, kb == 0, prev, me.t);
-                ring_drain(ring, prev, me.t);
+                ring_tile(ring, it, me, acc, P.kblocks);
 #pragma unroll
                 for (int j = 0; j < 16; ++j) {
                     const int col = nt * BN + 8 * j + me.c_in_tile;

@@ -3,7 +3,8 @@
 // sklearn.cluster.AgglomerativeClustering(n_clusters=20), i.e. scipy.cluster.hierarchy.ward over the full tree).
 //
 // K7 alq_pdist_f64   scipy's pdist(X, 'euclidean') in fp64: fp32 rows widened to fp64 (exact), s summed k = 0, 1, ...
-//                    as `d = a - b; s = s + d*d` with no FMA, then sqrt(s).  Two layouts of the result (below).
+//                    by d2_step (alq_common.cuh: `d = a - b; s = s + d*d` with no FMA), then sqrt(s).  Two layouts of
+//                    the result (below).
 //                    One CTA owns a 64 x 64 tile of pairs of the upper triangle (each pair computed once; written to
 //                    (i, j) and (j, i) of the square matrix, or once to the condensed vector);
 //                    256 threads x 4 x 4 pairs in registers; k-chunks of both row blocks arrive
@@ -195,10 +196,7 @@ pdist_f64_kernel(const float* __restrict__ x, int n, int d, int64_t ldx, double*
 #pragma unroll
             for (int a = 0; a < 4; ++a)
 #pragma unroll
-                for (int b = 0; b < 4; ++b) {
-                    const double df = __dsub_rn(av[a], bv[b]);
-                    acc[a][b] = __dadd_rn(acc[a][b], __dmul_rn(df, df));
-                }
+                for (int b = 0; b < 4; ++b) acc[a][b] = d2_step(acc[a][b], av[a], bv[b]);
         }
     }
 #pragma unroll

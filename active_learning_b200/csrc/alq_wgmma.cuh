@@ -1,7 +1,8 @@
 // The Hopper 3xTF32 tile pipeline of the wgmma kernels (K3 in alq_mindist_tc.cu, K9 in alq_vaal.cu, K13 in
-// alq_probcover.cu): TMA tile loads, SWIZZLE_128B shared-memory descriptors, the m64n128k8 TF32 MMA, the host-side
-// tensor-map encoder, and the ring that connects them.  Operands are fp32 rows already split into TF32 hi/lo pairs; a
-// stage row is BK = 32 fp32 = 128 bytes, one swizzle span.
+// alq_probcover.cu, K15 in alq_typiclust.cu, K18 in alq_cal.cu): TMA tile loads, SWIZZLE_128B shared-memory
+// descriptors, the m64n128k8 TF32 MMA, the host-side tensor-map encoder, the ring that connects them, and the
+// coefficient of the chain's error bound.  Operands are fp32 rows already split into TF32 hi/lo pairs; a stage row is
+// BK = 32 fp32 = 128 bytes, one swizzle span.
 //
 // The ring (one CTA per SM, 3 warpgroups):
 //   warpgroup 0    TMA producer (one thread): per k-block, the hi and lo boxes of a 128-row block of X and of a
@@ -9,9 +10,12 @@
 //   warpgroups 1-2 consumers: each owns 64 of the tile's 128 rows and issues hi*hi' + hi*lo' + lo*hi' per 8-wide
 //                  k-step, k ascending, into one m64n128 fp32 register fragment (ring_mma), keeping one stage in
 //                  flight and handing the previous one back on `empty`.
-// Each kernel keeps its own work schedule and epilogue; the producer and the consumers walk the same sequence of
-// k-blocks, counted by `it`.  K3, K9 and K13 all issue this one chain, so the 3xTF32 error bound of DESIGN section 4,
-// measured through K3, holds for all three.
+// The producer and the consumers walk the same sequence of k-blocks, counted by `it`.  K9, K15 and K18 run the
+// row-block schedule: ring_produce_rows on the producer, ring_tile per tile on the consumers.  K13 keeps its own
+// producer loop over the upper-triangle tiles and consumes each tile with ring_tile.  K3 keeps both loops (its factored
+// form switches accumulators inside a tile) around ring_load, ring_mma and ring_drain.  Each kernel keeps its own
+// epilogue.  All five issue this one chain, so the 3xTF32 error bound of DESIGN section 4 (band_coef), measured
+// through K3, holds for all of them.
 #pragma once
 #include <cuda.h>
 
@@ -175,6 +179,30 @@ __device__ __forceinline__ void ring_drain(const Ring& r, int prev, int t) {
     wgmma_wait<0>();
     if (prev >= 0 && t == 0) mbar_arrive(&r.empty[prev]);
 }
+
+// Consumer, one 128 x 128 tile: its `kblocks` k-blocks from `it` on through ring_mma (acc overwritten), then ring_drain.
+__device__ __forceinline__ void ring_tile(const Ring& r, uint32_t& it, const Role& me, float (&acc)[64], int kblocks) {
+    int prev = -1;
+    for (int kb = 0; kb < kblocks; ++kb, ++it) ring_mma(r, it, me.a_off, acc, kb == 0, prev, me.t);
+    ring_drain(r, prev, me.t);
+}
+
+// Producer thread of the row-block schedule: the CTA's 128-row blocks of X rb = blockIdx.x, blockIdx.x + gridDim.x, ...
+// below `rblocks`, for each every 128-row tile of Y ct = 0 .. ctiles - 1, for each its k-blocks.  The consumers walk
+// the same sequence: per row block, one ring_tile per ct in ascending order.
+__device__ __forceinline__ void ring_produce_rows(const Ring& r, const CUtensorMap* x_hi, const CUtensorMap* x_lo,
+                                                  const CUtensorMap* y_hi, const CUtensorMap* y_lo, int rblocks,
+                                                  int ctiles, int kblocks) {
+    uint32_t it = 0;
+    for (int rb = blockIdx.x; rb < rblocks; rb += gridDim.x)
+        for (int ct = 0; ct < ctiles; ++ct)
+            for (int kb = 0; kb < kblocks; ++kb, ++it) ring_load(r, it, x_hi, x_lo, rb * BM, y_hi, y_lo, ct * BN, kb * BK);
+}
+
+// DESIGN section 4: ring_mma's chain over d columns gives |g - <x, y>| <= (1 + 3 ceil(d / 8)) 2^-20 |x||y|.  A d2
+// formed as nrm2_x + nrm2_y - 2g carries twice that; the 1e-6 covers |x||y| formed in fp64 from the norms.  The band of
+// K13, K15 and K18 is band_coef(d) |x||y| plus each kernel's own slack for its fp64 terms.
+inline double band_coef(int d) { return 2.0 * (1.0 + 3.0 * ((d + 7) / 8)) * ldexp(1.0, -20) * (1.0 + 1e-6); }
 
 using EncodeFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                               const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,

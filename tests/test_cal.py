@@ -91,17 +91,6 @@ def test_band_holds_for_unnormalised_rows(d):
         assert (np.abs(CO.screen_d2(nx[i], ny[j], g) - e) <= b).all(), adder
 
 
-def test_the_knn_kernel_issues_only_the_rings_chain():
-    """K18's screen rests on the 3xTF32 bound measured through K3, so it may issue no MMA, TMA load or barrier of its own."""
-    path = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "active_learning_b200", "csrc",
-                        "alq_cal.cu")
-    with open(path) as f:
-        src = f.read()
-    assert "ring_mma(" in src
-    for own in ("wgmma_tf32(", "tma_load_2d(", "mbar_init("):
-        assert own not in src, own
-
-
 def test_score_keys_and_order():
     """A zero score's key is +0.0, so zero scores tie by position; NaN sorts last; larger scores come first."""
     s = np.array([0.0, 1.5, 0.0, np.nan, 1.5, 2.0, -0.0])

@@ -215,6 +215,10 @@ def test_errors_are_clean_and_leave_the_context_usable(eng):
         eng.typicality(xhat, rows, [0, 0, 300], 20)                      # an empty group
     with pytest.raises(ValueError):
         eng.kmeans(xhat, 0, np.zeros(300), 301)
+    shifted = torch.empty(300 * 16 + 1, device="cuda")[1:].view(300, 16)   # contiguous, 4 bytes off 16-byte alignment
+    shifted.copy_(xhat)
+    with pytest.raises(AlqError, match="xhat / hi / lo not 16-byte aligned"):
+        eng.kmeans_assign(shifted, xhat[:20].clone())                    # K15's recheck reads xhat as float4
     typ, best = eng.typicality(xhat, rows, [0, 300], 32)
     want = T.typicality(xhat.cpu().numpy(), np.arange(300), 32)
     assert typ.cpu().numpy().tolist() == want.tolist() and best[0] == int(np.argmax(want))

@@ -123,18 +123,6 @@ def test_the_adder_models_are_exact_on_tf32_integers_and_differ_elsewhere():
     assert (P.emulate_3xtf32(fam, fam[::-1], adder="align", bits=21) != g["align"]).any()
 
 
-def test_the_tensor_core_kernels_issue_only_the_rings_chain():
-    """test_gpu_tf32_bound.py measures the bound through K3 and applies it to K13 (and DESIGN section 4 to K9) because all
-    three issue one chain: alq_wgmma.cuh's tc::ring_mma.  None of them may issue MMAs, TMA loads or barriers of its own."""
-    csrc = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "active_learning_b200", "csrc")
-    for name in ("alq_mindist_tc.cu", "alq_vaal.cu", "alq_probcover.cu"):
-        with open(os.path.join(csrc, name)) as f:
-            src = f.read()
-        assert "ring_mma(" in src, name
-        for own in ("wgmma_tf32(", "tma_load_2d(", "mbar_init("):
-            assert own not in src, (name, own)
-
-
 # ---- the sampler's host logic ------------------------------------------------------------------------------------------
 class ProbCoverEngine(OracleEngine):
     """The oracle engine plus K13 / K14 by the NumPy statement; counts the graph builds."""

@@ -108,17 +108,6 @@ def test_assign_band_holds_for_centres_inside_the_unit_ball(d):
         assert (c1[ok] == want[ok]).all() and ok.any()
 
 
-def test_the_assignment_kernel_issues_only_the_rings_chain():
-    """K15's screen rests on the 3xTF32 bound measured through K3, so it may issue no MMA, TMA load or barrier of its own."""
-    path = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "active_learning_b200", "csrc",
-                        "alq_typiclust.cu")
-    with open(path) as f:
-        src = f.read()
-    assert "ring_mma(" in src
-    for own in ("wgmma_tf32(", "tma_load_2d(", "mbar_init("):
-        assert own not in src, own
-
-
 # ---- the sampler's host logic ------------------------------------------------------------------------------------------
 class TypiClustEngine(OracleEngine):
     """The oracle engine plus normalize / kmeans / typicality by the NumPy statement; records each K."""
