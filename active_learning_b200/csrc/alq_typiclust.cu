@@ -5,6 +5,8 @@
 // K15 alq_kmeans_assign label_i = the exact fp64 argmin over the centres c of d2(xhat_i, c) = exact_d2 (K7's pair
 //                       arithmetic, alq_common.cuh), ties to the lowest centre.
 //   split      the centres [K, d] through the same kernel (no normalisation): hi / lo and cn = |c|^2 in fp64.
+//   domain     km_domain_kernel counts the rows and centres whose squared norm is not in [0, 2] (the band's slack is
+//              absolute, DESIGN section 4) and the call refuses them by name before the screen (one 4-byte copy).
 //   screen     one CTA per SM, persistent over 128-row blocks; for each, every 128-centre tile on the ring of
 //              alq_wgmma.cuh (warpgroup 0 runs tc::ring_produce_rows, warpgroups 1-2 tc::ring_tile).  The epilogue
 //              forms d2~ = nrm2_i + cn_c - 2 g in fp64 and the band b = band_coef(d) sqrt(nrm2_i) sqrt(cn_c) + slack of
@@ -37,6 +39,7 @@ namespace tk {
 using tc::BK;
 using tc::BM;
 constexpr int K_MAX = 8192;                     // K16's histogram lives in shared memory
+constexpr double NRM2_MAX = 2.0;                // the band's absolute slack is derived for squared norms in [0, 2]
 
 // ---- K15 ---------------------------------------------------------------------------------------------------------------
 struct AssignParams {
@@ -49,6 +52,16 @@ struct AssignParams {
     int* list;                         // [n] the rows left to the exact recheck
     unsigned int* counts;              // [0] labels changed, [1] rows listed
 };
+
+// rows (nrm2) and centres (cn) whose squared norm lies outside [0, NRM2_MAX], NaN and infinity included, are counted in
+// *bad
+__global__ void __launch_bounds__(256) km_domain_kernel(const double* __restrict__ nrm2, int n, const double* __restrict__ cn,
+                                                        int k, unsigned int* bad) {
+    const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (i >= static_cast<long long>(n) + k) return;
+    const double v = i < n ? nrm2[i] : cn[i - n];
+    if (!(v >= 0.0 && v <= NRM2_MAX)) atomicAdd(bad, 1u);
+}
 
 // the two smallest lower bounds (l1 at c1, then l2) and the smallest upper bound u of a row
 struct Near {
@@ -417,7 +430,7 @@ extern "C" int alq_kmeans_assign(alq_ctx* ctx, const float* xhat, const float* h
     const int ni = static_cast<int>(n);
     const size_t ce = static_cast<size_t>(k) * d;
     int rc = alq_scratch_reserve(ctx, scratch_need({ce * 4, ce * 4, ce * 4, static_cast<size_t>(k) * 8,
-                                                    static_cast<size_t>(n) * 4, 8}));
+                                                    static_cast<size_t>(n) * 4, 12}));
     if (rc) return rc;
     ScratchCursor cur(ctx->scratch);
     float* chi = cur.take<float>(ce);
@@ -425,12 +438,21 @@ extern "C" int alq_kmeans_assign(alq_ctx* ctx, const float* xhat, const float* h
     float* cc = cur.take<float>(ce);                   // the centres' copy the split reads back
     double* cn = cur.take<double>(k);
     int* list = cur.take<int>(n);
-    unsigned int* cnt = cur.take<unsigned int>(2);
+    unsigned int* cnt = cur.take<unsigned int>(3);     // [0] labels changed, [1] rows listed, [2] norms refused
     ALQ_CUDA(ctx, cudaMemcpyAsync(cc, centres, ce * 4, cudaMemcpyDeviceToDevice, st));
-    ALQ_CUDA(ctx, cudaMemsetAsync(cnt, 0, 8, st));
+    ALQ_CUDA(ctx, cudaMemsetAsync(cnt, 0, 12, st));
     rs::normalize_split_kernel<<<(k + rs::NORM_WARPS - 1) / rs::NORM_WARPS, rs::NORM_WARPS * 32, 0, st>>>(
         nullptr, k, d, d, cc, chi, clo, cn, 0);
     ALQ_LAUNCH_CHECK(ctx);
+    const unsigned int dblocks = static_cast<unsigned int>((static_cast<long long>(ni) + k + 255) / 256);
+    km_domain_kernel<<<dblocks, 256, 0, st>>>(nrm2, ni, cn, k, cnt + 2);
+    ALQ_LAUNCH_CHECK(ctx);
+    unsigned int bad = 0u;
+    ALQ_CUDA(ctx, cudaMemcpyAsync(&bad, cnt + 2, 4, cudaMemcpyDeviceToHost, st));
+    ALQ_CUDA(ctx, cudaStreamSynchronize(st));
+    if (bad)
+        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_kmeans_assign: %u rows or centres have a squared norm that is not in [0, 2]",
+                 bad);
 
     CUtensorMap mxh, mxl, mch, mcl;
     if (!tc::make_map(&mxh, hi, n, d, BM) || !tc::make_map(&mxl, lo, n, d, BM) || !tc::make_map(&mch, chi, k, d, BM) ||
@@ -439,8 +461,8 @@ extern "C" int alq_kmeans_assign(alq_ctx* ctx, const float* xhat, const float* h
     AssignParams P{};
     P.nrm2 = nrm2; P.cn = cn;
     P.n = ni; P.K = k; P.ctiles = (k + BM - 1) / BM; P.kblocks = (d + BK - 1) / BK; P.rblocks = (ni + BM - 1) / BM;
-    // DESIGN section 4: the slack covers the fp64 epilogue (d2 <= 4) and the exact sum's own rounding (d 2^-53 of at
-    // most 4)
+    // DESIGN section 4: with squared norms in [0, 2], d2 <= 8 and the slack covers the fp64 epilogue and the exact
+    // sum's own rounding (d 2^-53 of at most 8)
     P.coef = tc::band_coef(d);
     P.slack = 1e-9;
     P.labels = labels; P.list = list; P.counts = cnt;

@@ -898,7 +898,10 @@ class Engine:
     def kmeans_assign(self, xhat: torch.Tensor, centres: torch.Tensor, labels: Optional[torch.Tensor] = None):
         """K15: labels[i] = the lowest c of the minimum of the exact fp64 d2(xhat_i, centres_c) (K7's pair arithmetic).
         `labels` (int32, CUDA) holds the previous labels and is updated in place; None starts from -1.  Returns
-        (labels, rows whose label changed, rows the tensor-core screen left to the exact recheck)."""
+        (labels, rows whose label changed, rows the tensor-core screen left to the exact recheck).  The screen's band
+        is certified for squared norms in [0, 2] (DESIGN section 4): a row or centre outside it (NaN and infinity
+        included) raises AlqError and leaves `labels` untouched; normalised rows and centres that are their means lie
+        inside."""
         xhat, centres = self._kmeans_inputs(xhat, centres)
         if labels is None:
             labels = torch.full((xhat.shape[0],), -1, dtype=torch.int32, device=xhat.device)
@@ -925,8 +928,9 @@ class Engine:
         """k-means of the rows of xhat [n, d] (d % 4 == 0) into K clusters.  Seeding: k-means++ with nothing labeled,
         CoresetQuery's D^2 cold start through greedy_select (centre 0 = row first_pick, then one D^2 draw per uniform,
         K - 1 of them).  Then Lloyd: assign (K15), and while some label changed and fewer than max_iter assignments
-        ran, update (K16) and assign again; one 8-byte copy per assignment.  Returns (labels int32 CUDA [n], centres
-        [K, d], assignments run, seed rows)."""
+        ran, update (K16) and assign again; one 4-byte and one 8-byte copy per assignment.  The rows' squared norms must
+        lie in [0, 2] (normalised rows do; AlqError otherwise, from the first assignment).  Returns (labels int32 CUDA
+        [n], centres [K, d], assignments run, seed rows)."""
         xhat = _f32c(xhat, "xhat").contiguous()
         n, d = xhat.shape
         K = int(K)

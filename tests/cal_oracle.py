@@ -19,8 +19,9 @@ section 2).
 
 `authors_select` restates the authors' loop literally: sklearn's KNeighborsClassifier and one `kneighbors` per candidate,
 torch fp32 softmax / log_softmax / KLDivLoss(reduction="none") summed over the classes, the mean over the neighbours,
-np.argpartition for the top b.  `band` is K18's screen band and `score_bound` the bound on K19's distance from `scores`
-that CUDA's exp / log allow (both DESIGN section 4).
+np.argpartition for the top b.  `band` is K18's screen band, `screen_lower` its fp32 lower bounds in the kernel's order and
+`fallback_decide` its fallback decision; `score_bound` is the bound on K19's distance from `scores` that CUDA's exp / log
+allow (DESIGN section 4).
 """
 import math
 
@@ -152,6 +153,74 @@ def band(d, nrm_i, nrm_j):
     coef = 2.0 * P.screen_bound(d, 1.0, 1.0) * (1.0 + 1e-6)
     t = si + sj
     return coef * (si * sj) + (4.0 * d + 32.0) * U * (t * t) + d * 2.0 ** -100 * (1.0 + t)
+
+
+def _f32_down(v):
+    """fp64 values rounded down to fp32 (__double2float_rd): NumPy rounds to nearest, so step down where that lands
+    above the fp64 value."""
+    v = np.asarray(v, dtype=np.float64)
+    with np.errstate(over="ignore", invalid="ignore"):
+        f = v.astype(np.float32)
+        return np.where(f.astype(np.float64) > v, np.nextafter(f, np.float32(-np.inf)), f).astype(np.float32)
+
+
+def screen_lower(d, nrm_i, nrm_j, g):
+    """K18's lower bounds L [.., ..] float32 for fp32 dot products g of rows with squared norms nrm_i, nrm_j (their
+    lane-ordered fp64 values) at width d, as knn_screen_kernel forms them: d2~ = (nrm_i + nrm_j) - 2 g,
+    t = sqrt(nrm_i) + sqrt(nrm_j), b = (coef (sx sy) + rel (t t)) + abs (1 + t), fl32_down(d2~ - b)."""
+    ni, nj = np.asarray(nrm_i, dtype=np.float64), np.asarray(nrm_j, dtype=np.float64)
+    sx, sy = np.sqrt(ni), np.sqrt(nj)
+    coef = 2.0 * P.screen_bound(d, 1.0, 1.0) * (1.0 + 1e-6)
+    rel, abs_ = (4.0 * d + 32.0) * U, d * 2.0 ** -100
+    t = sx + sy
+    b = (coef * (sx * sy) + rel * (t * t)) + abs_ * (1.0 + t)
+    return _f32_down(screen_d2(ni, nj, g) - b)
+
+
+S_KEPT = 32                            # lower bounds K18 keeps per row
+
+
+def fallback_decide(L, exact, k):
+    """K18's fallback decision per row of the lower bounds L [n, m]: the kept set is the S_KEPT smallest L, L* the
+    (S_KEPT + 1)-th smallest (+inf for m <= S_KEPT), E_k the k-th exact d2 over the kept columns in (d2, column) order,
+    and the row falls back iff L* <= E_k.  `exact(rows, cols)` gives exact_d2 for index pairs; it is called only for the
+    kept columns and those tied with the last kept bound.  Returns, per row, the frozenset of decisions the kernel can
+    reach: two only when L ties across the boundary and the kept set changes the decision, which needs a bound above its
+    exact value (a tied column at or above L* never sets E_k below L*)."""
+    L = np.asarray(L, dtype=np.float32)
+    n, m = L.shape
+    if m <= S_KEPT:
+        return [frozenset([False])] * n
+    order = np.argsort(L, axis=1, kind="stable")
+    srt = np.take_along_axis(L, order, axis=1)
+    lstar = srt[:, S_KEPT]
+    edge = srt[:, S_KEPT - 1]
+    # the columns certainly kept (below the last kept bound) and the candidates for the rest (tied with it)
+    rows, cols = [], []
+    for i in range(n):
+        c = np.flatnonzero(L[i] <= edge[i]) if lstar[i] == edge[i] else order[i, :S_KEPT]
+        rows.append(np.full(len(c), i))
+        cols.append(c)
+    ex = exact(np.concatenate(rows), np.concatenate(cols))
+    out, at = [], 0
+    for i in range(n):
+        c = cols[i]
+        e = ex[at:at + len(c)]
+        at += len(c)
+        if np.isinf(lstar[i]):
+            out.append(frozenset([False]))
+            continue
+        sure = L[i, c] < edge[i]
+        need = S_KEPT - int(sure.sum())            # kept from the tied columns
+        o = np.lexsort((c[~sure], e[~sure]))
+        tied_e, tied_c = e[~sure][o], c[~sure][o]
+        dec = set()
+        for pick in (slice(0, need), slice(len(tied_c) - need, len(tied_c))):   # the smallest and the largest E_k
+            ke, kc = np.concatenate([e[sure], tied_e[pick]]), np.concatenate([c[sure], tied_c[pick]])
+            ek = ke[np.lexsort((kc, ke))][k - 1]
+            dec.add(bool(float(lstar[i]) <= ek))
+        out.append(frozenset(dec))
+    return out
 
 
 def screen_d2(nrm_i, nrm_j, g):

@@ -18,7 +18,8 @@ Matching sklearn's k-means or faiss's fp32 distances is not a goal (DESIGN secti
              rest is np.random.choice(available-and-unpicked positions ascending, rest, replace=False).
 
 `authors_select` restates the authors' loop literally (np.unique, np.bincount, a lexsort for pandas' sort, brute-force
-fp64 k-NN for faiss); while no kept cluster runs dry it equals `select`.  `assign_decide` is K15's band decision.
+fp64 k-NN for faiss); while no kept cluster runs dry it equals `select`.  `assign_decide` is K15's band decision and
+`exact_argmin` the assignment by brute force (`exact_d2_table`), for rows and centres of any norm.
 """
 import numpy as np
 import torch
@@ -221,3 +222,24 @@ def assign_decide(d, nrm_rows, cn, g):
     l2 = srt[:, 1] if low.shape[1] > 1 else np.full(low.shape[0], np.inf)
     c1 = np.argmin(low, axis=1)
     return l2 > u, c1
+
+
+def exact_d2_table(x, c, chunk=256):
+    """[n, K] exact_d2(x_i, c_c) for every pair, by brute force (no screen, so any norm): per chunk of rows the sums
+    d = a - b, s = s + d * d, k ascending, in fp64."""
+    x, c = np.asarray(x, dtype=np.float32), np.asarray(c, dtype=np.float32)
+    c64 = c.astype(np.float64)
+    out = np.empty((x.shape[0], c.shape[0]))
+    for lo in range(0, x.shape[0], chunk):
+        xs = x[lo:lo + chunk].astype(np.float64)
+        s = np.zeros((xs.shape[0], c.shape[0]))
+        for k in range(x.shape[1]):
+            df = xs[:, k, None] - c64[None, :, k]
+            s = s + df * df
+        out[lo:lo + chunk] = s
+    return out
+
+
+def exact_argmin(x, c, chunk=256):
+    """label_i = the lowest c of the minimum exact_d2(x_i, c_c) over ALL centres (exact_d2_table's brute force)."""
+    return np.argmin(exact_d2_table(x, c, chunk), axis=1).astype(np.int64)     # the first minimum: the lowest centre
