@@ -151,10 +151,14 @@ SIGNATURES = {
     "alq_kmeans_update": (C.c_int, [C.c_void_p, c_f32p, C.c_int64, C.c_int32, c_i32p, C.c_int32, c_f32p, C.c_void_p]),
     "alq_typicality": (C.c_int, [C.c_void_p, c_f32p, C.c_int32, c_i32p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p,
                                  c_i32p, C.c_void_p]),
+    "alq_kmeans_nearest": (C.c_int, [C.c_void_p, c_f32p, C.c_int64, C.c_int32, c_i32p, c_f32p, C.c_int32, c_i32p,
+                                     C.c_void_p]),
     "alq_knn": (C.c_int, [C.c_void_p, c_f32p, C.c_int64, c_f32p, C.c_int64, C.c_int32, C.c_int32, c_i32p, C.c_void_p,
                           C.c_void_p, C.c_void_p]),
     "alq_cal_scores": (C.c_int, [C.c_void_p, c_f32p, C.c_int64, c_f32p, C.c_int64, C.c_int32, c_i32p, C.c_int32,
                                  C.c_void_p, c_f32p, C.c_void_p]),
+    "alq_alfamix_rho": (C.c_int, [C.c_void_p, c_f32p, C.c_int64, C.c_int32, c_f32p, C.c_int32, c_f32p, c_f32p, C.c_int32,
+                                  C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
 }
 
 

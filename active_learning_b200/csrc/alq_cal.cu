@@ -319,18 +319,7 @@ knn_fallback_kernel(const float* __restrict__ x, const float* __restrict__ y, in
 __global__ void __launch_bounds__(256) cal_lse_kernel(const float* __restrict__ z, int rows, int C, double* __restrict__ lse) {
     const int r = blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= rows) return;
-    const float* zr = z + static_cast<size_t>(r) * C;
-    float mx = -INFINITY;
-    bool nan = false;
-    for (int c = 0; c < C; ++c) {
-        const float v = __ldg(zr + c);
-        nan |= v != v;
-        mx = v > mx ? v : mx;
-    }
-    const double m = nan ? static_cast<double>(NAN) : static_cast<double>(mx);
-    double s = 0.0;
-    for (int c = 0; c < C; ++c) s = __dadd_rn(s, exp(__dsub_rn(static_cast<double>(__ldg(zr + c)), m)));
-    lse[r] = __dadd_rn(m, log(s));
+    lse[r] = row_lse(z + static_cast<size_t>(r) * C, C);
 }
 
 constexpr int KL_THREADS = 256;

@@ -393,4 +393,20 @@ __device__ __forceinline__ bool pair_less(double a, int ca, double b, int cb) {
     return a < b || (a == b && ca < cb);
 }
 
+// ---- a row's log-sum-exp in fp64 (K19, K20; the NumPy statement is cal_oracle.log_softmax) ----
+// m + log(sum_c exp(z_c - m)), m = max_c z_c, c ascending; NaN when a logit is NaN
+__device__ __forceinline__ double row_lse(const float* __restrict__ zr, int C) {
+    float mx = -INFINITY;
+    bool nan = false;
+    for (int c = 0; c < C; ++c) {
+        const float v = __ldg(zr + c);
+        nan |= v != v;
+        mx = v > mx ? v : mx;
+    }
+    const double m = nan ? static_cast<double>(NAN) : static_cast<double>(mx);
+    double s = 0.0;
+    for (int c = 0; c < C; ++c) s = __dadd_rn(s, exp(__dsub_rn(static_cast<double>(__ldg(zr + c)), m)));
+    return __dadd_rn(m, log(s));
+}
+
 static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }

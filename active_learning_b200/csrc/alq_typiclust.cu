@@ -26,6 +26,10 @@
 //              position, so a duplicate row counts with d2 = 0), their ascending fp64 sum / k = mean, typicality =
 //              1 / (mean + 1e-5), and per group the argmax (lowest position on ties).  64 x 64 block-diagonal tiles of
 //              d2_step; each warp keeps the sorted 32 smallest of its rows across the lanes.  m x m is never formed.
+// K21 alq_kmeans_nearest per cluster c < K the row labeled c with the smallest exact fp64 d2(xhat_i, centre_c), the lowest
+//              row on ties, -1 for an empty cluster.  A thread per row computes its d2 to its own centre; an fp64 d2 >= 0
+//              orders as its 64-bit pattern, so one atomicMin per row finds each cluster's smallest d2 and a second one,
+//              over the rows that reach it, the lowest such row (the d2 leaves no bits of a 64-bit key for the row).
 #include <math.h>
 
 #include <algorithm>
@@ -38,7 +42,7 @@ namespace tk {
 
 using tc::BK;
 using tc::BM;
-constexpr int K_MAX = 8192;                     // K16's histogram lives in shared memory
+constexpr int K_MAX = 32768;                    // K16's histogram lives in shared memory: 128 KB at K_MAX
 constexpr double NRM2_MAX = 2.0;                // the band's absolute slack is derived for squared norms in [0, 2]
 
 // ---- K15 ---------------------------------------------------------------------------------------------------------------
@@ -398,6 +402,32 @@ __global__ void __launch_bounds__(256) km_typ_argmax_kernel(const double* __rest
     }
 }
 
+// ---- K21 ---------------------------------------------------------------------------------------------------------------
+// d2[i] = exact_d2(xhat_i, centre_{labels[i]}); best_d2[c] = the smallest over the rows labeled c (as 64-bit patterns)
+__global__ void __launch_bounds__(256) km_near_d2_kernel(const float* __restrict__ xhat, int n, int d, const int* __restrict__ labels,
+                                                         const float* __restrict__ cen, int K, double* __restrict__ d2,
+                                                         unsigned long long* __restrict__ best_d2) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int c = labels[i];
+    if (c < 0 || c >= K) return;
+    const double v = exact_d2(xhat + static_cast<size_t>(i) * d, cen + static_cast<size_t>(c) * d, d);
+    d2[i] = v;
+    atomicMin(best_d2 + c, static_cast<unsigned long long>(__double_as_longlong(v)));
+}
+
+// best_row[c] = the lowest row labeled c whose d2 equals best_d2[c]; best_row starts at 0xffffffff, which stays (-1 as
+// int32) for an empty cluster
+__global__ void __launch_bounds__(256) km_near_row_kernel(int n, const int* __restrict__ labels, int K, const double* __restrict__ d2,
+                                                          const unsigned long long* __restrict__ best_d2,
+                                                          unsigned int* __restrict__ best_row) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int c = labels[i];
+    if (c < 0 || c >= K) return;
+    if (static_cast<unsigned long long>(__double_as_longlong(d2[i])) == best_d2[c]) atomicMin(best_row + c, static_cast<unsigned int>(i));
+}
+
 }  // namespace tk
 
 extern "C" int alq_kmeans_rows(alq_ctx* ctx, const float* x, int64_t n, int32_t d, int64_t ldx, int32_t normalise,
@@ -500,6 +530,8 @@ extern "C" int alq_kmeans_update(alq_ctx* ctx, const float* xhat, int64_t n, int
     int* start = cur.take<int>(k);
     int* order = cur.take<int>(n);
     const size_t hsm = static_cast<size_t>(k) * 4;
+    ALQ_CUDA(ctx, cudaFuncSetAttribute(km_hist_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(hsm)));
+    ALQ_CUDA(ctx, cudaFuncSetAttribute(km_place_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(hsm)));
     km_hist_kernel<<<chunks, 256, hsm, st>>>(labels, ni, k, hist);
     ALQ_LAUNCH_CHECK(ctx);
     km_scan_kernel<<<1, 1024, 0, st>>>(hist, chunks, k, count, start);
@@ -549,5 +581,30 @@ extern "C" int alq_typicality(alq_ctx* ctx, const float* xhat, int32_t d, const 
     km_typ_argmax_kernel<<<groups, 256, 0, st>>>(typ, dg, best);
     ALQ_LAUNCH_CHECK(ctx);
     ALQ_CUDA(ctx, cudaStreamSynchronize(st));
+    return ALQ_OK;
+}
+
+extern "C" int alq_kmeans_nearest(alq_ctx* ctx, const float* xhat, int64_t n, int32_t d, const int32_t* labels,
+                                  const float* centres, int32_t k, int32_t* nearest, void* stream) {
+    using namespace tk;
+    if (!ctx) return ALQ_ERR_INVALID;
+    if (n < 1 || n >= (1LL << 31)) ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_kmeans_nearest: n=%lld outside [1, 2^31)", (long long)n);
+    if (d < 4 || d % 4) ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_kmeans_nearest: d=%d must be a positive multiple of 4", d);
+    if (k < 1) ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_kmeans_nearest: K=%d must be positive", k);
+    if (!xhat || !labels || !centres || !nearest || !aligned16(xhat) || !aligned16(centres))
+        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_kmeans_nearest: null pointer or xhat / centres not 16-byte aligned");
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int ni = static_cast<int>(n);
+    int rc = alq_scratch_reserve(ctx, scratch_need({static_cast<size_t>(n) * 8, static_cast<size_t>(k) * 8}));
+    if (rc) return rc;
+    ScratchCursor cur(ctx->scratch);
+    double* d2 = cur.take<double>(n);
+    unsigned long long* best = cur.take<unsigned long long>(k);
+    ALQ_CUDA(ctx, cudaMemsetAsync(best, 0xff, static_cast<size_t>(k) * 8, st));
+    ALQ_CUDA(ctx, cudaMemsetAsync(nearest, 0xff, static_cast<size_t>(k) * 4, st));
+    km_near_d2_kernel<<<(ni + 255) / 256, 256, 0, st>>>(xhat, ni, d, labels, centres, k, d2, best);
+    ALQ_LAUNCH_CHECK(ctx);
+    km_near_row_kernel<<<(ni + 255) / 256, 256, 0, st>>>(ni, labels, k, d2, best, reinterpret_cast<unsigned int*>(nearest));
+    ALQ_LAUNCH_CHECK(ctx);
     return ALQ_OK;
 }

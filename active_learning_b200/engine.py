@@ -975,6 +975,45 @@ class Engine:
                                             g, int(k), _ptr(typ), _ptr(best), self._stream()), "alq_typicality")
         return typ[:rows.numel()], best.cpu().numpy().astype(np.int64)
 
+    def kmeans_nearest(self, xhat: torch.Tensor, labels: torch.Tensor, centres: torch.Tensor) -> np.ndarray:
+        """K21: per cluster c < K the row labeled c with the smallest exact fp64 d2(xhat_i, centres_c) (K7's pair
+        arithmetic), the lowest row on ties; -1 for an empty cluster.  Rows labeled outside [0, K) are skipped.  Returns
+        host int64 [K]."""
+        xhat, centres = self._kmeans_inputs(xhat, centres)
+        if labels.dtype != torch.int32 or not labels.is_cuda or labels.numel() != xhat.shape[0]:
+            raise AlqError("kmeans_nearest: labels must be an int32 CUDA tensor with one entry per row")
+        k = centres.shape[0]
+        out = torch.empty(max(k, 1), dtype=torch.int32, device=xhat.device)
+        self._check(self.lib.alq_kmeans_nearest(self._h, _ptr(xhat), xhat.shape[0], xhat.shape[1], _ptr(labels.contiguous()),
+                                                _ptr(centres), k, _ptr(out), self._stream()), "alq_kmeans_nearest")
+        return out[:k].cpu().numpy().astype(np.int64)
+
+    # -- K20: ALFA-Mix -------------------------------------------------------------------------------
+    def alfamix_rho(self, logits: torch.Tensor, emb: torch.Tensor, anchors: torch.Tensor, weight: torch.Tensor,
+                    want_parts: bool = False):
+        """K20: ALFA-Mix's closed-form mixing test per row (spec: tests/alfamix_oracle.py).  logits [n, C], emb [n, Dp] and
+        anchors [C, Dp] (the raw embeddings and class anchors, zero columns past D), weight [C, D] the linear head, all
+        float32 CUDA.  rho_u = sqrt(D) t*_u / R_u, where t*_u is the smallest feature step along the loss gradient that
+        changes the predicted class and R_u the largest exact distance to an anchor; row u's mixed features flip its
+        prediction at cap eps exactly when rho_u < eps sqrt(D).  Returns rho float64 CUDA [n], or (rho, R^2, t*) with
+        want_parts.  AlqError for C < 2, mismatched shapes, or a non-finite entry."""
+        zl, z = _f32c(logits, "logits").contiguous(), _f32c(emb, "emb").contiguous()
+        a, w = _f32c(anchors, "anchors").contiguous(), _f32c(weight, "weight").contiguous()
+        if z.dim() == 2 and a.dim() == 2:
+            z, a = self._pad4(z), self._pad4(a)
+        if (zl.dim() != 2 or z.dim() != 2 or a.dim() != 2 or w.dim() != 2 or zl.shape[0] != z.shape[0]
+                or zl.shape[1] != w.shape[0] or a.shape[0] != w.shape[0] or a.shape[1] != z.shape[1]
+                or w.shape[1] > z.shape[1]):
+            raise AlqError(f"alfamix_rho: need logits [n, C], emb [n, Dp], anchors [C, Dp] and weight [C, D <= Dp], got "
+                           f"{tuple(zl.shape)}, {tuple(z.shape)}, {tuple(a.shape)} and {tuple(w.shape)}")
+        n = zl.shape[0]
+        outs = [torch.empty(max(n, 1), dtype=torch.float64, device=zl.device) for _ in range(3 if want_parts else 1)]
+        ptrs = [_ptr(t) for t in outs] + [None] * (3 - len(outs))
+        self._check(self.lib.alq_alfamix_rho(self._h, _ptr(zl), n, zl.shape[1], _ptr(z), z.shape[1], _ptr(a), _ptr(w),
+                                             w.shape[1], *ptrs, self._stream()), "alq_alfamix_rho")
+        outs = [t[:n] for t in outs]
+        return tuple(outs) if want_parts else outs[0]
+
     # -- K18 / K19: CAL ------------------------------------------------------------------------------
     def knn(self, x: torch.Tensor, y: torch.Tensor, k: int):
         """K18: the k nearest rows of y [m, d] for every row of x [n, d] (float32 CUDA, d % 4 == 0) by the exact fp64

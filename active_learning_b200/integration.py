@@ -16,6 +16,7 @@ from __future__ import annotations
 
 from .query_strategies.coreset import (BADGEQuery, CoresetQuery, PartitionedBADGEQuery,
                                        PartitionedCoresetQuery)
+from .query_strategies.alfamix import ALFAMixQuery
 from .query_strategies.balanced_random import BalancedRandomQuery
 from .query_strategies.cal import CALQuery
 from .query_strategies.balancing import BalancingQuery
@@ -42,6 +43,7 @@ _MIXINS = {
     "ProbCoverSampler": ProbCoverQuery,
     "TypiClustSampler": TypiClustQuery,
     "CALSampler": CALQuery,
+    "ALFAMixSampler": ALFAMixQuery,
 }
 
 

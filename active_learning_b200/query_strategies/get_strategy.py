@@ -1,8 +1,10 @@
 """`--strategy` dispatch, same contract as active_learning/src/query_strategies/get_strategy.py:
 `get_strategy(name)` returns the class called `name`.  Every class name the reference dispatches is implemented: the
 thirteen accelerated samplers (the seven of the north-star path plus MASE / BASE / Balancing, SURVEY.md section 8f,
-MarginClustering, VAAL and BalancedRandom) and the default RandomSampler.  ProbCoverSampler, TypiClustSampler and
-CALSampler are this project's additions (no reference counterpart; ProbCoverSampler needs the sampler kwarg `delta`)."""
+MarginClustering, VAAL and BalancedRandom) and the default RandomSampler.  ProbCoverSampler, TypiClustSampler,
+CALSampler and ALFAMixSampler are this project's additions (no reference counterpart; ProbCoverSampler needs the sampler
+kwarg `delta`)."""
+from .alfamix_sampler import ALFAMixSampler  # noqa: F401
 from .badge_sampler import BADGESampler  # noqa: F401
 from .balanced_random_sampler import BalancedRandomSampler  # noqa: F401
 from .balancing_sampler import BalancingSampler  # noqa: F401
@@ -24,7 +26,7 @@ from .vaal_sampler import VAALSampler  # noqa: F401
 ACCELERATED = ("MarginSampler", "ConfidenceSampler", "EntropySampler", "CoresetSampler",
                "PartitionedCoresetSampler", "BADGESampler", "PartitionedBADGESampler", "MASESampler", "BASESampler",
                "BalancingSampler", "MarginClusteringSampler", "VAALSampler", "BalancedRandomSampler",
-               "ProbCoverSampler", "TypiClustSampler", "CALSampler")
+               "ProbCoverSampler", "TypiClustSampler", "CALSampler", "ALFAMixSampler")
 NOT_ON_THIS_PATH = ()
 
 

@@ -42,11 +42,7 @@ class MASEQuery(EngineMixin):
         labeled_idxs = np.asarray(idxs_for_query)[pos].tolist()
         return labeled_idxs, budget
 
-    # ---- mase_sampler.py:29-102 --------------------------------------------------------------------
-    def _head(self):
-        core_net = self.net.module if hasattr(self.net, "module") else self.net   # :46-49
-        return core_net.linear.weight, core_net.linear.bias
-
+    # ---- mase_sampler.py:29-102 (the head through EngineMixin._head, :46-49) ---------------------------
     def _margins_device(self, idxs, want_per_class, dataset=None, labels_out=None):
         """(min_margins [n] fp32, pred [n] int32, per_class [n, C] fp32 or None), all on the query device."""
         eng = self.get_engine()

@@ -147,6 +147,16 @@ class EngineMixin:
             state.pop(k, None)
         return state
 
+    def _head(self):
+        """(weight [C, D], bias [C]) of the task network's linear head (resnet_simclr.py's `linear`), through a
+        DataParallel / DistributedDataParallel wrapper."""
+        core_net = self.net.module if hasattr(self.net, "module") else self.net
+        linear = getattr(core_net, "linear", None)
+        if linear is None or not hasattr(linear, "weight"):
+            raise AttributeError(f"{type(self).__name__} needs the task network's linear head: "
+                                 f"{type(core_net).__name__} has no `.linear` layer with a weight")
+        return linear.weight, linear.bias
+
     def _query_device(self):
         eng = self.get_engine()
         return getattr(eng, "device", self.device)

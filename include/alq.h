@@ -533,16 +533,20 @@ int alq_probcover_select(alq_ctx* ctx, const int64_t* row_ptr, const int32_t* co
  *   (K7's pair arithmetic: d = a - b, s = s + d * d, k ascending, no FMA).  The pairs are screened on the tensor cores
  *   (3xTF32) with a rigorous band (DESIGN section 4); a row whose nearest centre the band cannot isolate is recomputed
  *   exactly against every centre.  labels is read (the previous labels; any value outside [0, K) counts as a change)
- *   and written.  counts_host[0] = rows whose label changed, counts_host[1] = rows rechecked.  K in [1, 8192].
+ *   and written.  counts_host[0] = rows whose label changed, counts_host[1] = rows rechecked.  K in [1, 32768].
  *   Synchronous (one 8-byte copy).
  * alq_kmeans_update (K16): for every c < K with m_c = |{i : labels[i] == c}| > 0, centres[c] = fl32(S_c / m_c), S_c the
  *   fp64 sum of the member rows of xhat in ascending row order (one sequential chain per column).  Clusters with no
- *   member, and rows whose label is outside [0, K), are left alone.  K in [1, 8192].  Asynchronous on `stream`.
+ *   member, and rows whose label is outside [0, K), are left alone.  K in [1, 32768].  Asynchronous on `stream`.
  * alq_typicality (K17): rows[group_off_host[g] .. group_off_host[g + 1]) (int32 row ids of xhat[., d], device) form group
  *   g, every group non-empty.  For each listed row, k = min(k_max, m_g / 2) and mean = the ascending fp64 sum of the k
  *   smallest exact fp64 d2 (K7's arithmetic) to the other rows of its group (itself excluded by position) divided by k;
  *   typ = 1 / (mean + 1e-5) (fp64, device, one per listed row; 0 for a group of one row).  best[g] = the position in
- *   rows of the group's largest typ, the lowest on ties.  k_max in [1, 32].  Synchronous. */
+ *   rows of the group's largest typ, the lowest on ties.  k_max in [1, 32].  Synchronous.
+ * alq_kmeans_nearest (K21): nearest[c] (int32, device) = for every c < K the row i with labels[i] == c and the smallest
+ *   exact fp64 d2(xhat_i, centres_c) (K7's pair arithmetic), the lowest row on ties; -1 when no row is labeled c.  Rows
+ *   whose label is outside [0, K) are skipped.  xhat [n, d], centres [K, d]: fp32, 16-byte aligned, d % 4 == 0.
+ *   Asynchronous on `stream`. */
 int alq_kmeans_rows(alq_ctx* ctx, const float* x, int64_t n, int32_t d, int64_t ldx, int32_t normalise, float* xhat,
                     float* hi, float* lo, double* nrm2, void* stream);
 int alq_kmeans_assign(alq_ctx* ctx, const float* xhat, const float* hi, const float* lo, const double* nrm2, int64_t n,
@@ -551,6 +555,8 @@ int alq_kmeans_update(alq_ctx* ctx, const float* xhat, int64_t n, int32_t d, con
                       float* centres, void* stream);
 int alq_typicality(alq_ctx* ctx, const float* xhat, int32_t d, const int32_t* rows, const int64_t* group_off_host,
                    int32_t groups, int32_t k_max, double* typ, int32_t* best, void* stream);
+int alq_kmeans_nearest(alq_ctx* ctx, const float* xhat, int64_t n, int32_t d, const int32_t* labels, const float* centres,
+                       int32_t k, int32_t* nearest, void* stream);
 
 /* ---- K18 / K19: CAL (Margatina, Vernikos, Barrault & Aletras, EMNLP 2021) ---------------------------------------------
  * alq_knn (K18): for every row i of x[n, d], idx[i][0..k) = the k rows j of y[m, d] with the smallest exact fp64
@@ -572,6 +578,20 @@ int alq_knn(alq_ctx* ctx, const float* x, int64_t n, const float* y, int64_t m, 
             double* d2, int64_t* fallback_rows_host, void* stream);
 int alq_cal_scores(alq_ctx* ctx, const float* cand_logits, int64_t n, const float* ref_logits, int64_t m, int32_t c,
                    const int32_t* idx, int32_t k, double* score, float* key, void* stream);
+
+/* ---- K20: ALFA-Mix (Parvaneh et al., CVPR 2022) -----------------------------------------------------------------------
+ * alq_alfamix_rho (K20): the closed-form feature-mixing test of every row u of logits[n, C] (fp32, contiguous) with its
+ *   embedding emb[n, dp] against the head weight[C, D] and the anchors[C, dp] (fp32, contiguous; emb and anchors padded
+ *   with zero columns from D to dp, dp % 4 == 0).  In fp64: G = weight weight^T (ascending-d chain per entry);
+ *   lse_u as alq_cal_scores forms it, yhat = the lowest class of the largest logit, r_c = exp(l_c - lse_u) - [c == yhat];
+ *   w_k = sum_c G_kc r_c (c ascending); s2 = sum_k r_k w_k (k ascending); t* = min over {k : w_k > w_yhat} of
+ *   ((l_yhat - l_k) sqrt(s2)) / (w_k - w_yhat), +inf when s2 <= 0 or no k qualifies; R2 = max_c of the exact fp64
+ *   d2(emb_u, anchors_c) (K7's pair arithmetic); rho = (sqrt(D) t*) / sqrt(R2), +inf when R2 = 0 or t* = +inf.
+ *   rho, r2 and tstar are fp64 [n] on the device; r2 and tstar may be NULL.  C >= 2, 1 <= D <= dp; a non-finite logit,
+ *   embedding, anchor or weight entry is ALQ_ERR_INVALID.  Synchronous. */
+int alq_alfamix_rho(alq_ctx* ctx, const float* logits, int64_t n, int32_t c, const float* emb, int32_t dp,
+                    const float* anchors, const float* weight, int32_t d, double* rho, double* r2, double* tstar,
+                    void* stream);
 
 #ifdef __cplusplus
 }
