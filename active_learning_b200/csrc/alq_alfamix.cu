@@ -200,8 +200,9 @@ extern "C" int alq_alfamix_rho(alq_ctx* ctx, const float* logits, int64_t n, int
         ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_alfamix_rho: null pointer");
     const cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int ni = static_cast<int>(n);
-    // rows per chunk of the residual and w = r G pass: r and w stay below 2^25 entries each
-    const int chunk = std::min(ni, std::max(TT, static_cast<int>(((1LL << 25) / c) / TT * TT)));
+    // rows per chunk of the residual and w = r G pass: r and w stay below 2^25 entries each, and w = r G's row tiles
+    // (gridDim.y) within CUDA's 65 535
+    const int chunk = std::min({ni, 65535 * TT, std::max(TT, static_cast<int>(((1LL << 25) / c) / TT * TT))});
     const size_t cc = static_cast<size_t>(c) * c, rc = static_cast<size_t>(chunk) * c;
     int rcode = alq_scratch_reserve(ctx, scratch_need({cc * 8, rc * 8, rc * 8, static_cast<size_t>(chunk) * 4,
                                                        static_cast<size_t>(n) * 8, 4}));

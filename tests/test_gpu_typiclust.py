@@ -48,8 +48,8 @@ def _centres(rng, xhat, k):
     return cen
 
 
-@pytest.mark.parametrize("k", [1, 127, 128, 129, 500, 700])
-@pytest.mark.parametrize("d", [4, 28, 64, 520, 2048])
+@pytest.mark.parametrize("d,k", [(d, k) for d in (4, 28, 64, 520, 2048) for k in (1, 127, 128, 129, 500, 700)]
+                         + [(4, 32768), (64, 32768)])                  # K_MAX: 256 centre tiles
 def test_assign_labels_equal_the_exact_argmin(eng, d, k):
     rng = np.random.default_rng(d * 1000 + k)
     n = 1037                                                            # a partial last row tile
