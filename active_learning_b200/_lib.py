@@ -159,6 +159,10 @@ SIGNATURES = {
                                  C.c_void_p, c_f32p, C.c_void_p]),
     "alq_alfamix_rho": (C.c_int, [C.c_void_p, c_f32p, C.c_int64, C.c_int32, c_f32p, C.c_int32, c_f32p, c_f32p, C.c_int32,
                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "alq_herding_kernel": (C.c_int, [C.c_void_p, c_f32p, C.c_int64, C.c_int32, C.c_int64, C.c_void_p, c_f32p, C.c_int64,
+                                     C.c_void_p]),
+    "alq_herding_select": (C.c_int, [C.c_void_p, c_f32p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, c_i32p,
+                                     c_f32p, C.c_void_p, C.c_void_p, C.c_void_p]),
 }
 
 

@@ -10,6 +10,10 @@
 //                    256 threads x 4 x 4 pairs in registers; k-chunks of both row blocks arrive
 //                    with 4-byte cp.async (any ld, any alignment, zero-filled past d and past n) into a two-stage fp32
 //                    ring and are widened once into an fp64 tile that the inner loop reads.
+// K22 alq_herding_kernel  MaxHerdingSampler's Gaussian kernel matrix: K7's square-layout kernel with another epilogue,
+//                    K_ij = K_ji = fl32(exp(-(s / q))) of the same fp64 s, into an n x n fp32 matrix (alq_herding.cu runs
+//                    the greedy over it).  The diagonal s_ii is 0 for a finite row and NaN for a row with a NaN or
+//                    infinite entry, so the diagonal tiles flag non-finite rows with no extra pass.
 // K8 alq_ward_nn_chain  scipy's nn_chain (Ward update) as ONE launch of one thread-block cluster (16 CTAs when the GPU
 //                    can place them, else 8).  CTA r owns columns [lo_r, hi_r) with their cluster sizes in shared
 //                    memory.  A scan of row x: per-CTA (value, lowest index) -> DSMEM exchange -> every CTA resolves
@@ -141,10 +145,19 @@ struct Band {
     int64_t base;
 };
 
-template <bool CONDENSED>
+// What the tile's epilogue writes: K7's sqrt(s) in the square or the condensed layout, or K22's fl32(exp(-(s / q))) in
+// the square layout (T = float; `bad` counts the rows whose s_ii is not 0)
+enum class PdOut { SQUARE, CONDENSED, GAUSS };
+struct Gauss {
+    double q;
+    unsigned int* bad;
+};
+
+template <PdOut OUT, typename T>
 __global__ void __launch_bounds__(PD_THREADS, 2)
-pdist_f64_kernel(const float* __restrict__ x, int n, int d, int64_t ldx, double* __restrict__ dist, int64_t ldd,
-                 const Band band) {
+pdist_f64_kernel(const float* __restrict__ x, int n, int d, int64_t ldx, T* __restrict__ dist, int64_t ldd,
+                 const Band band, const Gauss gauss) {
+    constexpr bool CONDENSED = OUT == PdOut::CONDENSED;
     const int ti = CONDENSED ? band.tile_lo + static_cast<int>(blockIdx.y) : static_cast<int>(blockIdx.y);
     const int tj = blockIdx.x;
     if (ti > tj) return;                                   // upper triangle of tiles only
@@ -209,7 +222,13 @@ pdist_f64_kernel(const float* __restrict__ x, int n, int d, int64_t ldx, double*
                 if (band.row_lo <= i && i < band.row_hi && i < j && j < n)
                     dist[cidx(i, j, n) - band.base] = __dsqrt_rn(acc[a][b]);
             } else if (i < n && j < n && (ti != tj || i <= j)) {
-                const double v = __dsqrt_rn(acc[a][b]);
+                T v;
+                if constexpr (OUT == PdOut::GAUSS) {
+                    v = __double2float_rn(exp(-__ddiv_rn(acc[a][b], gauss.q)));
+                    if (i == j && acc[a][b] != 0.0) atomicAdd(gauss.bad, 1u);
+                } else {
+                    v = __dsqrt_rn(acc[a][b]);
+                }
                 dist[static_cast<int64_t>(i) * ldd + j] = v;
                 dist[static_cast<int64_t>(j) * ldd + i] = v;
             }
@@ -521,18 +540,19 @@ void heap_pushpop(std::vector<int64_t>& h, int64_t item) {
 
 // K7 launches for either layout over the rows [row_lo, row_hi) (the square layout always takes [0, n)); `name` is the
 // entry point's, for its error messages
-template <bool CONDENSED>
-int pdist_run(alq_ctx* ctx, const char* name, const float* x, int64_t n, int32_t d, int64_t ldx, double* dist, int64_t ldd,
-              int64_t row_lo, int64_t row_hi, void* stream) {
+template <PdOut OUT, typename T>
+int pdist_run(alq_ctx* ctx, const char* name, const float* x, int64_t n, int32_t d, int64_t ldx, T* dist, int64_t ldd,
+              int64_t row_lo, int64_t row_hi, void* stream, Gauss gauss = Gauss{1.0, nullptr}) {
     const int64_t nt = (n + PD_TILE - 1) / PD_TILE;
     if (nt > 65535) ALQ_FAIL(ctx, ALQ_ERR_INVALID, "%s: n=%lld exceeds %d rows", name, (long long)n, 65535 * PD_TILE);
     const int64_t t0 = row_lo / PD_TILE, t1 = (row_hi + PD_TILE - 1) / PD_TILE;
     if (t1 <= t0) return ALQ_OK;                           // an empty band writes nothing
     ALQ_CUDA(ctx, cudaSetDevice(ctx->device));
-    pdist_f64_kernel<CONDENSED><<<dim3(static_cast<unsigned>(nt), static_cast<unsigned>(t1 - t0)), PD_THREADS, 0,
-                                  static_cast<cudaStream_t>(stream)>>>(
+    pdist_f64_kernel<OUT, T><<<dim3(static_cast<unsigned>(nt), static_cast<unsigned>(t1 - t0)), PD_THREADS, 0,
+                               static_cast<cudaStream_t>(stream)>>>(
         x, static_cast<int>(n), d, ldx, dist, ldd,
-        Band{static_cast<int>(row_lo), static_cast<int>(row_hi), static_cast<int>(t0), row_lo * n - row_lo * (row_lo + 1) / 2});
+        Band{static_cast<int>(row_lo), static_cast<int>(row_hi), static_cast<int>(t0), row_lo * n - row_lo * (row_lo + 1) / 2},
+        gauss);
     ALQ_LAUNCH_CHECK(ctx);
     return ALQ_OK;
 }
@@ -587,7 +607,7 @@ extern "C" int alq_pdist_f64(alq_ctx* ctx, const float* x, int64_t n, int32_t d,
     if (!x || !dist || n < 1 || d < 1 || ldx < d || ldd < n)
         ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_pdist_f64: bad arguments (n=%lld d=%d ldx=%lld ldd=%lld)", (long long)n, d,
                  (long long)ldx, (long long)ldd);
-    return pdist_run<false>(ctx, "alq_pdist_f64", x, n, d, ldx, dist, ldd, 0, n, stream);
+    return pdist_run<PdOut::SQUARE>(ctx, "alq_pdist_f64", x, n, d, ldx, dist, ldd, 0, n, stream);
 }
 
 extern "C" int alq_pdist_f64_condensed(alq_ctx* ctx, const float* x, int64_t n, int32_t d, int64_t ldx, double* dist,
@@ -596,7 +616,7 @@ extern "C" int alq_pdist_f64_condensed(alq_ctx* ctx, const float* x, int64_t n, 
     if (!x || !dist || n < 1 || d < 1 || ldx < d)
         ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_pdist_f64_condensed: bad arguments (n=%lld d=%d ldx=%lld)", (long long)n, d,
                  (long long)ldx);
-    return pdist_run<true>(ctx, "alq_pdist_f64_condensed", x, n, d, ldx, dist, 0, 0, n, stream);
+    return pdist_run<PdOut::CONDENSED>(ctx, "alq_pdist_f64_condensed", x, n, d, ldx, dist, 0, 0, n, stream);
 }
 
 extern "C" int alq_pdist_f64_condensed_rows(alq_ctx* ctx, const float* x, int64_t n, int32_t d, int64_t ldx,
@@ -605,7 +625,31 @@ extern "C" int alq_pdist_f64_condensed_rows(alq_ctx* ctx, const float* x, int64_
     if (!x || !dist || n < 1 || d < 1 || ldx < d || row_lo < 0 || row_hi > n || row_lo > row_hi)
         ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_pdist_f64_condensed_rows: bad arguments (n=%lld d=%d ldx=%lld rows [%lld, %lld))",
                  (long long)n, d, (long long)ldx, (long long)row_lo, (long long)row_hi);
-    return pdist_run<true>(ctx, "alq_pdist_f64_condensed_rows", x, n, d, ldx, dist, 0, row_lo, row_hi, stream);
+    return pdist_run<PdOut::CONDENSED>(ctx, "alq_pdist_f64_condensed_rows", x, n, d, ldx, dist, 0, row_lo, row_hi, stream);
+}
+
+extern "C" int alq_herding_kernel(alq_ctx* ctx, const float* x, int64_t n, int32_t d, int64_t ldx, const double* q_host,
+                                  float* k, int64_t ldk, void* stream) {
+    if (!ctx) return ALQ_ERR_INVALID;
+    if (!x || !k || !q_host || n < 1 || d < 1 || ldx < d || ldk < n)
+        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_herding_kernel: bad arguments (n=%lld d=%d ldx=%lld ldk=%lld)", (long long)n, d,
+                 (long long)ldx, (long long)ldk);
+    const double q = *q_host;
+    if (!(std::isfinite(q) && std::fpclassify(q) == FP_NORMAL && q > 0.0))
+        ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_herding_kernel: q=%g must be a finite positive normal number", q);
+    int rc = alq_scratch_reserve(ctx, scratch_need({sizeof(unsigned int)}));
+    if (rc) return rc;
+    unsigned int* bad = ScratchCursor(ctx->scratch).take<unsigned int>(1);
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    ALQ_CUDA(ctx, cudaSetDevice(ctx->device));
+    ALQ_CUDA(ctx, cudaMemsetAsync(bad, 0, sizeof(unsigned int), st));
+    rc = pdist_run<PdOut::GAUSS>(ctx, "alq_herding_kernel", x, n, d, ldx, k, ldk, 0, n, stream, Gauss{q, bad});
+    if (rc) return rc;
+    unsigned int h = 0;
+    ALQ_CUDA(ctx, cudaMemcpyAsync(&h, bad, sizeof(unsigned int), cudaMemcpyDeviceToHost, st));
+    ALQ_CUDA(ctx, cudaStreamSynchronize(st));
+    if (h) ALQ_FAIL(ctx, ALQ_ERR_NUMERIC, "alq_herding_kernel: %u rows hold a NaN or infinite entry", h);
+    return ALQ_OK;
 }
 
 extern "C" int alq_pdist_f64_expand(alq_ctx* ctx, const double* rows, int64_t n, int64_t row_lo, int64_t row_hi,

@@ -842,6 +842,71 @@ class Engine:
                                                   _ptr(picks), C.byref(steps), self._stream()), "alq_probcover_select")
         return picks[:steps.value].cpu().numpy().astype(np.int64), int(steps.value)
 
+    # -- K22 / K23: MaxHerding --------------------------------------------------------------------------
+    HERDING_ROW_BYTES = 4 + 8 + 1 + 12 + 2   # per row: m, the gain, the candidate flag, S's entry, labeled + avail
+
+    @classmethod
+    def herding_bytes(cls, n: int, d: int) -> int:
+        """Device memory a MaxHerding query over n rows of width d needs: the 4 n^2 fp32 kernel matrix, xhat (4 n dp, dp
+        = d padded to a multiple of 4), the per-row arrays of the greedy and Ward's headroom."""
+        n, dp = int(n), max(4, (int(d) + 3) & ~3)
+        return 4 * n * n + 4 * n * dp + cls.HERDING_ROW_BYTES * n + cls.WARD_HEADROOM_BYTES
+
+    def herding_guard(self, n: int, d: int):
+        """AlqError naming n, the bytes needed and the bytes free when herding_bytes(n, d) does not fit the device."""
+        need, free = self.herding_bytes(n, d), self._ward_free_bytes()
+        if need > free:
+            raise AlqError(f"maxherding: n={n} rows of width {d} need {need} bytes of device memory (the 4 n^2 kernel matrix, "
+                           f"xhat and {self.WARD_HEADROOM_BYTES} headroom); {free} are free; use a smaller "
+                           f"subset_unlabeled")
+
+    def herding_kernel(self, xhat: torch.Tensor, sigma: float) -> torch.Tensor:
+        """K22: the Gaussian kernel matrix K [n, n] (float32 CUDA) of the rows of xhat [n, d] (float32 CUDA):
+        K_ij = fl32(exp(-(s_ij / q))), s_ij the exact fp64 squared distance (K7's pair arithmetic), q = 2 sigma^2 in fp64.
+        Exactly symmetric, diagonal 1.  ValueError for a bad sigma (maxherding.herding_q); AlqError when the matrix does
+        not fit (herding_guard, before any allocation) or for a row with a NaN or infinite entry."""
+        from .query_strategies.maxherding import herding_q
+        q = herding_q(sigma)
+        x = _f32c(xhat, "xhat")
+        if x.dim() != 2 or x.shape[0] == 0:
+            raise AlqError(f"herding_kernel: need a non-empty [n, d] matrix, got {tuple(x.shape)}")
+        n, d = x.shape
+        self.herding_guard(n, d)
+        out = torch.empty((n, n), dtype=torch.float32, device=x.device)
+        qh = C.c_double(q)
+        self._check(self.lib.alq_herding_kernel(self._h, _ptr(x), n, d, _ld(x), C.byref(qh), _ptr(out), n,
+                                                self._stream()), "alq_herding_kernel")
+        return out
+
+    def herding_select(self, K: torch.Tensor, labeled: torch.Tensor, avail: torch.Tensor, budget: int):
+        """K23: the greedy coverage picks over herding_kernel's matrix, starting from the rows with labeled != 0 and
+        choosing among the rows with avail != 0 (uint8 or bool CUDA masks, one entry per row).  Returns (picks: host int64
+        array in pick order, min(budget, available rows) long; m: float32 CUDA [n], the final per-row maxima; the sum
+        over the steps of the rows each pick changed)."""
+        n = K.shape[0] if K.dim() == 2 else -1
+        if (not K.is_cuda or K.dtype != torch.float32 or K.dim() != 2 or K.shape[1] != n or K.stride(1) != 1
+                or K.stride(0) < n):
+            raise AlqError("herding_select: K must be a square row-major float32 CUDA matrix")
+        masks = []
+        for name, t in (("labeled", labeled), ("avail", avail)):
+            if not t.is_cuda or t.dtype not in (torch.uint8, torch.bool) or t.numel() != n:
+                raise AlqError(f"herding_select: {name} must be a uint8 or bool CUDA mask with one entry per row")
+            masks.append(t.contiguous().view(torch.uint8).reshape(-1))
+        budget = int(budget)
+        picks = torch.empty(max(budget, 1), dtype=torch.int32, device=K.device)
+        m = torch.empty(n, dtype=torch.float32, device=K.device)
+        steps, sum_s = C.c_int64(0), C.c_int64(0)
+        self._check(self.lib.alq_herding_select(self._h, _ptr(K), n, K.stride(0), _ptr(masks[0]), _ptr(masks[1]), budget,
+                                                _ptr(picks), _ptr(m), C.byref(steps), C.byref(sum_s), self._stream()),
+                    "alq_herding_select")
+        return picks[:steps.value].cpu().numpy().astype(np.int64), m, int(sum_s.value)
+
+    @staticmethod
+    def herding_release():
+        """Return the query's kernel matrix to the device (torch.cuda.empty_cache, as ward_tree does): the caching
+        allocator would otherwise keep its 4 n^2 bytes."""
+        torch.cuda.empty_cache()
+
     # -- K15 / K16 / K17: TypiClust ----------------------------------------------------------------------
     KMEANS_MAX_ITER = 100
 

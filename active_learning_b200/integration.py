@@ -22,6 +22,7 @@ from .query_strategies.cal import CALQuery
 from .query_strategies.balancing import BalancingQuery
 from .query_strategies.margin_clustering import MarginClusteringQuery
 from .query_strategies.mase import BASEQuery, MASEQuery
+from .query_strategies.maxherding import MaxHerdingQuery
 from .query_strategies.probcover import ProbCoverQuery
 from .query_strategies.typiclust import TypiClustQuery
 from .query_strategies.uncertainty import ConfidenceQuery, EntropyQuery, MarginQuery
@@ -44,6 +45,7 @@ _MIXINS = {
     "TypiClustSampler": TypiClustQuery,
     "CALSampler": CALQuery,
     "ALFAMixSampler": ALFAMixQuery,
+    "MaxHerdingSampler": MaxHerdingQuery,
 }
 
 

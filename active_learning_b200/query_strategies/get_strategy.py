@@ -2,8 +2,8 @@
 `get_strategy(name)` returns the class called `name`.  Every class name the reference dispatches is implemented: the
 thirteen accelerated samplers (the seven of the north-star path plus MASE / BASE / Balancing, SURVEY.md section 8f,
 MarginClustering, VAAL and BalancedRandom) and the default RandomSampler.  ProbCoverSampler, TypiClustSampler,
-CALSampler and ALFAMixSampler are this project's additions (no reference counterpart; ProbCoverSampler needs the sampler
-kwarg `delta`)."""
+CALSampler, ALFAMixSampler and MaxHerdingSampler are this project's additions (no reference counterpart; ProbCoverSampler
+needs the sampler kwarg `delta`, MaxHerdingSampler the sampler kwarg `sigma`)."""
 from .alfamix_sampler import ALFAMixSampler  # noqa: F401
 from .badge_sampler import BADGESampler  # noqa: F401
 from .balanced_random_sampler import BalancedRandomSampler  # noqa: F401
@@ -16,6 +16,7 @@ from .entropy_sampler import EntropySampler  # noqa: F401
 from .margin_clustering_sampler import MarginClusteringSampler  # noqa: F401
 from .margin_sampler import MarginSampler  # noqa: F401
 from .mase_sampler import MASESampler  # noqa: F401
+from .maxherding_sampler import MaxHerdingSampler  # noqa: F401
 from .partitioned_badge_sampler import PartitionedBADGESampler  # noqa: F401
 from .partitioned_coreset_sampler import PartitionedCoresetSampler  # noqa: F401
 from .probcover_sampler import ProbCoverSampler  # noqa: F401
@@ -26,7 +27,8 @@ from .vaal_sampler import VAALSampler  # noqa: F401
 ACCELERATED = ("MarginSampler", "ConfidenceSampler", "EntropySampler", "CoresetSampler",
                "PartitionedCoresetSampler", "BADGESampler", "PartitionedBADGESampler", "MASESampler", "BASESampler",
                "BalancingSampler", "MarginClusteringSampler", "VAALSampler", "BalancedRandomSampler",
-               "ProbCoverSampler", "TypiClustSampler", "CALSampler", "ALFAMixSampler")
+               "ProbCoverSampler", "TypiClustSampler", "CALSampler", "ALFAMixSampler",
+               "MaxHerdingSampler")
 NOT_ON_THIS_PATH = ()
 
 

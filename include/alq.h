@@ -593,6 +593,28 @@ int alq_alfamix_rho(alq_ctx* ctx, const float* logits, int64_t n, int32_t c, con
                     const float* anchors, const float* weight, int32_t d, double* rho, double* r2, double* tstar,
                     void* stream);
 
+/* ---- K22 / K23: MaxHerding (Bae, Noh & Sutherland, ECCV 2024) ---------------------------------------------------------
+ * alq_herding_kernel (K22): the Gaussian kernel matrix of the rows of x[n, d] (fp32, ldx >= d, any alignment):
+ *   k[i * ldk + j] = k[j * ldk + i] = fl32(exp(-(s_ij / q))) (fp32, device, ldk >= n), s_ij the exact fp64 d2 of rows i
+ *   and j as alq_pdist_f64 forms it (K7's pair arithmetic: d = a - b, s = s + d * d, k ascending, no FMA), q = *q_host =
+ *   2 sigma^2 formed by the caller.  Exactly symmetric; the diagonal of a finite row is 1.  q must be a finite positive normal
+ *   number (ALQ_ERR_INVALID); a row with a NaN or infinite entry is ALQ_ERR_NUMERIC (the matrix is then undefined).
+ *   n <= 65535 * 64.  Synchronous (one 4-byte copy).
+ * alq_herding_select (K23): the greedy maximisation of F(S) = sum_i max over s in L u S of k[s, i] over that matrix, L
+ *   the rows with labeled != 0.  m_i = max over l in L of k[l, i] (0.0f with none); gain_c = sum over i ascending of
+ *   max(0, (double)k[i, c] - (double)m_i) in fp64.  Each step picks c* = the lowest row of the largest gain among the
+ *   rows with avail != 0 not yet picked, forms S = {i : k[c*, i] > m_i} ascending, subtracts from every candidate's gain
+ *   sum over i in S ascending of (max(0, k[i, c] - m_i) - max(0, k[i, c] - k[c*, i])) (fp64, each operation rounded on
+ *   its own), then sets m_i = k[c*, i] on S.  *n_picks_host = min(budget, rows with avail != 0) steps; picks (int32,
+ *   device) in pick order; m (fp32 [n], device) the final maxima; *sum_s_host (may be NULL) = sum of |S| over the steps.
+ *   One 4-byte copy after the set-up, then three launches per step and no host synchronisation until the end.
+ *   Synchronous. */
+int alq_herding_kernel(alq_ctx* ctx, const float* x, int64_t n, int32_t d, int64_t ldx, const double* q_host, float* k,
+                       int64_t ldk, void* stream);
+int alq_herding_select(alq_ctx* ctx, const float* k, int64_t n, int64_t ldk, const uint8_t* labeled, const uint8_t* avail,
+                       int64_t budget, int32_t* picks, float* m, int64_t* n_picks_host, int64_t* sum_s_host,
+                       void* stream);
+
 #ifdef __cplusplus
 }
 #endif
