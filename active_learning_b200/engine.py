@@ -37,6 +37,58 @@ def _ld(t: torch.Tensor) -> int:
     return t.stride(0) if t.dim() == 2 and t.shape[0] > 1 else t.shape[-1]
 
 
+def _mask(t, n: int, device: torch.device, method: str, name: str) -> torch.Tensor:
+    """t as a contiguous 1-D uint8 view: a uint8 (or bool) CUDA tensor on `device` with n entries, else AlqError."""
+    if (not isinstance(t, torch.Tensor) or not t.is_cuda or t.device != device or t.dtype not in (torch.uint8, torch.bool)
+            or t.numel() != n):
+        raise AlqError(f"{method}: {name} must be a CUDA uint8 (or bool) tensor on {device} with one entry per row "
+                       f"({n})")
+    return t.contiguous().view(torch.uint8).reshape(-1)
+
+
+def _i32(t, shape: Sequence[Optional[int]], device: torch.device, method: str, name: str) -> torch.Tensor:
+    """t contiguous: an int32 CUDA tensor on `device` of `shape` (None: any extent), else AlqError."""
+    if (not isinstance(t, torch.Tensor) or not t.is_cuda or t.device != device or t.dtype != torch.int32
+            or t.dim() != len(shape) or any(s is not None and s != e for s, e in zip(shape, t.shape))):
+        dims = ", ".join("any" if s is None else str(s) for s in shape)
+        raise AlqError(f"{method}: {name} must be an int32 CUDA tensor on {device} of shape [{dims}]")
+    return t.contiguous()
+
+
+def _pad_width(d: int) -> int:
+    """d rounded up to a multiple of 4 (at least 4): the tensor maps want 16-byte rows."""
+    return max(4, (int(d) + 3) & ~3)
+
+
+def _pad4(x: torch.Tensor) -> torch.Tensor:
+    """x with zero columns up to _pad_width (a zero column changes no distance, norm or dot product)."""
+    n, d = x.shape
+    dp = _pad_width(d)
+    if dp == d:
+        return x
+    slab = torch.zeros((n, dp), dtype=torch.float32, device=x.device)
+    slab[:, :d] = x
+    return slab
+
+
+def _finite_rows(x: torch.Tensor, method: str) -> torch.Tensor:
+    """x as float32 CUDA rows padded by _pad4; ValueError (naming `method`) for an empty matrix or a NaN or infinity."""
+    x = _f32c(x, "x")
+    if x.dim() != 2 or x.shape[0] == 0:
+        raise ValueError(f"{method}: need a non-empty [n, d] matrix, got {tuple(x.shape)}")
+    if not bool(torch.isfinite(x).all()):
+        raise ValueError(f"{method}: the embeddings contain NaN or infinity")
+    return _pad4(x)
+
+
+def _check_fits(engine, method: str, n: int, need: int, what: str, shrink: str):
+    """AlqError naming n, the bytes needed (for `what`) and the bytes free when `need` exceeds engine._ward_free_bytes()."""
+    free = engine._ward_free_bytes()
+    if need > free:
+        raise AlqError(f"{method}: n={n} rows need {need} bytes of device memory ({what}); {free} are free; use a "
+                       f"smaller {shrink}")
+
+
 def ward_labels_host(merge_xy: np.ndarray, merge_dist: np.ndarray, n: int, n_clusters: int) -> np.ndarray:
     """alq_ward_labels (host-only, no GPU): K8's discovery-order merge list -> sklearn's labels for n_clusters (int64)."""
     lib = _lib.load()
@@ -631,15 +683,9 @@ class Engine:
     # -- K10: per-class counts and class-balanced picks (BalancedRandomSampler) -----------------------------
     CLASS_MAX = 32768      # ALQ_CLASS_MAX of include/alq.h
 
-    @staticmethod
-    def _class_inputs(labels: torch.Tensor, avail: torch.Tensor, what: str):
-        if not isinstance(labels, torch.Tensor) or not labels.is_cuda or labels.dtype != torch.int32 or labels.dim() != 1:
-            raise AlqError(f"{what}: labels must be a 1-D CUDA int32 tensor")
-        if not isinstance(avail, torch.Tensor) or not avail.is_cuda or avail.dtype not in (torch.uint8, torch.bool):
-            raise AlqError(f"{what}: avail must be a CUDA uint8 (or bool) tensor")
-        if avail.numel() != labels.numel() or avail.device != labels.device:
-            raise AlqError(f"{what}: avail must hold one entry per label on the labels' device")
-        return labels.contiguous(), avail.contiguous().view(torch.uint8).reshape(-1)
+    def _class_inputs(self, labels: torch.Tensor, avail: torch.Tensor, what: str):
+        labels = _i32(labels, (None,), self.device, what, "labels")
+        return labels, _mask(avail, labels.numel(), self.device, what, "avail")
 
     def class_counts(self, labels: torch.Tensor, avail: torch.Tensor, num_classes: int) -> torch.Tensor:
         """K10: counts[c] = number of rows with avail != 0 and labels == c, as a CUDA int32 [num_classes] tensor.
@@ -725,14 +771,8 @@ class Engine:
             raise AlqError(f"{name}: n={n} rows, need n < 2^31")
         if not isinstance(xn, torch.Tensor) or not xn.is_cuda or xn.dtype != torch.float32 or xn.numel() != n:
             raise AlqError(f"{name}: xn must be a CUDA float32 tensor with one entry per row")
-        if not isinstance(labels, torch.Tensor) or not labels.is_cuda or labels.dtype != torch.int32 or labels.numel() != n:
-            raise AlqError(f"{name}: labels must be a CUDA int32 tensor with one entry per row")
-        masks = []
-        for mname, m in (("avail", avail), ("labeled", labeled)):
-            if (not isinstance(m, torch.Tensor) or not m.is_cuda or m.dtype not in (torch.uint8, torch.bool)
-                    or m.numel() != n or m.device != dev):
-                raise AlqError(f"{name}: {mname} must be a CUDA uint8 (or bool) tensor with one entry per row")
-            masks.append(m.contiguous().view(torch.uint8).reshape(-1))
+        labels = _i32(labels, (n,), self.device, name, "labels")
+        masks = [_mask(avail, n, self.device, name, "avail"), _mask(labeled, n, self.device, name, "labeled")]
         c, budget = int(num_classes), int(budget)
         if not 1 <= c <= self.CLASS_MAX:
             raise AlqError(f"{name}: num_classes={c} outside [1, {self.CLASS_MAX}]")
@@ -740,7 +780,7 @@ class Engine:
             raise AlqError(f"{name}: budget={budget} is negative")
         if emb.shape[1] % 4 or _ld(emb) % 4 or emb.data_ptr() % 16:
             raise AlqError(f"{name}: emb needs d and its leading dimension multiples of 4 and a 16-byte aligned base")
-        xn, labels = xn.contiguous().reshape(-1), labels.contiguous()
+        xn = xn.contiguous().reshape(-1)
         so, free_min = None, 0
         if shard_off is not None:
             from .sharding import balancing_agreement
@@ -792,17 +832,8 @@ class Engine:
         delta = float(delta)
         if not (math.isfinite(delta) and delta > 0):
             raise ValueError(f"probcover: delta must be finite and > 0, got {delta}")
-        x = _f32c(x, "x")
-        if x.dim() != 2 or x.shape[0] == 0:
-            raise ValueError(f"probcover: need a non-empty [n, d] matrix, got {tuple(x.shape)}")
-        n, d = x.shape
-        if not bool(torch.isfinite(x).all()):
-            raise ValueError("probcover: the embeddings contain NaN or infinity")
-        dp = max(4, (d + 3) & ~3)
-        if dp != d:                                    # the tensor maps want 16-byte rows: zero columns change no distance
-            slab = torch.zeros((n, dp), dtype=torch.float32, device=x.device)
-            slab[:, :d] = x
-            x = slab
+        x = _finite_rows(x, "probcover")
+        n, dp = x.shape
         nt = (n + 127) // 128
         xhat = torch.empty((n, dp), dtype=torch.float32, device=x.device)
         tile = torch.empty(n * nt, dtype=torch.int32, device=x.device)
@@ -811,11 +842,8 @@ class Engine:
         self._check(self.lib.alq_probcover_graph(self._h, _ptr(x), n, dp, _ld(x), C.byref(dh), _ptr(xhat), _ptr(tile),
                                                  _ptr(row_ptr), None, C.byref(nnz), C.byref(rech), self._stream()),
                     "alq_probcover_graph")
-        need, free = self.probcover_bytes(nnz.value), self._ward_free_bytes()
-        if need > free:
-            raise AlqError(f"probcover: n={n} rows at delta={delta} give nnz={nnz.value} edges, which need {need} bytes of "
-                           f"device memory (4 nnz with {self.PROBCOVER_HEADROOM_BYTES} headroom); {free} are free; use a "
-                           f"smaller delta or subset_unlabeled")
+        _check_fits(self, "probcover", n, self.probcover_bytes(nnz.value), f"4 nnz for nnz={nnz.value} edges at "
+                    f"delta={delta}, with {self.PROBCOVER_HEADROOM_BYTES} headroom", "delta or subset_unlabeled")
         cols = torch.empty(max(nnz.value, 1), dtype=torch.int32, device=x.device)
         self._check(self.lib.alq_probcover_graph(self._h, None, n, dp, dp, C.byref(dh), _ptr(xhat), _ptr(tile),
                                                  _ptr(row_ptr), _ptr(cols), C.byref(nnz), C.byref(rech), self._stream()),
@@ -827,13 +855,11 @@ class Engine:
         of uncovered rows in its ball and covers them, starting from the balls of the rows with labeled != 0 covered, and
         stops early when nothing uncovered is left.  Returns (picks: host int64 array in pick order, greedy steps)."""
         n = row_ptr.numel() - 1
-        if (not labeled.is_cuda or labeled.dtype not in (torch.uint8, torch.bool) or labeled.numel() != n
-                or row_ptr.dtype != torch.int64 or cols.dtype != torch.int32 or not row_ptr.is_cuda or not cols.is_cuda):
-            raise AlqError("probcover_select: row_ptr (int64), cols (int32) and labeled (uint8 or bool, one entry per row) "
-                           "must be CUDA tensors")
+        if row_ptr.dtype != torch.int64 or cols.dtype != torch.int32 or not row_ptr.is_cuda or not cols.is_cuda:
+            raise AlqError("probcover_select: row_ptr (int64) and cols (int32) must be CUDA tensors")
+        lab = _mask(labeled, n, self.device, "probcover_select", "labeled")
         budget = int(budget)
         row_ptr, cols = row_ptr.contiguous(), cols.contiguous()
-        lab = labeled.contiguous().view(torch.uint8).reshape(-1)
         picks = torch.empty(max(budget, 1), dtype=torch.int32, device=row_ptr.device)
         # an empty cols tensor has a null data pointer, which the library refuses: any device address stands in
         cp = _ptr(cols) if cols.numel() else _ptr(row_ptr)
@@ -849,16 +875,13 @@ class Engine:
     def herding_bytes(cls, n: int, d: int) -> int:
         """Device memory a MaxHerding query over n rows of width d needs: the 4 n^2 fp32 kernel matrix, xhat (4 n dp, dp
         = d padded to a multiple of 4), the per-row arrays of the greedy and Ward's headroom."""
-        n, dp = int(n), max(4, (int(d) + 3) & ~3)
-        return 4 * n * n + 4 * n * dp + cls.HERDING_ROW_BYTES * n + cls.WARD_HEADROOM_BYTES
+        n = int(n)
+        return 4 * n * n + 4 * n * _pad_width(d) + cls.HERDING_ROW_BYTES * n + cls.WARD_HEADROOM_BYTES
 
     def herding_guard(self, n: int, d: int):
         """AlqError naming n, the bytes needed and the bytes free when herding_bytes(n, d) does not fit the device."""
-        need, free = self.herding_bytes(n, d), self._ward_free_bytes()
-        if need > free:
-            raise AlqError(f"maxherding: n={n} rows of width {d} need {need} bytes of device memory (the 4 n^2 kernel matrix, "
-                           f"xhat and {self.WARD_HEADROOM_BYTES} headroom); {free} are free; use a smaller "
-                           f"subset_unlabeled")
+        _check_fits(self, "maxherding", n, self.herding_bytes(n, d), f"the 4 n^2 kernel matrix, xhat of width {d} and "
+                    f"{self.WARD_HEADROOM_BYTES} headroom", "subset_unlabeled")
 
     def herding_kernel(self, xhat: torch.Tensor, sigma: float) -> torch.Tensor:
         """K22: the Gaussian kernel matrix K [n, n] (float32 CUDA) of the rows of xhat [n, d] (float32 CUDA):
@@ -887,11 +910,8 @@ class Engine:
         if (not K.is_cuda or K.dtype != torch.float32 or K.dim() != 2 or K.shape[1] != n or K.stride(1) != 1
                 or K.stride(0) < n):
             raise AlqError("herding_select: K must be a square row-major float32 CUDA matrix")
-        masks = []
-        for name, t in (("labeled", labeled), ("avail", avail)):
-            if not t.is_cuda or t.dtype not in (torch.uint8, torch.bool) or t.numel() != n:
-                raise AlqError(f"herding_select: {name} must be a uint8 or bool CUDA mask with one entry per row")
-            masks.append(t.contiguous().view(torch.uint8).reshape(-1))
+        masks = [_mask(labeled, n, self.device, "herding_select", "labeled"),
+                 _mask(avail, n, self.device, "herding_select", "avail")]
         budget = int(budget)
         picks = torch.empty(max(budget, 1), dtype=torch.int32, device=K.device)
         m = torch.empty(n, dtype=torch.float32, device=K.device)
@@ -910,27 +930,10 @@ class Engine:
     # -- K15 / K16 / K17: TypiClust ----------------------------------------------------------------------
     KMEANS_MAX_ITER = 100
 
-    @staticmethod
-    def _pad4(x: torch.Tensor) -> torch.Tensor:
-        """x with zero columns up to a multiple of 4 (the tensor maps want 16-byte rows; a zero column changes no
-        distance, norm or dot product)."""
-        n, d = x.shape
-        dp = max(4, (d + 3) & ~3)
-        if dp == d:
-            return x
-        slab = torch.zeros((n, dp), dtype=torch.float32, device=x.device)
-        slab[:, :d] = x
-        return slab
-
     def normalize(self, x: torch.Tensor) -> torch.Tensor:
         """The rows of x [n, d] L2-normalised exactly as probcover_graph normalises them, padded with zero columns to a
         multiple of 4: xhat [n, dp] float32.  ValueError for n = 0 or non-finite rows."""
-        x = _f32c(x, "x")
-        if x.dim() != 2 or x.shape[0] == 0:
-            raise ValueError(f"normalize: need a non-empty [n, d] matrix, got {tuple(x.shape)}")
-        if not bool(torch.isfinite(x).all()):
-            raise ValueError("normalize: the embeddings contain NaN or infinity")
-        return self._kmeans_rows(self._pad4(x), True)[0]
+        return self._kmeans_rows(_finite_rows(x, "normalize"), True)[0]
 
     def _kmeans_rows(self, x: torch.Tensor, normalise: bool):
         """(xhat, hi, lo, nrm2): K15's row operands; with normalise, xhat = the normalised rows of x."""
@@ -970,8 +973,9 @@ class Engine:
         xhat, centres = self._kmeans_inputs(xhat, centres)
         if labels is None:
             labels = torch.full((xhat.shape[0],), -1, dtype=torch.int32, device=xhat.device)
-        elif labels.dtype != torch.int32 or not labels.is_cuda or labels.numel() != xhat.shape[0] or not labels.is_contiguous():
-            raise AlqError("kmeans_assign: labels must be a contiguous int32 CUDA tensor with one entry per row")
+        elif isinstance(labels, torch.Tensor) and not labels.is_contiguous():
+            raise AlqError("kmeans_assign: labels are updated in place and must be contiguous")
+        labels = _i32(labels, (xhat.shape[0],), self.device, "kmeans_assign", "labels")
         changed, rech = self._assign(self._kmeans_rows(xhat, False), centres, labels)
         return labels, changed, rech
 
@@ -982,10 +986,9 @@ class Engine:
         if (centres.dtype != torch.float32 or not centres.is_cuda or not centres.is_contiguous()
                 or centres.dim() != 2 or centres.shape[1] != xhat.shape[1]):
             raise AlqError("kmeans_update: centres must be a contiguous float32 CUDA tensor [K, d]")
-        if labels.dtype != torch.int32 or not labels.is_cuda or labels.numel() != xhat.shape[0]:
-            raise AlqError("kmeans_update: labels must be an int32 CUDA tensor with one entry per row")
         n, d = xhat.shape
-        self._check(self.lib.alq_kmeans_update(self._h, _ptr(xhat), n, d, _ptr(labels.contiguous()), centres.shape[0],
+        labels = _i32(labels, (n,), self.device, "kmeans_update", "labels")
+        self._check(self.lib.alq_kmeans_update(self._h, _ptr(xhat), n, d, _ptr(labels), centres.shape[0],
                                                _ptr(centres), self._stream()), "alq_kmeans_update")
         return centres
 
@@ -1027,9 +1030,7 @@ class Engine:
         float64 CUDA [len(rows)], host int64 [groups]: the position in rows of each group's largest, lowest on ties).
         k must lie in [1, 32] (AlqError otherwise)."""
         xhat = _f32c(xhat, "xhat").contiguous()
-        if rows.dtype != torch.int32 or not rows.is_cuda:
-            raise AlqError("typicality: rows must be an int32 CUDA tensor")
-        rows = rows.contiguous()
+        rows = _i32(rows, (None,), self.device, "typicality", "rows")
         goff = np.ascontiguousarray(group_off, dtype=np.int64)
         if goff.ndim != 1 or len(goff) < 2 or goff[-1] != rows.numel():
             raise AlqError("typicality: group_off must run from 0 to len(rows)")
@@ -1045,11 +1046,10 @@ class Engine:
         arithmetic), the lowest row on ties; -1 for an empty cluster.  Rows labeled outside [0, K) are skipped.  Returns
         host int64 [K]."""
         xhat, centres = self._kmeans_inputs(xhat, centres)
-        if labels.dtype != torch.int32 or not labels.is_cuda or labels.numel() != xhat.shape[0]:
-            raise AlqError("kmeans_nearest: labels must be an int32 CUDA tensor with one entry per row")
+        labels = _i32(labels, (xhat.shape[0],), self.device, "kmeans_nearest", "labels")
         k = centres.shape[0]
         out = torch.empty(max(k, 1), dtype=torch.int32, device=xhat.device)
-        self._check(self.lib.alq_kmeans_nearest(self._h, _ptr(xhat), xhat.shape[0], xhat.shape[1], _ptr(labels.contiguous()),
+        self._check(self.lib.alq_kmeans_nearest(self._h, _ptr(xhat), xhat.shape[0], xhat.shape[1], _ptr(labels),
                                                 _ptr(centres), k, _ptr(out), self._stream()), "alq_kmeans_nearest")
         return out[:k].cpu().numpy().astype(np.int64)
 
@@ -1065,7 +1065,7 @@ class Engine:
         zl, z = _f32c(logits, "logits").contiguous(), _f32c(emb, "emb").contiguous()
         a, w = _f32c(anchors, "anchors").contiguous(), _f32c(weight, "weight").contiguous()
         if z.dim() == 2 and a.dim() == 2:
-            z, a = self._pad4(z), self._pad4(a)
+            z, a = _pad4(z), _pad4(a)
         if (zl.dim() != 2 or z.dim() != 2 or a.dim() != 2 or w.dim() != 2 or zl.shape[0] != z.shape[0]
                 or zl.shape[1] != w.shape[0] or a.shape[0] != w.shape[0] or a.shape[1] != z.shape[1]
                 or w.shape[1] > z.shape[1]):
@@ -1104,10 +1104,8 @@ class Engine:
         zc, zr = _f32c(cand_logits, "cand_logits").contiguous(), _f32c(ref_logits, "ref_logits").contiguous()
         if zc.dim() != 2 or zr.dim() != 2 or zc.shape[1] != zr.shape[1]:
             raise AlqError(f"cal_scores: need logits [n, C] and [m, C], got {tuple(zc.shape)} and {tuple(zr.shape)}")
-        if idx.dtype != torch.int32 or not idx.is_cuda or idx.dim() != 2 or idx.shape[0] != zc.shape[0]:
-            raise AlqError("cal_scores: idx must be an int32 CUDA tensor [n, k]")
-        idx = idx.contiguous()
         n = zc.shape[0]
+        idx = _i32(idx, (n, None), self.device, "cal_scores", "idx")
         score = torch.empty(n, dtype=torch.float64, device=zc.device)
         key = torch.empty(n, dtype=torch.float32, device=zc.device)
         self._check(self.lib.alq_cal_scores(self._h, _ptr(zc), n, _ptr(zr), zr.shape[0], zc.shape[1], _ptr(idx),

@@ -1,10 +1,9 @@
 """ALFA-Mix (Parvaneh, Abbasnejad, Teney, Haffari, van den Hengel & Shi, "Active Learning by Feature Mixing", CVPR 2022)
 on the device (kernels K16, K20, K13's normalise, K5, K15, K21).
 
-The pool is CoreSet's (`get_idxs_for_coreset`: the same two shuffles, subset_labeled / subset_unlabeled honoured); its
-available rows are the candidates.  One pool forward of the task network gives the logits and the embeddings together
-(BADGE's and CAL's forward; the embedding cache applies under --freeze_feature).  The anchors are the fl32 means of the
-labeled embeddings per class (K16), a class with no labeled row taking the mean of all of them.
+The pool's available rows are the candidates.  One pool forward of the task network gives the logits and the embeddings
+together (BADGE's and CAL's forward; the embedding cache applies under --freeze_feature).  The anchors are the fl32 means
+of the labeled embeddings per class (K16), a class with no labeled row taking the mean of all of them.
 
 The paper mixes each candidate's embedding with every anchor, z + alpha * (a_c - z), at the closed-form alpha that steps
 along the loss gradient, and marks the candidate when the head's prediction changes.  With the algebra carried out, the
@@ -13,12 +12,11 @@ is one number per row, rho = sqrt(D) t* / max_c |a_c - z| (K20): the row flips f
 sqrt(D) exactly when rho < kappa.  The caps kappa_j = j * alpha_step grow until more than `budget` rows flip (or the
 last, j = ceil(1 / alpha_step)).  If no more rows than the budget flip they are all taken; otherwise the flipped rows,
 L2-normalised, are clustered by TypiClust's k-means into `budget` clusters and each non-empty cluster gives its row
-nearest the centre (K21).  The rest of the budget is ProbCover's random fill.  The spec is tests/alfamix_oracle.py.
+nearest the centre (K21).  The rest of the budget is PoolQuery's random fill.  The spec is tests/alfamix_oracle.py.
 
 ALFA-Mix is undefined without labeled rows: the query raises ValueError then.  NumPy draws: the pool's two shuffles, the
 k-means seeding when it runs, the fill when there is a remainder.  The head moves every round, so nothing but the
-embedding cache is kept across rounds.  In a ShardGroup every rank runs the whole query on its own GPU and returns the
-same picks.
+embedding cache is kept across rounds.
 """
 from __future__ import annotations
 
@@ -28,7 +26,7 @@ import numpy as np
 import torch
 
 from .balanced_random import _host_labels
-from .coreset import CoresetQuery
+from .coreset import PoolQuery
 
 
 def cap_walk(rho, budget, alpha_step):
@@ -49,7 +47,7 @@ def cap_walk(rho, budget, alpha_step):
     return np.flatnonzero(rho < j * alpha_step)
 
 
-class ALFAMixQuery(CoresetQuery):
+class ALFAMixQuery(PoolQuery):
     """The rows whose prediction feature mixing with the class anchors changes, spread by k-means."""
     ALPHA_STEP = 2.0 ** -5
     MAX_ITER = 100
@@ -75,13 +73,7 @@ class ALFAMixQuery(CoresetQuery):
         anchors = mean.expand(num_classes, -1).contiguous()
         return eng.kmeans_update(emb_lab, torch.as_tensor(labels.astype(np.int32), device=dev), anchors)
 
-    def query(self, budget):
-        union = np.asarray(self.get_idxs_for_coreset(), dtype=np.int64)      # RNG: two permutations
-        is_lab = self.already_labeled_idxs(boolean=True)[union]
-        avail = self.available_query_idxs(boolean=True)[union]
-        budget = int(min(int(avail.sum()), budget))
-        if budget <= 0:
-            return [], 0
+    def _positions(self, union, is_lab, avail, budget):
         lab_pos, cand_pos = np.flatnonzero(is_lab), np.flatnonzero(avail)
         if not len(lab_pos):
             raise ValueError("ALFAMixSampler needs labeled rows: the anchors are the labeled rows' class means")
@@ -100,18 +92,8 @@ class ALFAMixQuery(CoresetQuery):
                               weight.detach().to(dev, torch.float32))
         cand = cand_pos[cap_walk(rho.cpu().numpy(), budget, self.alpha_step)]
         if len(cand) <= budget:
-            picks = cand
-        else:
-            xhat = eng.normalize(emb.index_select(0, torch.as_tensor(cand, device=dev)))
-            first = int(np.random.choice(len(cand)))                          # TypiClust's seeding draws
-            unif = np.random.random_sample(budget - 1)
-            km_labels, centres, _, _ = eng.kmeans(xhat, first, unif, budget, self.MAX_ITER)
-            near = eng.kmeans_nearest(xhat, km_labels, centres)
-            picks = cand[near[near >= 0]]
-        rest = budget - len(picks)
-        if rest > 0:
-            free = avail.copy()
-            free[picks] = False
-            picks = np.concatenate([picks, np.random.choice(np.flatnonzero(free), rest, replace=False)])
-        labeled_idxs_cur_rd = union[picks].tolist()
-        return labeled_idxs_cur_rd, len(labeled_idxs_cur_rd)
+            return cand
+        xhat = eng.normalize(emb.index_select(0, torch.as_tensor(cand, device=dev)))
+        km_labels, centres, _, _ = self._kmeans(xhat, budget, self.MAX_ITER)
+        near = eng.kmeans_nearest(xhat, km_labels, centres)
+        return cand[near[near >= 0]]

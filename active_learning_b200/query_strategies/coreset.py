@@ -226,6 +226,46 @@ class CoresetQuery(EngineMixin):
         return labeled_idxs_cur_rd, len(labeled_idxs_cur_rd)
 
 
+class PoolQuery(CoresetQuery):
+    """The query body of the samplers that pick from CoreSet's pool by a rule of their own (ProbCover, TypiClust, CAL,
+    ALFA-Mix, MaxHerding).
+
+    The pool is CoreSet's (`get_idxs_for_coreset`: the same two shuffles, subset_labeled / subset_unlabeled honoured) and
+    the budget is clamped to its available rows; a budget <= 0 returns ([], 0) before anything else runs.  A subclass's
+    `_positions` returns pool positions in pick order, possibly fewer than the budget.  One deliberate deviation from the
+    papers: where a sampler's rule runs out of picks (the authors' loops would repeat a pick or index an empty cluster),
+    the rest of the budget is `np.random.choice(available-and-unpicked positions ascending, rest, replace=False)`, drawn
+    only when something is left.  In a ShardGroup every rank runs the whole query on its own GPU and returns the same
+    picks."""
+
+    def query(self, budget):
+        union = np.asarray(self.get_idxs_for_coreset(), dtype=np.int64)      # RNG: two permutations
+        is_lab = self.already_labeled_idxs(boolean=True)[union]
+        avail = self.available_query_idxs(boolean=True)[union]
+        budget = int(min(int(avail.sum()), budget))
+        if budget <= 0:
+            return [], 0
+        picks = self._positions(union, is_lab, avail, budget)
+        rest = budget - len(picks)
+        if rest > 0:
+            free = avail.copy()
+            free[picks] = False
+            picks = np.concatenate([picks, np.random.choice(np.flatnonzero(free), rest, replace=False)])
+        labeled_idxs_cur_rd = union[picks].tolist()
+        return labeled_idxs_cur_rd, len(labeled_idxs_cur_rd)
+
+    def _positions(self, union, is_lab, avail, budget):
+        """Positions in the pool in pick order, at most `budget` of them."""
+        raise NotImplementedError
+
+    def _kmeans(self, xhat, k, max_iter):
+        """Engine.kmeans of the rows of xhat into k clusters, seeded by CoresetQuery's D^2 cold start: one
+        np.random.choice(n) for the first centre, then k - 1 np.random.random_sample uniforms."""
+        first = int(np.random.choice(xhat.shape[0]))
+        unif = np.random.random_sample(k - 1)
+        return self.get_engine().kmeans(xhat, first, unif, k, max_iter)
+
+
 class PartitionedCoresetQuery(CoresetQuery):
     """partitioned_coreset_sampler.py: the selection runs independently inside `partitions` random
     groups.  Here the groups are one batch dimension of the same kernels (and, multi-GPU, the unit

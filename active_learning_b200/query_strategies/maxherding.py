@@ -1,17 +1,16 @@
 """MaxHerding (Bae, Noh & Sutherland, "Generalized Coverage for More Robust Low-Budget Active Learning", ECCV 2024) on the
 device (kernels K22, K23).
 
-The pool is CoreSet's (`get_idxs_for_coreset`: the same two shuffles, subset_labeled / subset_unlabeled honoured).  Its
-embeddings are L2-normalised as ProbCover normalises them, and K22 forms the Gaussian kernel matrix
+The pool's embeddings are L2-normalised as ProbCover normalises them, and K22 forms the Gaussian kernel matrix
 K_ij = fl32(exp(-(s_ij / q))) of the exact fp64 squared distances s_ij (K7's pair arithmetic), q = 2 sigma^2.  The greedy
 (K23) then maximises the generalised coverage F(S) = sum_i max_{s in L u S} K_is over the labeled rows L and the picks S,
 one available row at a time: the lowest position of the largest gain.  The gains are kept incrementally: a pick changes
 only the rows it now covers best, so a step reads those rows of K instead of all of it.  Once every gain is 0 (a kernel
-that underflowed at a small sigma) the lowest free position is taken; there is no NumPy draw after the two shuffles.
+that underflowed at a small sigma) the lowest free position is taken, so the greedy always fills the budget and there is
+no NumPy draw after the two shuffles.
 
 The n x n fp32 matrix (4 n^2 bytes: 53.7 GB at ImageNet-LT's 115 846 rows) is checked against the free device memory
-before anything is allocated, and released before the query returns: nothing is kept across rounds.  In a ShardGroup
-every rank runs the whole query on its own GPU and returns the same picks.
+before anything is allocated, and released before the query returns: nothing is kept across rounds.
 """
 from __future__ import annotations
 
@@ -21,7 +20,7 @@ import sys
 import numpy as np
 import torch
 
-from .coreset import CoresetQuery
+from .coreset import PoolQuery
 
 
 def herding_q(sigma):
@@ -38,7 +37,7 @@ def herding_q(sigma):
     return q
 
 
-class MaxHerdingQuery(CoresetQuery):
+class MaxHerdingQuery(PoolQuery):
     """Greedy maximum generalised coverage of CoreSet's pool under a Gaussian kernel."""
 
     def __init__(self, *args, **kwargs):
@@ -46,13 +45,7 @@ class MaxHerdingQuery(CoresetQuery):
         self.sigma = kwargs.get("sigma")
         herding_q(self.sigma)
 
-    def query(self, budget):
-        union = np.asarray(self.get_idxs_for_coreset(), dtype=np.int64)      # RNG: two permutations
-        is_lab = self.already_labeled_idxs(boolean=True)[union]
-        avail = self.available_query_idxs(boolean=True)[union]
-        budget = int(min(int(avail.sum()), budget))
-        if budget <= 0:
-            return [], 0
+    def _positions(self, union, is_lab, avail, budget):
         eng = self.get_engine()
         feats, _ = self._features(union.tolist())
         eng.herding_guard(feats.shape[0], feats.shape[1])
@@ -65,5 +58,4 @@ class MaxHerdingQuery(CoresetQuery):
         finally:
             del K
             eng.herding_release()
-        labeled_idxs_cur_rd = union[picks].tolist()
-        return labeled_idxs_cur_rd, len(labeled_idxs_cur_rd)
+        return picks

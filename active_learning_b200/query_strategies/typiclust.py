@@ -1,28 +1,25 @@
 """TypiClust (Hacohen, Dekel & Weinshall, "Active Learning on a Budget: Opposite Strategies Suit High and Low Budgets",
 ICML 2022) on the device (kernels K5, K15, K16, K17).
 
-The pool is CoreSet's (`get_idxs_for_coreset`: the same two shuffles, subset_labeled / subset_unlabeled honoured).  Its
-embeddings are L2-normalised as ProbCover normalises them and clustered by k-means into K = min(|labeled| + budget,
-MAX_NUM_CLUSTERS) clusters: k-means++ seeding is CoresetQuery's D^2 cold start (one np.random.choice(n), then K - 1
-np.random.random_sample uniforms), then Lloyd's loop with exact fp64 assignments (K15) and sequential fp64 means (K16)
-until no label changes, at most MAX_ITER assignments.
+The pool's embeddings are L2-normalised as ProbCover normalises them and clustered by k-means into K = min(|labeled| +
+budget, MAX_NUM_CLUSTERS) clusters: PoolQuery's k-means++ seeding draws, then Lloyd's loop with exact fp64 assignments
+(K15) and sequential fp64 means (K16) until no label changes, at most MAX_ITER assignments.
 
 Selection follows the authors' loop: clusters with more than MIN_CLUSTER_SIZE rows, ordered by (labeled rows ascending,
 size descending, id ascending), are visited cyclically; each visit takes the cluster's most typical available, unpicked
 row, typicality = 1 / (mean squared distance to its k = min(K_NN, m // 2) nearest such rows + 1e-5) (K17, one launch per
-cycle of the walk).  Two deliberate deviations, both where the authors' loop would index an empty cluster and fail: a
-visit to a cluster with no row left is skipped and uses no budget, and once every kept cluster is exhausted the rest of
-the budget is `np.random.choice(available-and-unpicked positions ascending, rest, replace=False)`, ProbCover's fill.
+cycle of the walk).  A visit to a cluster with no row left, where the authors' loop would index an empty cluster and fail,
+is skipped and uses no budget; once every kept cluster is exhausted PoolQuery's random fill takes the rest of the budget.
 
 K changes with the labeled set and the seeding draws every round, so nothing but the embedding cache is kept across
-rounds.  In a ShardGroup every rank runs the whole query on its own GPU and returns the same picks.
+rounds.
 """
 from __future__ import annotations
 
 import numpy as np
 import torch
 
-from .coreset import CoresetQuery
+from .coreset import PoolQuery
 
 
 def cluster_order(labels, is_lab, k, min_size):
@@ -33,7 +30,7 @@ def cluster_order(labels, is_lab, k, min_size):
     return ids[np.lexsort((ids, -size[ids], existing[ids]))]
 
 
-class TypiClustQuery(CoresetQuery):
+class TypiClustQuery(PoolQuery):
     """The most typical row of each uncovered k-means cluster of CoreSet's pool."""
     MAX_NUM_CLUSTERS = 500
     MIN_CLUSTER_SIZE = 5
@@ -62,27 +59,10 @@ class TypiClustQuery(CoresetQuery):
             free[new] = False
         return np.asarray(picks, dtype=np.int64)
 
-    def query(self, budget):
-        union = np.asarray(self.get_idxs_for_coreset(), dtype=np.int64)      # RNG: two permutations
-        is_lab = self.already_labeled_idxs(boolean=True)[union]
-        avail = self.available_query_idxs(boolean=True)[union]
-        budget = int(min(int(avail.sum()), budget))
-        if budget <= 0:
-            return [], 0
-        eng = self.get_engine()
+    def _positions(self, union, is_lab, avail, budget):
         feats, _ = self._features(union.tolist())
-        xhat = eng.normalize(feats)
-        n = len(union)
+        xhat = self.get_engine().normalize(feats)
         k = min(int(is_lab.sum()) + budget, self.MAX_NUM_CLUSTERS)
-        first = int(np.random.choice(n))                                      # CoresetQuery's D^2 cold start
-        unif = np.random.random_sample(k - 1)
-        labels, _, _, _ = eng.kmeans(xhat, first, unif, k, self.MAX_ITER)
+        labels, _, _, _ = self._kmeans(xhat, k, self.MAX_ITER)
         labels = labels.cpu().numpy().astype(np.int64)
-        picks = self._walk(xhat, labels, is_lab, avail, budget)
-        rest = budget - len(picks)
-        if rest > 0:                     # every kept cluster exhausted: the deliberate deviation above
-            free = avail.copy()
-            free[picks] = False
-            picks = np.concatenate([picks, np.random.choice(np.flatnonzero(free), rest, replace=False)])
-        labeled_idxs_cur_rd = union[picks].tolist()
-        return labeled_idxs_cur_rd, len(labeled_idxs_cur_rd)
+        return self._walk(xhat, labels, is_lab, avail, budget)

@@ -52,3 +52,26 @@ def test_empty_and_degenerate_inputs(eng):
     x = torch.zeros(8, 4, device="cuda")                             # all rows identical
     picks = eng.greedy_select(x, eng.row_norm2(x), torch.zeros(8, device="cuda"), [0, 8], [8])
     assert picks.tolist() == list(range(8))                          # every tie resolves to the lowest row
+
+
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs a second GPU")
+def test_int32_and_mask_arguments_on_another_gpu_are_refused(eng):
+    """Their pointers would be another device's addresses: refused before any launch, as the class and balancing calls
+    refuse them."""
+    from active_learning_b200._lib import AlqError
+    other = torch.device("cuda", (eng.device_index + 1) % torch.cuda.device_count())
+    n = 64
+    x = torch.nn.functional.normalize(torch.randn(n, 8, device=eng.device), dim=1)
+    mask = torch.zeros(n, dtype=torch.uint8, device=other)
+    labels = torch.zeros(n, dtype=torch.int32, device=other)
+    with pytest.raises(AlqError, match="herding_select: labeled"):
+        eng.herding_select(torch.eye(n, device=eng.device), mask, mask.to(eng.device), 1)
+    row_ptr = torch.zeros(n + 1, dtype=torch.int64, device=eng.device)
+    with pytest.raises(AlqError, match="probcover_select: labeled"):
+        eng.probcover_select(row_ptr, torch.zeros(0, dtype=torch.int32, device=eng.device), mask, 1)
+    with pytest.raises(AlqError, match="kmeans_assign: labels"):
+        eng.kmeans_assign(x, x[:4].clone(), labels)
+    with pytest.raises(AlqError, match="kmeans_update: labels"):
+        eng.kmeans_update(x, labels, x[:4].clone())
+    with pytest.raises(AlqError, match="kmeans_nearest: labels"):
+        eng.kmeans_nearest(x, labels, x[:4].clone())
