@@ -204,16 +204,18 @@ extern "C" int alq_alfamix_rho(alq_ctx* ctx, const float* logits, int64_t n, int
     // (gridDim.y) within CUDA's 65 535
     const int chunk = std::min({ni, 65535 * TT, std::max(TT, static_cast<int>(((1LL << 25) / c) / TT * TT))});
     const size_t cc = static_cast<size_t>(c) * c, rc = static_cast<size_t>(chunk) * c;
-    int rcode = alq_scratch_reserve(ctx, scratch_need({cc * 8, rc * 8, rc * 8, static_cast<size_t>(chunk) * 4,
-                                                       static_cast<size_t>(n) * 8, 4}));
+    double *g, *r, *w, *r2s;
+    int* yhat;
+    unsigned int* bad;
+    int rcode = alq_scratch_carve(ctx, [&](ScratchCursor& cur) {
+        g = cur.take<double>(cc);
+        r = cur.take<double>(rc);
+        w = cur.take<double>(rc);
+        yhat = cur.take<int>(chunk);
+        r2s = cur.take<double>(n);
+        bad = cur.take<unsigned int>(1);
+    });
     if (rcode) return rcode;
-    ScratchCursor cur(ctx->scratch);
-    double* g = cur.take<double>(cc);
-    double* r = cur.take<double>(rc);
-    double* w = cur.take<double>(rc);
-    int* yhat = cur.take<int>(chunk);
-    double* r2s = cur.take<double>(n);
-    unsigned int* bad = cur.take<unsigned int>(1);
     if (!r2) r2 = r2s;
 
     ALQ_CUDA(ctx, cudaMemsetAsync(bad, 0, 4, st));

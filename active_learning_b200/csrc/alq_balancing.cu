@@ -324,6 +324,7 @@ struct BalLoop {
     static constexpr int kThreads = kBalThreads;
     static constexpr auto kernel = balancing_loop_kernel;
     size_t smem = 0, sum_smem = 0;
+    double *partial = nullptr, *sums0 = nullptr;
 
     int plan_smem(alq_ctx* ctx, BalCall& B) {
         smem = bal_loop_smem(B.c, B.d, B.nseg);
@@ -334,22 +335,19 @@ struct BalLoop {
         return ALQ_OK;
     }
     static int nchunks(const BalCall& B) { return (B.n + kSumChunk - 1) / kSumChunk; }
-    // all of K11's scratch, reserved with the counts' (the first four) and sized from the shape
-    size_t need_with_counts(const BalCall& B) const {
+    template <class Bytes>
+    int fits(alq_ctx*, BalCall&, Bytes&&) { return ALQ_OK; }
+    // the fp64 class sums: per chunk, the labeled rows' and every CTA's running copy
+    void carve(ScratchCursor& cur, const BalCall& B, size_t, BalArgs& A) {
         const size_t cd = static_cast<size_t>(B.c) * B.d;
-        return scratch_need({B.entries * 4, static_cast<size_t>(B.c) * 4, 8, static_cast<size_t>(B.nseg) * 4,
-                             static_cast<size_t>(nchunks(B)) * cd * 8, cd * 8, static_cast<size_t>(B.S.grid) * cd * 8,
-                             static_cast<size_t>(B.n), (kMtN + 1) * 4 * 2, B.sharded ? 0 : B.words_max, 16});
+        partial = cur.take<double>(static_cast<size_t>(nchunks(B)) * cd);
+        A.sums0 = sums0 = cur.take<double>(cd);
+        A.sums = cur.take<double>(static_cast<size_t>(B.S.grid) * cd);
     }
-    // the fp64 class sums
-    int setup(alq_ctx* ctx, BalCall& B, ScratchCursor& cur, BalArgs& A) {
+    int setup(alq_ctx* ctx, BalCall& B, BalArgs& A) {
         const alq_balancing_desc* D = B.D;
         const int n = B.n, c = B.c, d = B.d, nch = nchunks(B);
         const size_t cd = static_cast<size_t>(c) * d;
-        double* partial = cur.take<double>(static_cast<size_t>(nch) * cd);
-        double* sums0 = cur.take<double>(cd);
-        A.sums = cur.take<double>(static_cast<size_t>(B.S.grid) * cd);
-        A.sums0 = sums0;
         A.xn = D->xn;
         if (sum_smem > 48u * 1024u)
             ALQ_CUDA(ctx, cudaFuncSetAttribute(bal_class_sum_partial_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(sum_smem)));

@@ -132,6 +132,11 @@ struct BalCall {
     int budget;                                  // at most n_avail
     int32_t* counts;                             // counts_h and seg_h on the device
     int32_t* seg_avail;
+    size_t avail_of(int r) const {               // the available rows of rank r's segments
+        int64_t a = 0;
+        for (int g = r * S.grid; g < (r + 1) * S.grid; ++g) a += seg_h[g];
+        return static_cast<size_t>(a);
+    }
 };
 
 size_t up128(size_t v) { return (v + 127) & ~size_t(127); }
@@ -145,9 +150,10 @@ size_t bal_words_bytes(const SegShard& S, int64_t budget, bool sharded) {
 // The body of both entry points, alq_balancing_select (K11) and alq_balancing_table_select (K12).  K's steps, in the
 // order they run:
 //   int plan_smem(ctx, BalCall&)                       the shared-memory limit; sets smem, the loop's dynamic shared memory
-//   size_t need_with_counts(const BalCall&)            scratch reserved together with the counts' (0: theirs alone)
-//   int setup(ctx, BalCall&, ScratchCursor&, Args&)    after the counts: the loop's own limits, scratch (continuing
-//                                                      behind the counts' or from a new reservation) and set-up launches
+//   int fits(ctx, BalCall&, bytes_for)                 after the counts: the loop's memory limits; bytes_for(na) measures
+//                                                      the call's scratch layout with na available rows on the rank
+//   void carve(ScratchCursor&, const BalCall&, na, Args&)   the loop's own buffers in that layout
+//   int setup(ctx, BalCall&, Args&)                    its set-up uploads and launches
 template <class K>
 int bal_select(alq_ctx* ctx, const alq_balancing_desc* D, void* stream) {
     if (!ctx) return ALQ_ERR_INVALID;
@@ -224,14 +230,16 @@ int bal_select(alq_ctx* ctx, const alq_balancing_desc* D, void* stream) {
     // ---- set-up: K10's table pass over the labeled rows (the counts) and one launch counting the available rows of
     // every global segment; a labeled or available row whose label is outside [0, c) fails naming the row and its label
     B.entries = alq_class_table_entries(n, c);
-    rc = alq_scratch_reserve(ctx, std::max(scratch_need({B.entries * 4, static_cast<size_t>(c) * 4, 8, static_cast<size_t>(nseg) * 4}),
-                                           k.need_with_counts(B)));
+    int32_t* tab;
+    unsigned int* bad;
+    auto counts_layout = [&](ScratchCursor& cur) {
+        tab = cur.take<int32_t>(B.entries);
+        B.counts = cur.take<int32_t>(c);
+        bad = cur.take<unsigned int>(2);
+        B.seg_avail = cur.take<int32_t>(nseg);
+    };
+    rc = alq_scratch_carve(ctx, counts_layout);
     if (rc != ALQ_OK) return rc;
-    ScratchCursor cur(ctx->scratch);
-    int32_t* tab = cur.take<int32_t>(B.entries);
-    B.counts = cur.take<int32_t>(c);
-    unsigned int* bad = cur.take<unsigned int>(2);
-    B.seg_avail = cur.take<int32_t>(nseg);
     ALQ_CUDA(ctx, cudaMemsetAsync(bad, 0xff, 2 * sizeof(unsigned int), st));
     rc = alq_class_table_pass(ctx, D->labels, D->labeled, n, c, tab, bad, B.counts, st);
     if (rc != ALQ_OK) return rc;
@@ -262,15 +270,30 @@ int bal_select(alq_ctx* ctx, const alq_balancing_desc* D, void* stream) {
         return ALQ_OK;
     }
 
-    // ---- the loop's own set-up, the working mask, the RNG state -------------------------------------------------------
+    // ---- the call's whole scratch: the counts' buffers, the loop's own, the working mask, the RNG state, the words and
+    // the status.  The carve may move the arena, so the counts go up again from the host.  Then the loop's own set-up.
     typename K::Args A{};
-    rc = k.setup(ctx, B, cur, A);
-    if (rc != ALQ_OK || B.declined) return rc;
     const size_t words = bal_words_bytes(S, B.budget, B.sharded);
-    uint8_t* avail = cur.take<uint8_t>(n);
-    unsigned int* mt = cur.take<unsigned int>(2 * (kMtN + 1));
-    char* word_scratch = cur.take<char>(B.sharded ? 0 : words);
-    int* small = cur.take<int>(4);                                    // [0] status, [1] balancing steps
+    uint8_t* avail;
+    unsigned int* mt;
+    char* word_scratch;
+    int* small;
+    auto layout = [&](ScratchCursor& cur, size_t na) {
+        counts_layout(cur);
+        k.carve(cur, B, na, A);
+        avail = cur.take<uint8_t>(n);
+        mt = cur.take<unsigned int>(2 * (kMtN + 1));
+        word_scratch = cur.take<char>(B.sharded ? 0 : words);
+        small = cur.take<int>(4);                                     // [0] status, [1] balancing steps
+    };
+    rc = k.fits(ctx, B, [&](size_t na) { return alq_layout_bytes([&](ScratchCursor& cur) { layout(cur, na); }); });
+    if (rc != ALQ_OK || B.declined) return rc;
+    rc = alq_scratch_carve(ctx, [&](ScratchCursor& cur) { layout(cur, B.avail_of(S.rank)); });
+    if (rc != ALQ_OK) return rc;
+    ALQ_CUDA(ctx, cudaMemcpyAsync(B.counts, B.counts_h.data(), static_cast<size_t>(c) * 4, cudaMemcpyHostToDevice, st));
+    ALQ_CUDA(ctx, cudaMemcpyAsync(B.seg_avail, B.seg_h.data(), static_cast<size_t>(nseg) * 4, cudaMemcpyHostToDevice, st));
+    rc = k.setup(ctx, B, A);
+    if (rc != ALQ_OK) return rc;
     std::vector<unsigned int> mt_h(kMtN + 1);
     std::copy(D->mt_key_host, D->mt_key_host + kMtN, mt_h.begin());
     mt_h[kMtN] = static_cast<unsigned int>(*D->mt_pos_host);

@@ -487,64 +487,62 @@ struct TabLoop {
         smem = bal_table_smem(c, d, nseg, pend_cap);
         return ALQ_OK;
     }
-    // the table's rows are the available rows: sized after the counts
-    size_t need_with_counts(const BalCall&) const { return 0; }
-    // the table and the per-CTA sums must fit the device's free memory: checked before anything is reserved for them;
-    // then the table slots, the fp64 class sums in row order per class and their squared norms
-    int setup(alq_ctx* ctx, BalCall& B, ScratchCursor& cur, TabArgs& A) {
+    int32_t *off = nullptr, *slot_lo = nullptr, *grp = nullptr;
+    double *sums0 = nullptr, *q0 = nullptr;
+
+    // the table and the per-CTA sums must fit the device's free memory: checked before anything is reserved for them
+    template <class Bytes>
+    int fits(alq_ctx* ctx, BalCall& B, Bytes&& bytes_for) {
         const alq_balancing_desc* D = B.D;
         const SegShard& S = B.S;
-        const cudaStream_t st = B.st;
-        const int n = B.n, c = B.c, d = B.d, grid = S.grid, nseg = B.nseg;
-        std::vector<int64_t> avail_of(S.world, 0);                    // available rows per rank: its table rows
-        for (int g = 0; g < nseg; ++g) avail_of[g / grid] += B.seg_h[g];
-        const size_t cd = static_cast<size_t>(c) * d;
-        const size_t words_b = bal_words_bytes(S, B.budget, B.sharded);
-        auto need_for = [&](size_t na) {
-            return scratch_need({static_cast<size_t>(c) * 4, static_cast<size_t>(nseg) * 4, static_cast<size_t>(c + 1) * 4,
-                                 static_cast<size_t>(grid) * 4, static_cast<size_t>(std::max<int64_t>(B.labeled_total, 1)) * 4,
-                                 cd * 8, static_cast<size_t>(c) * 8, static_cast<size_t>(grid) * cd * 8, na * c * 8,
-                                 na * 8, na * 4, static_cast<size_t>(n), (kMtN + 1) * 4 * 2, B.sharded ? 0 : words_b, 16});
-        };
-        const size_t na = static_cast<size_t>(avail_of[S.rank]);
-        const size_t need = need_for(na);
+        const int c = B.c, grid = S.grid;
+        const size_t cd = static_cast<size_t>(c) * B.d;
         if (B.sharded) {
             // the same decision on every rank: every rank's share against the group's least free memory (the caller's
             // gather; this context's scratch is not counted, so the check is conservative)
             for (int r = 0; r < S.world; ++r) {
-                const size_t nr = need_for(static_cast<size_t>(avail_of[r]));
-                const size_t want = nr + (nr >> 2) + (1u << 20);            // what alq_scratch_reserve allocates
+                const size_t na = B.avail_of(r);
+                const size_t want = alq_scratch_alloc_bytes(bytes_for(na));
                 if (D->group_free_bytes < 0 || want > static_cast<size_t>(D->group_free_bytes))
                     BAL_LIMIT(B, "%s: rank %d's %lld x %d table (%zu bytes) and %d copies of the class sums (%zu bytes) need "
                               "%zu bytes of device memory, the group has %lld free (limit: table in device memory)", kName, r,
-                              (long long)avail_of[r], c, static_cast<size_t>(avail_of[r]) * c * 8, grid,
-                              static_cast<size_t>(grid) * cd * 8, want, (long long)D->group_free_bytes);
+                              (long long)na, c, na * c * 8, grid, static_cast<size_t>(grid) * cd * 8, want,
+                              (long long)D->group_free_bytes);
             }
-        } else if (need > ctx->scratch_bytes) {
+            return ALQ_OK;
+        }
+        const size_t na = B.avail_of(S.rank), need = bytes_for(na);
+        if (need > ctx->scratch_bytes) {
             size_t free_b = 0, total_b = 0;
             ALQ_CUDA(ctx, cudaMemGetInfo(&free_b, &total_b));
-            const size_t want = need + (need >> 2) + (1u << 20);           // what alq_scratch_reserve allocates
+            const size_t want = alq_scratch_alloc_bytes(need);
             if (want > free_b + ctx->scratch_bytes)
                 BAL_LIMIT(B, "%s: the %lld x %d table (%zu bytes) and %d copies of the class sums (%zu bytes) need %zu bytes "
                           "of device memory, %zu are free (limit: table in device memory)", kName, (long long)B.n_avail, c,
                           na * c * 8, grid, static_cast<size_t>(grid) * cd * 8, want, free_b + ctx->scratch_bytes);
         }
-        const int rc = alq_scratch_reserve(ctx, need);
-        if (rc != ALQ_OK) return rc;
-        cur = ScratchCursor(ctx->scratch);                            // the counts move to the front of the new scratch
-        B.counts = cur.take<int32_t>(c);
-        B.seg_avail = cur.take<int32_t>(nseg);
-        int32_t* off = cur.take<int32_t>(c + 1);
-        int32_t* slot_lo = cur.take<int32_t>(grid);
-        int32_t* grp = cur.take<int32_t>(static_cast<size_t>(std::max<int64_t>(B.labeled_total, 1)));
-        double* sums0 = cur.take<double>(cd);
-        double* q0 = cur.take<double>(c);
-        A.sums0 = sums0; A.q0 = q0;
+        return ALQ_OK;
+    }
+    // the table slots, the fp64 class sums in row order per class and their squared norms, the per-CTA sums and the
+    // table of the rank's na available rows
+    void carve(ScratchCursor& cur, const BalCall& B, size_t na, TabArgs& A) {
+        const int c = B.c, grid = B.S.grid;
+        const size_t cd = static_cast<size_t>(c) * B.d;
+        off = cur.take<int32_t>(c + 1);
+        A.slot_lo = slot_lo = cur.take<int32_t>(grid);
+        grp = cur.take<int32_t>(static_cast<size_t>(std::max<int64_t>(B.labeled_total, 1)));
+        A.sums0 = sums0 = cur.take<double>(cd);
+        A.q0 = q0 = cur.take<double>(c);
         A.sums = cur.take<double>(static_cast<size_t>(grid) * cd);
         A.table = cur.take<double>(na * c);
         A.xn64 = cur.take<double>(na);
         A.slot_row = cur.take<int32_t>(na);
-        A.slot_lo = slot_lo;
+    }
+    int setup(alq_ctx* ctx, BalCall& B, TabArgs& A) {
+        const alq_balancing_desc* D = B.D;
+        const SegShard& S = B.S;
+        const cudaStream_t st = B.st;
+        const int n = B.n, c = B.c, d = B.d, grid = S.grid;
         A.pend_cap = pend_cap;
 
         // table slots: the available rows of this rank's segments only
@@ -552,8 +550,6 @@ struct TabLoop {
         off_h[0] = 0;
         for (int k = 0; k < c; ++k) off_h[k + 1] = off_h[k] + B.counts_h[k];
         for (int b = 0, s = 0; b < grid; ++b) { slot_lo_h[b] = s; s += B.seg_h[S.rank * grid + b]; }
-        ALQ_CUDA(ctx, cudaMemcpyAsync(B.counts, B.counts_h.data(), static_cast<size_t>(c) * 4, cudaMemcpyHostToDevice, st));
-        ALQ_CUDA(ctx, cudaMemcpyAsync(B.seg_avail, B.seg_h.data(), static_cast<size_t>(nseg) * 4, cudaMemcpyHostToDevice, st));
         ALQ_CUDA(ctx, cudaMemcpyAsync(off, off_h.data(), static_cast<size_t>(c + 1) * 4, cudaMemcpyHostToDevice, st));
         ALQ_CUDA(ctx, cudaMemcpyAsync(slot_lo, slot_lo_h.data(), static_cast<size_t>(grid) * 4, cudaMemcpyHostToDevice, st));
 

@@ -388,24 +388,25 @@ extern "C" int alq_knn(alq_ctx* ctx, const float* x, int64_t n, const float* y, 
     const cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int ni = static_cast<int>(n), mi = static_cast<int>(m);
     const size_t xe = static_cast<size_t>(n) * d, ye = static_cast<size_t>(m) * d;
-    int rc = alq_scratch_reserve(ctx, scratch_need({xe * 4, xe * 4, ye * 4, ye * 4, static_cast<size_t>(n) * 8,
-                                                    static_cast<size_t>(n) * 8, static_cast<size_t>(m) * 8,
-                                                    static_cast<size_t>(m) * 8, static_cast<size_t>(n) * S * 4,
-                                                    static_cast<size_t>(n) * 4, static_cast<size_t>(n) * 4, 8}));
+    float *xhi, *xlo, *yhi, *ylo, *lstar;
+    double *nx, *sx, *ny, *sy;
+    int *cand, *list;
+    unsigned int* cnt;                                      // [0] rows refused by their norm, [1] rows listed
+    int rc = alq_scratch_carve(ctx, [&](ScratchCursor& cur) {
+        xhi = cur.take<float>(xe);
+        xlo = cur.take<float>(xe);
+        yhi = cur.take<float>(ye);
+        ylo = cur.take<float>(ye);
+        nx = cur.take<double>(n);
+        sx = cur.take<double>(n);
+        ny = cur.take<double>(m);
+        sy = cur.take<double>(m);
+        cand = cur.take<int>(static_cast<size_t>(n) * S);
+        lstar = cur.take<float>(n);
+        list = cur.take<int>(n);
+        cnt = cur.take<unsigned int>(2);
+    });
     if (rc) return rc;
-    ScratchCursor cur(ctx->scratch);
-    float* xhi = cur.take<float>(xe);
-    float* xlo = cur.take<float>(xe);
-    float* yhi = cur.take<float>(ye);
-    float* ylo = cur.take<float>(ye);
-    double* nx = cur.take<double>(n);
-    double* sx = cur.take<double>(n);
-    double* ny = cur.take<double>(m);
-    double* sy = cur.take<double>(m);
-    int* cand = cur.take<int>(static_cast<size_t>(n) * S);
-    float* lstar = cur.take<float>(n);
-    int* list = cur.take<int>(n);
-    unsigned int* cnt = cur.take<unsigned int>(2);          // [0] rows refused by their norm, [1] rows listed
     ALQ_CUDA(ctx, cudaMemsetAsync(cnt, 0, 8, st));
     rs::normalize_split_kernel<<<(ni + rs::NORM_WARPS - 1) / rs::NORM_WARPS, rs::NORM_WARPS * 32, 0, st>>>(
         nullptr, ni, d, d, const_cast<float*>(x), xhi, xlo, nx, 0);
@@ -463,11 +464,12 @@ extern "C" int alq_cal_scores(alq_ctx* ctx, const float* cand_logits, int64_t n,
     if (!cand_logits || !ref_logits || !idx || !score || !key) ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_cal_scores: null pointer");
     const cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int ni = static_cast<int>(n), mi = static_cast<int>(m);
-    int rc = alq_scratch_reserve(ctx, scratch_need({static_cast<size_t>(n) * 8, static_cast<size_t>(m) * 8}));
+    double *lse_c, *lse_r;
+    int rc = alq_scratch_carve(ctx, [&](ScratchCursor& cur) {
+        lse_c = cur.take<double>(n);
+        lse_r = cur.take<double>(m);
+    });
     if (rc) return rc;
-    ScratchCursor cur(ctx->scratch);
-    double* lse_c = cur.take<double>(n);
-    double* lse_r = cur.take<double>(m);
     cal_lse_kernel<<<(ni + 255) / 256, 256, 0, st>>>(cand_logits, ni, c, lse_c);
     ALQ_LAUNCH_CHECK(ctx);
     cal_lse_kernel<<<(mi + 255) / 256, 256, 0, st>>>(ref_logits, mi, c, lse_r);

@@ -215,11 +215,13 @@ extern "C" int alq_class_counts(alq_ctx* ctx, const int32_t* labels, const uint8
         return ALQ_OK;
     }
     const size_t entries = alq_class_table_entries(n, c);
-    int rc = alq_scratch_reserve(ctx, scratch_need({entries * sizeof(int32_t), sizeof(unsigned int)}));
+    int32_t* tab;
+    unsigned int* bad;
+    int rc = alq_scratch_carve(ctx, [&](ScratchCursor& cur) {
+        tab = cur.take<int32_t>(entries);
+        bad = cur.take<unsigned int>(1);
+    });
     if (rc != ALQ_OK) return rc;
-    ScratchCursor cur(ctx->scratch);
-    int32_t* tab = cur.take<int32_t>(entries);
-    unsigned int* bad = cur.take<unsigned int>(1);
     ALQ_CUDA(ctx, cudaMemsetAsync(bad, 0xff, sizeof(unsigned int), st));
     rc = alq_class_table_pass(ctx, labels, avail, static_cast<int>(n), c, tab, bad, counts, st);
     if (rc != ALQ_OK) return rc;
@@ -250,11 +252,12 @@ extern "C" int alq_class_pick(alq_ctx* ctx, const int32_t* labels, const uint8_t
         return ALQ_OK;
     }
     const size_t entries = alq_class_table_entries(n, c);
-    int rc = alq_scratch_reserve(ctx, scratch_need({entries * sizeof(int32_t), (static_cast<size_t>(c) + 1) * sizeof(int32_t)}));
+    int32_t *tab, *koff;
+    int rc = alq_scratch_carve(ctx, [&](ScratchCursor& cur) {
+        tab = cur.take<int32_t>(entries);
+        koff = cur.take<int32_t>(static_cast<size_t>(c) + 1);
+    });
     if (rc != ALQ_OK) return rc;
-    ScratchCursor cur(ctx->scratch);
-    int32_t* tab = cur.take<int32_t>(entries);
-    int32_t* koff = cur.take<int32_t>(static_cast<size_t>(c) + 1);
     rc = alq_class_table_pass(ctx, labels, avail, static_cast<int>(n), c, tab, nullptr, nullptr, st);
     if (rc != ALQ_OK) return rc;
     class_budget_prefix_kernel<<<1, 1024, 0, st>>>(k, c, koff);

@@ -141,8 +141,6 @@ cudaError_t alq_gridsync_launch(alq_ctx* ctx, cudaStream_t st, Launch&& launch) 
     return e;
 }
 
-// Device scratch: returns a 256-byte aligned pointer into the arena, growing it if needed.
-int alq_scratch_reserve(alq_ctx* ctx, size_t bytes);
 // The start-of-call handshake of a collective call over the group's windows (alq_comm.cu): once this rank has cleared
 // its window for the call (earlier on `st`), store `tag` into ready[rank] of every rank's window, the u64
 // ready[ALQ_MAX_WORLD] at its head.  Peers write into this window only after they have seen it.
@@ -154,8 +152,15 @@ int alq_class_table_pass(alq_ctx* ctx, const int32_t* labels, const uint8_t* ava
                          unsigned int* bad, int32_t* counts, cudaStream_t st);
 size_t alq_class_table_entries(int64_t n, int c);
 int alq_pinned_reserve(alq_ctx* ctx, size_t bytes);
-int alq_arena2_reserve(alq_ctx* ctx, size_t bytes);
 
+// Device arenas, grow-only: each holds at least `bytes` afterwards.  Called through alq_scratch_carve alone.
+int alq_scratch_reserve(alq_ctx* ctx, size_t bytes);
+int alq_arena2_reserve(alq_ctx* ctx, size_t bytes);
+// The bytes alq_scratch_reserve allocates when a call needs `bytes` and the arena has to grow.
+size_t alq_scratch_alloc_bytes(size_t bytes);
+
+// Hands out an arena's buffers in order, each on a 256-byte boundary.  With a null base it only measures: take()
+// advances the offset alone and returns nullptr.
 struct ScratchCursor {
     char* base;
     size_t off = 0;
@@ -163,15 +168,33 @@ struct ScratchCursor {
     template <typename T>
     T* take(size_t count) {
         off = (off + 255) & ~size_t(255);
-        T* p = reinterpret_cast<T*>(base + off);
+        T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
         off += count * sizeof(T);
         return p;
     }
 };
-static inline size_t scratch_need(std::initializer_list<size_t> sizes) {
-    size_t t = 0;
-    for (size_t s : sizes) t = ((t + 255) & ~size_t(255)) + s;
-    return t + 256;
+
+// The bytes that `layout(ScratchCursor&)`, a call's takes, spans.
+template <typename Layout>
+size_t alq_layout_bytes(Layout&& layout) {
+    ScratchCursor m(nullptr);
+    layout(m);
+    return m.off;
+}
+
+// One call's device scratch, sized and carved by the same takes: runs `layout` once measuring, reserves exactly what it
+// spans and runs it again on the arena, where its takes store the call's pointers.  A reservation may move the arena, so
+// pointers from an earlier carve die with it.  ctx->scratch serves every entry point; an entry point that holds
+// ctx->scratch buffers calls no other entry point that takes scratch.  ctx->arena2 is for the two that must hold buffers
+// across such calls: alq_uncertainty_query_host and BASE's select (alq_mase.cu).
+template <typename Layout>
+int alq_scratch_carve(alq_ctx* ctx, Layout&& layout, bool arena2 = false) {
+    const size_t bytes = alq_layout_bytes(layout);
+    const int rc = arena2 ? alq_arena2_reserve(ctx, bytes) : alq_scratch_reserve(ctx, bytes);
+    if (rc != ALQ_OK) return rc;
+    ScratchCursor cur(arena2 ? ctx->arena2 : ctx->scratch);
+    layout(cur);
+    return ALQ_OK;
 }
 
 // ---------------------------------------------------------------------------------------------

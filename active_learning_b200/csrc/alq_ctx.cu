@@ -110,6 +110,8 @@ extern "C" int alq_set_option(alq_ctx* ctx, const char* key, int64_t value) {
 
 extern "C" int64_t alq_launch_count(const alq_ctx* ctx) { return ctx ? ctx->launches : 0; }
 
+size_t alq_scratch_alloc_bytes(size_t bytes) { return bytes + (bytes >> 2) + (1u << 20); }
+
 int alq_scratch_reserve(alq_ctx* ctx, size_t bytes) {
     if (bytes <= ctx->scratch_bytes) return ALQ_OK;
     // grow-only; callers never hold scratch pointers across API calls
@@ -117,7 +119,7 @@ int alq_scratch_reserve(alq_ctx* ctx, size_t bytes) {
     if (ctx->scratch) cudaFree(ctx->scratch);
     ctx->scratch = nullptr;
     ctx->scratch_bytes = 0;
-    size_t want = bytes + (bytes >> 2) + (1u << 20);
+    const size_t want = alq_scratch_alloc_bytes(bytes);
     if (cudaMalloc(&ctx->scratch, want) != cudaSuccess) {
         cudaGetLastError();
         ALQ_FAIL(ctx, ALQ_ERR_NOMEM, "scratch allocation of %zu bytes failed", want);

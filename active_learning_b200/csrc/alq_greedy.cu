@@ -746,33 +746,32 @@ extern "C" int alq_greedy_select(alq_ctx* ctx, const alq_greedy_desc* D, void* s
 
     // ---- scratch --------------------------------------------------------------------------------------
     const size_t n_best = sample ? 0 : static_cast<size_t>(bmax) * P;
-    const size_t need = scratch_need({segs.size() * sizeof(BlockSeg), P * sizeof(int) * 5, n_best * 8,
-                                      static_cast<size_t>(total_picks) * sizeof(double),
-                                      sched.size() * sizeof(PartSched), leaf_off_all.size() * 4 + 4,
-                                      level_off_all.size() * 4 + 4, comb_all.size() * 4 + 4,
-                                      static_cast<size_t>(cfull_total) * 4 + 16, static_cast<size_t>(cfull_total) * 4 + 16,
-                                      leaf_off_all.size() * 4 + 4,
-                                      static_cast<size_t>(P) * kCL * 8, 64});
-    int rc = alq_scratch_reserve(ctx, need);
+    BlockSeg* d_segs;
+    PartSched* d_sched;
+    int *d_budget, *d_pick_off, *d_first, *d_cur, *d_cfull_off, *d_leaf_off, *d_level_off, *d_comb, *d_posinv, *d_status;
+    unsigned long long* d_best;
+    double *d_unif, *d_cta_part;
+    float *d_cfull, *d_leafval;
+    int rc = alq_scratch_carve(ctx, [&](ScratchCursor& cur) {
+        d_segs = cur.take<BlockSeg>(segs.size());
+        d_budget = cur.take<int>(P);
+        d_pick_off = cur.take<int>(P);
+        d_first = cur.take<int>(P);
+        d_cur = cur.take<int>(P);
+        d_cfull_off = cur.take<int>(P);
+        d_best = cur.take<unsigned long long>(n_best);
+        d_unif = cur.take<double>(total_picks);
+        d_sched = cur.take<PartSched>(sched.size());
+        d_leaf_off = cur.take<int>(leaf_off_all.size() + 1);
+        d_level_off = cur.take<int>(level_off_all.size() + 1);
+        d_comb = cur.take<int>(comb_all.size() + 1);
+        d_cfull = cur.take<float>(cfull_total + 4);
+        d_posinv = cur.take<int>(cfull_total + 4);
+        d_leafval = cur.take<float>(leaf_off_all.size() + 1);
+        d_cta_part = cur.take<double>(static_cast<size_t>(P) * kCL);
+        d_status = cur.take<int>(1);
+    });
     if (rc) return rc;
-    ScratchCursor cur(ctx->scratch);
-    BlockSeg* d_segs = cur.take<BlockSeg>(segs.size());
-    int* d_budget = cur.take<int>(P);
-    int* d_pick_off = cur.take<int>(P);
-    int* d_first = cur.take<int>(P);
-    int* d_cur = cur.take<int>(P);
-    int* d_cfull_off = cur.take<int>(P);
-    unsigned long long* d_best = cur.take<unsigned long long>(n_best);
-    double* d_unif = cur.take<double>(total_picks);
-    PartSched* d_sched = cur.take<PartSched>(sched.size());
-    int* d_leaf_off = cur.take<int>(leaf_off_all.size() + 1);
-    int* d_level_off = cur.take<int>(level_off_all.size() + 1);
-    int* d_comb = cur.take<int>(comb_all.size() + 1);
-    float* d_cfull = cur.take<float>(cfull_total + 4);
-    int* d_posinv = cur.take<int>(cfull_total + 4);
-    float* d_leafval = cur.take<float>(leaf_off_all.size() + 1);
-    double* d_cta_part = cur.take<double>(static_cast<size_t>(P) * kCL);
-    int* d_status = cur.take<int>(1);
 
     // pageable sources: the runtime stages them before returning, so the vectors may die afterwards
     ALQ_CUDA(ctx, cudaMemcpyAsync(d_segs, segs.data(), segs.size() * sizeof(BlockSeg), cudaMemcpyHostToDevice, st));

@@ -1027,29 +1027,31 @@ int alq_greedy_persist(alq_ctx* ctx, const alq_greedy_desc* D, void* stream) {
 
     // ---- scratch ----------------------------------------------------------------------------------------------
     const int total_picks = pick_off[P];
-    const size_t need = scratch_need({segs.size() * sizeof(BlockSeg), groups.size() * sizeof(PGroup),
-                                      leaf_off_all.size() * 4 + 4, level_off_all.size() * 4 + 4, sched_all.size() * 4 + 4,
-                                      static_cast<size_t>(cfull_total) * 8 + 16, static_cast<size_t>(cfull_total) * 4 + 16,
-                                      static_cast<size_t>(total_picks) * 8 + 8, segtab.size() * 4 + 4, ncta_tab.size() * 4 + 4,
-                                      static_cast<size_t>(P + 1) * 4, static_cast<size_t>(P) * 4, 64, 64, comm ? 0 : win_bytes});
-    int rc = alq_scratch_reserve(ctx, need);
+    BlockSeg* d_segs;
+    PGroup* d_groups;
+    int *d_leaf_off, *d_level_off, *d_posinv, *d_segtab, *d_ncta, *d_part_off, *d_cfull_off, *d_status;
+    unsigned int* d_sched;
+    unsigned long long *d_valw, *d_prof;
+    double* d_unif;
+    char* d_win = Gc.window;
+    int rc = alq_scratch_carve(ctx, [&](ScratchCursor& cur) {
+        d_segs = cur.take<BlockSeg>(segs.size());
+        d_groups = cur.take<PGroup>(groups.size());
+        d_leaf_off = cur.take<int>(leaf_off_all.size() + 1);
+        d_level_off = cur.take<int>(level_off_all.size() + 1);
+        d_sched = cur.take<unsigned int>(sched_all.size() + 1);
+        d_valw = cur.take<unsigned long long>(cfull_total + 2);
+        d_posinv = cur.take<int>(cfull_total + 4);
+        d_unif = cur.take<double>(total_picks + 1);
+        d_segtab = cur.take<int>(segtab.size() + 1);
+        d_ncta = cur.take<int>(ncta_tab.size() + 1);
+        d_part_off = cur.take<int>(P + 1);
+        d_cfull_off = cur.take<int>(P);
+        d_status = cur.take<int>(1);
+        d_prof = cur.take<unsigned long long>(8);
+        if (!comm) d_win = cur.take<char>(win_bytes);
+    });
     if (rc) return rc;
-    ScratchCursor cur(ctx->scratch);
-    BlockSeg* d_segs = cur.take<BlockSeg>(segs.size());
-    PGroup* d_groups = cur.take<PGroup>(groups.size());
-    int* d_leaf_off = cur.take<int>(leaf_off_all.size() + 1);
-    int* d_level_off = cur.take<int>(level_off_all.size() + 1);
-    unsigned int* d_sched = cur.take<unsigned int>(sched_all.size() + 1);
-    unsigned long long* d_valw = cur.take<unsigned long long>(cfull_total + 2);
-    int* d_posinv = cur.take<int>(cfull_total + 4);
-    double* d_unif = cur.take<double>(total_picks + 1);
-    int* d_segtab = cur.take<int>(segtab.size() + 1);
-    int* d_ncta = cur.take<int>(ncta_tab.size() + 1);
-    int* d_part_off = cur.take<int>(P + 1);
-    int* d_cfull_off = cur.take<int>(P);
-    int* d_status = cur.take<int>(1);
-    unsigned long long* d_prof = cur.take<unsigned long long>(8);
-    char* d_win = comm ? Gc.window : cur.take<char>(win_bytes);
 
     ALQ_CUDA(ctx, cudaMemcpyAsync(d_segs, segs.data(), segs.size() * sizeof(BlockSeg), cudaMemcpyHostToDevice, st));
     ALQ_CUDA(ctx, cudaMemcpyAsync(d_groups, groups.data(), groups.size() * sizeof(PGroup), cudaMemcpyHostToDevice, st));

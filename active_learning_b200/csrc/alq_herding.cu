@@ -225,20 +225,22 @@ extern "C" int alq_herding_select(alq_ctx* ctx, const float* k, int64_t n, int64
     const int n_col = (ni + COL_THREADS - 1) / COL_THREADS;
     const int n_seg = (ni + SEG - 1) / SEG;
     const int n_part = std::min(ctx->sm_count, (ni + ARG_THREADS - 1) / ARG_THREADS);
-    int rc = alq_scratch_reserve(ctx, scratch_need({static_cast<size_t>(n) * 8, static_cast<size_t>(n),
-                                                    static_cast<size_t>(n_seg) * SEG * sizeof(Entry),
-                                                    static_cast<size_t>(n_seg) * 4, static_cast<size_t>(n_part) * 8,
-                                                    static_cast<size_t>(n_part) * 4, 8, 4}));
+    double *gain, *part_g;
+    uint8_t* cand;
+    Entry* seg;
+    int *seg_cnt, *part_p, *n_avail;
+    unsigned long long* s_total;
+    int rc = alq_scratch_carve(ctx, [&](ScratchCursor& cur) {
+        gain = cur.take<double>(n);
+        cand = cur.take<uint8_t>(n);
+        seg = cur.take<Entry>(static_cast<size_t>(n_seg) * SEG);
+        seg_cnt = cur.take<int>(n_seg);
+        part_g = cur.take<double>(n_part);
+        part_p = cur.take<int>(n_part);
+        s_total = cur.take<unsigned long long>(1);
+        n_avail = cur.take<int>(1);
+    });
     if (rc) return rc;
-    ScratchCursor cur(ctx->scratch);
-    double* gain = cur.take<double>(n);
-    uint8_t* cand = cur.take<uint8_t>(n);
-    Entry* seg = cur.take<Entry>(static_cast<size_t>(n_seg) * SEG);
-    int* seg_cnt = cur.take<int>(n_seg);
-    double* part_g = cur.take<double>(n_part);
-    int* part_p = cur.take<int>(n_part);
-    unsigned long long* s_total = cur.take<unsigned long long>(1);
-    int* n_avail = cur.take<int>(1);
 
     ALQ_CUDA(ctx, cudaSetDevice(ctx->device));
     ALQ_CUDA(ctx, cudaMemcpyAsync(cand, avail, static_cast<size_t>(n), cudaMemcpyDeviceToDevice, st));

@@ -508,17 +508,20 @@ extern "C" int alq_base_select(alq_ctx* ctx, const float* min_margin, const floa
     const int chunk = parallel ? static_cast<int>(std::min<size_t>(256, (ctx->smem_optin - 1024 - bitset_bytes) / per_class_smem)) : 0;
     const size_t resolve_smem = chunk * per_class_smem + bitset_bytes;
     // private arena: alq_select_smallest re-carves the shared scratch on every call
-    int rc = alq_arena2_reserve(ctx, scratch_need({static_cast<size_t>(n) * sizeof(float), static_cast<size_t>(n), sizeof(unsigned int),
-                                                   static_cast<size_t>(c) * kBaseList * sizeof(unsigned long long),
-                                                   static_cast<size_t>(c) * sizeof(int), sizeof(int)}));
+    float* keys;
+    unsigned char* taken;
+    unsigned int* dup;
+    unsigned long long* cand;
+    int *fail, *status;
+    int rc = alq_scratch_carve(ctx, [&](ScratchCursor& cur) {
+        keys = cur.take<float>(n);
+        taken = cur.take<unsigned char>(n);
+        dup = cur.take<unsigned int>(1);
+        cand = cur.take<unsigned long long>(static_cast<size_t>(c) * kBaseList);
+        fail = cur.take<int>(c);
+        status = cur.take<int>(1);
+    }, /*arena2=*/true);
     if (rc) return rc;
-    ScratchCursor cur(ctx->arena2);
-    float* keys = cur.take<float>(n);
-    unsigned char* taken = cur.take<unsigned char>(n);
-    unsigned int* dup = cur.take<unsigned int>(1);
-    unsigned long long* cand = cur.take<unsigned long long>(static_cast<size_t>(c) * kBaseList);
-    int* fail = cur.take<int>(c);
-    int* status = cur.take<int>(1);
     ALQ_CUDA(ctx, cudaMemsetAsync(taken, 0, static_cast<size_t>(n), st));
     ALQ_CUDA(ctx, cudaMemsetAsync(dup, 0, sizeof(unsigned int), st));
     int kgrid = static_cast<int>((n + 255) / 256);

@@ -180,19 +180,19 @@ int alq_min_dist_tc(alq_ctx* ctx, const float* x, int64_t ldx, const float* xn, 
     live = std::max(1, std::min(live, grid));
     const int rounds = (m_blocks + live - 1) / live;
     const int items_per_cta = rounds + 1;
-    int rc = alq_scratch_reserve(ctx, scratch_need({xe * 4, xe * 4, ye * 4, ye * 4, xae * 4, xae * 4, yae * 4, yae * 4,
-                                                    static_cast<size_t>(n) * 4, static_cast<size_t>(m) * 4,
-                                                    static_cast<size_t>(grid) * items_per_cta * sizeof(WorkItem),
-                                                    static_cast<size_t>(grid) * 4}));
+    float *xh, *xl, *yh, *yl, *xah, *xal, *yah, *yal, *xnn, *ynn;
+    WorkItem* d_items;
+    int* d_counts;
+    int rc = alq_scratch_carve(ctx, [&](ScratchCursor& cur) {
+        xh = cur.take<float>(xe); xl = cur.take<float>(xe);
+        yh = cur.take<float>(ye); yl = cur.take<float>(ye);
+        xah = cur.take<float>(xae); xal = cur.take<float>(xae);
+        yah = cur.take<float>(yae); yal = cur.take<float>(yae);
+        xnn = cur.take<float>(n); ynn = cur.take<float>(m);
+        d_items = cur.take<WorkItem>(static_cast<size_t>(grid) * items_per_cta);
+        d_counts = cur.take<int>(grid);
+    });
     if (rc) return rc;
-    ScratchCursor cur(ctx->scratch);
-    float* xh = cur.take<float>(xe); float* xl = cur.take<float>(xe);
-    float* yh = cur.take<float>(ye); float* yl = cur.take<float>(ye);
-    float* xah = cur.take<float>(xae); float* xal = cur.take<float>(xae);
-    float* yah = cur.take<float>(yae); float* yal = cur.take<float>(yae);
-    float* xnn = cur.take<float>(n); float* ynn = cur.take<float>(m);
-    WorkItem* d_items = cur.take<WorkItem>(static_cast<size_t>(grid) * items_per_cta);
-    int* d_counts = cur.take<int>(grid);
 
     // ---- work list (see above): round r covers row blocks [r*live, r*live + mbs); CTA c takes part c % split of
     //      the column tiles of row block c / split

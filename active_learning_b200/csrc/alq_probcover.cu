@@ -339,13 +339,16 @@ extern "C" int alq_probcover_graph(alq_ctx* ctx, const float* x, int64_t n, int3
     const int ni = static_cast<int>(n);
     const int nt = (ni + BM - 1) / BM;
     const size_t e = static_cast<size_t>(n) * d;
-    int rc = alq_scratch_reserve(ctx, scratch_need({e * 4, e * 4, static_cast<size_t>(n) * 8, 8}));
+    float *hi, *lo;
+    double* nrm2;
+    unsigned long long* rech;
+    int rc = alq_scratch_carve(ctx, [&](ScratchCursor& cur) {
+        hi = cur.take<float>(e);
+        lo = cur.take<float>(e);
+        nrm2 = cur.take<double>(n);
+        rech = cur.take<unsigned long long>(1);
+    });
     if (rc) return rc;
-    ScratchCursor cur(ctx->scratch);
-    float* hi = cur.take<float>(e);
-    float* lo = cur.take<float>(e);
-    double* nrm2 = cur.take<double>(n);
-    unsigned long long* rech = cur.take<unsigned long long>(1);
 
     rs::normalize_split_kernel<<<(ni + NORM_WARPS - 1) / NORM_WARPS, NORM_WARPS * 32, 0, st>>>(x, ni, d, ldx, xhat, hi, lo, nrm2, fill ? 0 : 1);
     ALQ_LAUNCH_CHECK(ctx);
@@ -403,25 +406,25 @@ extern "C" int alq_probcover_select(alq_ctx* ctx, const int64_t* row_ptr, const 
     if ((ni + grid - 1) / grid > kSegRowsMax)
         ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_probcover_select: n=%d rows over %d CTAs exceed %d rows per CTA segment", ni, grid,
                  kSegRowsMax);
-    int rc = alq_scratch_reserve(ctx, scratch_need({static_cast<size_t>(n) * 4, static_cast<size_t>(n),
-                                                    static_cast<size_t>(4) * grid * 8, 16}));
+    SelArgs A{};
+    char* words;
+    int* small;                                                      // [0] status, [1] steps
+    int rc = alq_scratch_carve(ctx, [&](ScratchCursor& cur) {
+        A.deg = cur.take<int>(n);
+        A.covered = cur.take<uint8_t>(n);
+        words = cur.take<char>(static_cast<size_t>(4) * grid * 8);
+        small = cur.take<int>(4);
+    });
     if (rc) return rc;
-    ScratchCursor cur(ctx->scratch);
-    int* deg = cur.take<int>(n);
-    uint8_t* covered = cur.take<uint8_t>(n);
-    char* words = cur.take<char>(static_cast<size_t>(4) * grid * 8);
-    int* small = cur.take<int>(4);                                   // [0] status, [1] steps
-    ALQ_CUDA(ctx, cudaMemsetAsync(covered, 0, static_cast<size_t>(n), st));
+    ALQ_CUDA(ctx, cudaMemsetAsync(A.covered, 0, static_cast<size_t>(n), st));
     ALQ_CUDA(ctx, cudaMemsetAsync(words, 0, static_cast<size_t>(4) * grid * 8, st));
     ALQ_CUDA(ctx, cudaMemsetAsync(small, 0, 4 * sizeof(int), st));
     const long long* rp = reinterpret_cast<const long long*>(row_ptr);
-    pc_cover_kernel<<<(ni + 7) / 8, 256, 0, st>>>(rp, cols, ni, labeled, covered);
+    pc_cover_kernel<<<(ni + 7) / 8, 256, 0, st>>>(rp, cols, ni, labeled, A.covered);
     ALQ_LAUNCH_CHECK(ctx);
-    pc_deg_kernel<<<(ni + 7) / 8, 256, 0, st>>>(rp, cols, ni, covered, deg);
+    pc_deg_kernel<<<(ni + 7) / 8, 256, 0, st>>>(rp, cols, ni, A.covered, A.deg);
     ALQ_LAUNCH_CHECK(ctx);
-    SelArgs A{};
     A.row_ptr = rp; A.cols = cols; A.n = ni; A.budget = static_cast<int>(budget);
-    A.deg = deg; A.covered = covered;
     A.S.world = 1; A.S.rank = 0; A.S.grid = grid;
     A.S.off[0] = 0; A.S.off[1] = ni;
     A.W.peer[0] = words;

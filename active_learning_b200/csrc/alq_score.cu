@@ -1289,8 +1289,6 @@ static int uncertainty_tail_impl(alq_ctx* ctx, const float* logits, int64_t n, i
         if (rc) return rc;
         if (!sharded) return alq_select_smallest(ctx, scores, n, b, out_pos, stream);
         const int64_t k = std::min<int64_t>(b, n);
-        rc = alq_scratch_reserve(ctx, scratch_need({static_cast<size_t>(n) * 8 + 16, static_cast<size_t>(k + 1) * 4}));   // the selects below reuse the front
-        if (rc) return rc;
         int32_t* pos_loc = nullptr;
         if (cudaMallocAsync(reinterpret_cast<void**>(&pos_loc), static_cast<size_t>(k + 1) * 4, st) != cudaSuccess) {
             cudaGetLastError();
@@ -1305,9 +1303,13 @@ static int uncertainty_tail_impl(alq_ctx* ctx, const float* logits, int64_t n, i
         if (int rc0 = alq_comm_check(ctx)) return rc0;       // a previous asynchronous exchange that timed out
     constexpr int kBucketCap = 48;          // per sub-list: a bucket holds up to 16 x 48 words (about b / grid = 68 expected)
     static_assert(132 * kBucketLanes <= 2 * 2048, "bucket counters live in the slot's cross-rank words");
-    int rc = alq_scratch_reserve(ctx, scratch_need({static_cast<size_t>(n) * 8 + 16, static_cast<size_t>(ctx->sm_count) * kBucketLanes * kBucketCap * 8}));
-    if (rc) return rc;
+    const bool buckets = !sharded && ctx->tail_buckets && ctx->sm_count * kBucketLanes <= 2 * 2048;
     SelArgs sel{};
+    int rc = alq_scratch_carve(ctx, [&](ScratchCursor& cur) {
+        sel.g_cand = cur.take<unsigned long long>(n + 2);
+        if (buckets) sel.g_bucket = cur.take<unsigned long long>(static_cast<size_t>(ctx->sm_count) * kBucketLanes * kBucketCap);
+    });
+    if (rc) return rc;
     sel.b = static_cast<int>(b);
     sel.list_cap = kListCap;
     {   // the pipe plan put `reserve` bytes behind the ring: the list starts there, but never below 128 KB + scratch
@@ -1323,15 +1325,10 @@ static int uncertainty_tail_impl(alq_ctx* ctx, const float* logits, int64_t n, i
     sel.g_ctr = slot + 4 * 2048;
     sel.g_tot = slot + 2 * 2048;
     ctx->sel_last_ctr = sel.g_ctr;
-    {
-        ScratchCursor cur(ctx->scratch);
-        sel.g_cand = cur.take<unsigned long long>(n + 2);
-        if (sharded) sel.bucket_cap = ctx->tail_buckets ? kBucketCap : 0;      // sharded: the route needs no global lists, only the switch
-        if (!sharded && ctx->tail_buckets && ctx->sm_count * kBucketLanes <= 2 * 2048) {
-            sel.bucket_cap = kBucketCap;
-            sel.g_bucket = cur.take<unsigned long long>(static_cast<size_t>(ctx->sm_count) * kBucketLanes * kBucketCap);
-            sel.g_bcnt = sel.g_tot;          // the cross-rank sums are not used on one GPU: zeroed words of the slot
-        }
+    if (sharded) sel.bucket_cap = ctx->tail_buckets ? kBucketCap : 0;      // sharded: the route needs no global lists, only the switch
+    if (buckets) {
+        sel.bucket_cap = kBucketCap;
+        sel.g_bcnt = sel.g_tot;              // the cross-rank sums are not used on one GPU: zeroed words of the slot
     }
     sel.out_pos = out_pos;
     sel.ring_off = cfg.stages * cfg.tile_floats * 4;        // behind the stages' tiles

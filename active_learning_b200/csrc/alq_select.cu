@@ -372,16 +372,16 @@ extern "C" int alq_select_smallest(alq_ctx* ctx, const float* scores, int64_t n,
     }
     const int nblocks = static_cast<int>((n + kSelChunk - 1) / kSelChunk);
     const int64_t npad = next_pow2(b < 2 ? 2 : b);
-    const size_t need = scratch_need({sizeof(SelState), kBins * sizeof(uint32_t),
-                                      static_cast<size_t>(nblocks) * sizeof(uint32_t),
-                                      static_cast<size_t>(npad) * sizeof(unsigned long long)});
-    int rc = alq_scratch_reserve(ctx, need);
+    SelState* state;
+    uint32_t *hist, *eq_count;
+    unsigned long long* keys;
+    int rc = alq_scratch_carve(ctx, [&](ScratchCursor& cur) {
+        state = cur.take<SelState>(1);
+        hist = cur.take<uint32_t>(kBins);
+        eq_count = cur.take<uint32_t>(nblocks);
+        keys = cur.take<unsigned long long>(npad);
+    });
     if (rc) return rc;
-    ScratchCursor cur(ctx->scratch);
-    SelState* state = cur.take<SelState>(1);
-    uint32_t* hist = cur.take<uint32_t>(kBins);
-    uint32_t* eq_count = cur.take<uint32_t>(nblocks);
-    unsigned long long* keys = cur.take<unsigned long long>(npad);
 
     SelState init{};
     init.k = static_cast<unsigned long long>(b);
@@ -473,9 +473,9 @@ extern "C" int alq_topb_merge(alq_ctx* ctx, const uint64_t* keys, int64_t n, int
         ALQ_LAUNCH_CHECK(ctx);
         return ALQ_OK;
     }
-    int rc = alq_scratch_reserve(ctx, scratch_need({static_cast<size_t>(n) * 8}));
+    unsigned long long* work;
+    int rc = alq_scratch_carve(ctx, [&](ScratchCursor& cur) { work = cur.take<unsigned long long>(n); });
     if (rc) return rc;
-    unsigned long long* work = ScratchCursor(ctx->scratch).take<unsigned long long>(n);
     ALQ_CUDA(ctx, cudaMemcpyAsync(work, keys, static_cast<size_t>(n) * 8, cudaMemcpyDeviceToDevice, st));
     const int runs = static_cast<int>((n + kRun - 1) / kRun);
     sort_runs_kernel<<<runs, kRun / 2, 0, st>>>(work, n);
@@ -578,10 +578,9 @@ extern "C" int alq_topb_exchange(alq_ctx* ctx, const float* scores, const int32_
     // a previous (asynchronous) exchange that timed out is reported here, before its garbage can be built upon
     if (int rc0 = alq_comm_check(ctx)) return rc0;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    int rc = alq_scratch_reserve(ctx, scratch_need({8}));
+    unsigned int* ticket;
+    int rc = alq_scratch_carve(ctx, [&](ScratchCursor& cur) { ticket = cur.take<unsigned int>(1); });
     if (rc) return rc;
-    ScratchCursor cur(ctx->scratch);
-    unsigned int* ticket = cur.take<unsigned int>(1);
     int* status = ctx->xchg_status_dev;
     ALQ_CUDA(ctx, cudaMemsetAsync(ticket, 0, 4, st));
     G.epoch += 1;
@@ -632,14 +631,15 @@ extern "C" int alq_uncertainty_query_host(alq_ctx* ctx, const float* logits_host
     // private arena (not the shared scratch: alq_select_smallest re-carves that one)
     const int64_t chunk_rows = std::max<int64_t>(1, (32ll << 20) / (static_cast<int64_t>(c) * 4));
     const size_t chunk_elems = static_cast<size_t>(chunk_rows) * c;
-    int rc = alq_arena2_reserve(ctx, scratch_need({chunk_elems * sizeof(float), chunk_elems * sizeof(float),
-                                                   static_cast<size_t>(n) * sizeof(float),
-                                                   static_cast<size_t>(b) * sizeof(int32_t)}));
+    float *buf[2], *scores;
+    int32_t* pos;
+    int rc = alq_scratch_carve(ctx, [&](ScratchCursor& cur) {
+        buf[0] = cur.take<float>(chunk_elems);
+        buf[1] = cur.take<float>(chunk_elems);
+        scores = cur.take<float>(n);
+        pos = cur.take<int32_t>(b);
+    }, /*arena2=*/true);
     if (rc) return rc;
-    ScratchCursor cur(ctx->arena2);
-    float* buf[2] = {cur.take<float>(chunk_elems), cur.take<float>(chunk_elems)};
-    float* scores = cur.take<float>(n);
-    int32_t* pos = cur.take<int32_t>(b);
     auto cleanup = [&]() {};
     cudaStream_t ss[2] = {ctx->side_stream, ctx->side_stream2};
     int which = 0;

@@ -224,16 +224,14 @@ int alq_select_smallest_cluster(alq_ctx* ctx, const float* scores, int64_t n, in
                                 cudaStream_t st) {
     using namespace selc;
     if (n > static_cast<int64_t>(CL) * MAX_SLICE || b > MAX_B || n < 1 || b < 1) return ALQ_ERR_STATE;
-    const size_t hist_bytes = static_cast<size_t>(3) * CL * BINS * sizeof(uint32_t);
-    int rc = alq_scratch_reserve(ctx, scratch_need({hist_bytes, CL * 2 * sizeof(uint32_t), MAX_B * sizeof(unsigned long long),
-                                                    (MAX_B + 2) * sizeof(unsigned long long)}));
-    if (rc) return rc;
-    ScratchCursor cur(ctx->scratch);
     Scratch S;
-    S.hist_part = cur.take<uint32_t>(3 * CL * BINS);
-    S.counts = cur.take<uint32_t>(CL * 2);
-    S.words = cur.take<unsigned long long>(MAX_B);
-    S.sorted = cur.take<unsigned long long>(MAX_B + 2);
+    int rc = alq_scratch_carve(ctx, [&](ScratchCursor& cur) {
+        S.hist_part = cur.take<uint32_t>(3 * CL * BINS);
+        S.counts = cur.take<uint32_t>(CL * 2);
+        S.words = cur.take<unsigned long long>(MAX_B);
+        S.sorted = cur.take<unsigned long long>(MAX_B + 2);
+    });
+    if (rc) return rc;
     const int per = ((static_cast<int>(n) + CL - 1) / CL + 3) & ~3;
     size_t smem = std::max<size_t>(std::max<size_t>(static_cast<size_t>(per) * 4, static_cast<size_t>(b + 2) * 8), 2048 * 8) + 64;
     if (smem > ctx->smem_optin - 24 * 1024) return ALQ_ERR_STATE;

@@ -459,16 +459,19 @@ extern "C" int alq_kmeans_assign(alq_ctx* ctx, const float* xhat, const float* h
     const cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int ni = static_cast<int>(n);
     const size_t ce = static_cast<size_t>(k) * d;
-    int rc = alq_scratch_reserve(ctx, scratch_need({ce * 4, ce * 4, ce * 4, static_cast<size_t>(k) * 8,
-                                                    static_cast<size_t>(n) * 4, 12}));
+    float *chi, *clo, *cc;                             // cc: the centres' copy the split reads back
+    double* cn;
+    int* list;
+    unsigned int* cnt;                                 // [0] labels changed, [1] rows listed, [2] norms refused
+    int rc = alq_scratch_carve(ctx, [&](ScratchCursor& cur) {
+        chi = cur.take<float>(ce);
+        clo = cur.take<float>(ce);
+        cc = cur.take<float>(ce);
+        cn = cur.take<double>(k);
+        list = cur.take<int>(n);
+        cnt = cur.take<unsigned int>(3);
+    });
     if (rc) return rc;
-    ScratchCursor cur(ctx->scratch);
-    float* chi = cur.take<float>(ce);
-    float* clo = cur.take<float>(ce);
-    float* cc = cur.take<float>(ce);                   // the centres' copy the split reads back
-    double* cn = cur.take<double>(k);
-    int* list = cur.take<int>(n);
-    unsigned int* cnt = cur.take<unsigned int>(3);     // [0] labels changed, [1] rows listed, [2] norms refused
     ALQ_CUDA(ctx, cudaMemcpyAsync(cc, centres, ce * 4, cudaMemcpyDeviceToDevice, st));
     ALQ_CUDA(ctx, cudaMemsetAsync(cnt, 0, 12, st));
     rs::normalize_split_kernel<<<(k + rs::NORM_WARPS - 1) / rs::NORM_WARPS, rs::NORM_WARPS * 32, 0, st>>>(
@@ -521,14 +524,14 @@ extern "C" int alq_kmeans_update(alq_ctx* ctx, const float* xhat, int64_t n, int
     const cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int ni = static_cast<int>(n);
     const int chunks = (ni + CHUNK - 1) / CHUNK;
-    int rc = alq_scratch_reserve(ctx, scratch_need({static_cast<size_t>(chunks) * k * 4, static_cast<size_t>(k) * 4,
-                                                    static_cast<size_t>(k) * 4, static_cast<size_t>(n) * 4}));
+    int *hist, *count, *start, *order;
+    int rc = alq_scratch_carve(ctx, [&](ScratchCursor& cur) {
+        hist = cur.take<int>(static_cast<size_t>(chunks) * k);
+        count = cur.take<int>(k);
+        start = cur.take<int>(k);
+        order = cur.take<int>(n);
+    });
     if (rc) return rc;
-    ScratchCursor cur(ctx->scratch);
-    int* hist = cur.take<int>(static_cast<size_t>(chunks) * k);
-    int* count = cur.take<int>(k);
-    int* start = cur.take<int>(k);
-    int* order = cur.take<int>(n);
     const size_t hsm = static_cast<size_t>(k) * 4;
     ALQ_CUDA(ctx, cudaFuncSetAttribute(km_hist_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(hsm)));
     ALQ_CUDA(ctx, cudaFuncSetAttribute(km_place_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(hsm)));
@@ -566,11 +569,12 @@ extern "C" int alq_typicality(alq_ctx* ctx, const float* xhat, int32_t d, const 
     if (!xhat || !rows || !typ || !best) ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_typicality: null pointer");
     if (tiles >= (1LL << 31)) ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_typicality: too many row tiles");
     const cudaStream_t st = static_cast<cudaStream_t>(stream);
-    int rc = alq_scratch_reserve(ctx, scratch_need({static_cast<size_t>(groups + 1) * 4, static_cast<size_t>(groups + 1) * 4}));
+    int *dg, *dt;
+    int rc = alq_scratch_carve(ctx, [&](ScratchCursor& cur) {
+        dg = cur.take<int>(groups + 1);
+        dt = cur.take<int>(groups + 1);
+    });
     if (rc) return rc;
-    ScratchCursor cur(ctx->scratch);
-    int* dg = cur.take<int>(groups + 1);
-    int* dt = cur.take<int>(groups + 1);
     ALQ_CUDA(ctx, cudaMemcpyAsync(dg, goff.data(), goff.size() * 4, cudaMemcpyHostToDevice, st));
     ALQ_CUDA(ctx, cudaMemcpyAsync(dt, toff.data(), toff.size() * 4, cudaMemcpyHostToDevice, st));
     TypArgs A{};
@@ -595,11 +599,13 @@ extern "C" int alq_kmeans_nearest(alq_ctx* ctx, const float* xhat, int64_t n, in
         ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_kmeans_nearest: null pointer or xhat / centres not 16-byte aligned");
     const cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int ni = static_cast<int>(n);
-    int rc = alq_scratch_reserve(ctx, scratch_need({static_cast<size_t>(n) * 8, static_cast<size_t>(k) * 8}));
+    double* d2;
+    unsigned long long* best;
+    int rc = alq_scratch_carve(ctx, [&](ScratchCursor& cur) {
+        d2 = cur.take<double>(n);
+        best = cur.take<unsigned long long>(k);
+    });
     if (rc) return rc;
-    ScratchCursor cur(ctx->scratch);
-    double* d2 = cur.take<double>(n);
-    unsigned long long* best = cur.take<unsigned long long>(k);
     ALQ_CUDA(ctx, cudaMemsetAsync(best, 0xff, static_cast<size_t>(k) * 8, st));
     ALQ_CUDA(ctx, cudaMemsetAsync(nearest, 0xff, static_cast<size_t>(k) * 4, st));
     km_near_d2_kernel<<<(ni + 255) / 256, 256, 0, st>>>(xhat, ni, d, labels, centres, k, d2, best);

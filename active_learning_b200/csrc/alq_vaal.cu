@@ -143,13 +143,14 @@ extern "C" int alq_vaal_scores(alq_ctx* ctx, const float* mu, int64_t n, int32_t
     const int64_t slice = std::min<int64_t>(n, SLICE_ROWS);
     const size_t w1e = static_cast<size_t>(HID) * kp, w2e = static_cast<size_t>(HID) * HID;
     const size_t xe = static_cast<size_t>(slice) * kp, he = static_cast<size_t>(slice) * HID;
-    int rc = alq_scratch_reserve(ctx, scratch_need({w1e * 4, w1e * 4, w2e * 4, w2e * 4, xe * 4, xe * 4, he * 4, he * 4}));
+    float *w1h, *w1l, *w2h, *w2l, *xh, *xl, *hh, *hl;
+    int rc = alq_scratch_carve(ctx, [&](ScratchCursor& cur) {
+        w1h = cur.take<float>(w1e); w1l = cur.take<float>(w1e);
+        w2h = cur.take<float>(w2e); w2l = cur.take<float>(w2e);
+        xh = cur.take<float>(xe); xl = cur.take<float>(xe);
+        hh = cur.take<float>(he); hl = cur.take<float>(he);
+    });
     if (rc) return rc;
-    ScratchCursor cur(ctx->scratch);
-    float* w1h = cur.take<float>(w1e); float* w1l = cur.take<float>(w1e);
-    float* w2h = cur.take<float>(w2e); float* w2l = cur.take<float>(w2e);
-    float* xh = cur.take<float>(xe); float* xl = cur.take<float>(xe);
-    float* hh = cur.take<float>(he); float* hl = cur.take<float>(he);
 
     auto split = [&](const float* src, int64_t rows, int d, int64_t ld, int kpad, float* hi, float* lo) -> int {
         const int blocks = static_cast<int>(std::min<int64_t>((rows * kpad + 255) / 256, static_cast<int64_t>(ctx->sm_count) * 16));

@@ -568,11 +568,13 @@ int nn_chain_run(alq_ctx* ctx, const char* name, double* dist, int64_t n, int64_
     int cs = 0;
     int rc = ward_cluster_size<L>(ctx, smem, &cs);
     if (rc) return rc;
-    rc = alq_scratch_reserve(ctx, scratch_need({static_cast<size_t>(cs) * n * sizeof(int2), sizeof(int)}));
+    int2* chain;
+    int* status;
+    rc = alq_scratch_carve(ctx, [&](ScratchCursor& cur) {
+        chain = cur.take<int2>(static_cast<size_t>(cs) * n);
+        status = cur.take<int>(1);
+    });
     if (rc) return rc;
-    ScratchCursor cur(ctx->scratch);
-    int2* chain = cur.take<int2>(static_cast<size_t>(cs) * n);
-    int* status = cur.take<int>(1);
     ALQ_CUDA(ctx, cudaMemsetAsync(status, 0, sizeof(int), st));
 
     cudaLaunchConfig_t cfg = {};
@@ -637,9 +639,9 @@ extern "C" int alq_herding_kernel(alq_ctx* ctx, const float* x, int64_t n, int32
     const double q = *q_host;
     if (!(std::isfinite(q) && std::fpclassify(q) == FP_NORMAL && q > 0.0))
         ALQ_FAIL(ctx, ALQ_ERR_INVALID, "alq_herding_kernel: q=%g must be a finite positive normal number", q);
-    int rc = alq_scratch_reserve(ctx, scratch_need({sizeof(unsigned int)}));
+    unsigned int* bad;
+    int rc = alq_scratch_carve(ctx, [&](ScratchCursor& cur) { bad = cur.take<unsigned int>(1); });
     if (rc) return rc;
-    unsigned int* bad = ScratchCursor(ctx->scratch).take<unsigned int>(1);
     const cudaStream_t st = static_cast<cudaStream_t>(stream);
     ALQ_CUDA(ctx, cudaSetDevice(ctx->device));
     ALQ_CUDA(ctx, cudaMemsetAsync(bad, 0, sizeof(unsigned int), st));

@@ -6,6 +6,7 @@ tc::band_coef.  The distances they certify are K7's pair arithmetic, written onc
 and the ring is correct only while its producer and consumers walk one k-block sequence, which K9, K15 and K18 take
 from tc::ring_produce_rows and tc::ring_tile."""
 import os
+import re
 
 CSRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "active_learning_b200", "csrc")
 RING_KERNELS = {"alq_mindist_tc.cu": "K3", "alq_vaal.cu": "K9", "alq_probcover.cu": "K13", "alq_typiclust.cu": "K15",
@@ -44,3 +45,16 @@ def test_the_exact_pair_arithmetic_and_the_band_coefficient_are_written_once():
     assert [n for n, s in srcs.items() if "ldexp(1.0, -20)" in s] == ["alq_wgmma.cuh"]
     for name in ("alq_probcover.cu", "alq_typiclust.cu", "alq_cal.cu"):
         assert "tc::band_coef(d)" in srcs[name], name
+
+
+def test_every_scratch_layout_is_written_once():
+    """Each entry point's takes both size and carve its scratch (alq_scratch_carve): no list of sizes beside them, no
+    cursor or reservation outside the helper, and the arena's growth rule in alq_ctx.cu alone."""
+    srcs = _all_sources()
+    assert [n for n, s in srcs.items() if "scratch_" "need" in s] == []      # a size list beside the takes
+    assert [n for n, s in srcs.items() if re.search(r"\bScratchCursor\s*(\w+\s*)?[({]", s)] == ["alq_common.cuh"]
+    for fn in ("alq_scratch_reserve", "alq_arena2_reserve"):
+        calls = {n: len(re.findall(r"\b%s\(" % fn, s)) for n, s in srcs.items()}
+        # alq_common.cuh: the declaration and the helper's call; alq_ctx.cu: the definition
+        assert {n: k for n, k in calls.items() if k} == {"alq_common.cuh": 2, "alq_ctx.cu": 1}, fn
+    assert [n for n, s in srcs.items() if re.search(r"\(\s*\w+\s*>>\s*2\s*\)\s*\+\s*\(\s*1u?\s*<<\s*20\s*\)", s)] == ["alq_ctx.cu"]
