@@ -163,6 +163,13 @@ SIGNATURES = {
                                      C.c_void_p]),
     "alq_herding_select": (C.c_int, [C.c_void_p, c_f32p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, c_i32p,
                                      c_f32p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "alq_bait_fisher": (C.c_int, [C.c_void_p, c_f32p, C.c_int64, C.c_int32, C.c_int64, c_f32p, C.c_int32, C.c_void_p,
+                                  C.c_void_p, C.c_void_p]),
+    "alq_bait_init": (C.c_int, [C.c_void_p, c_f32p, C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                C.c_void_p, C.c_void_p, C.c_void_p]),
+    "alq_bait_select": (C.c_int, [C.c_void_p, c_f32p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_void_p,
+                                  C.c_void_p, C.c_void_p, C.c_void_p, c_i32p, C.c_int64, c_i32p, C.c_int64, C.c_int64,
+                                  c_i32p, C.c_void_p, c_i32p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
 }
 
 

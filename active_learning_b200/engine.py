@@ -927,6 +927,106 @@ class Engine:
         allocator would otherwise keep its 4 n^2 bytes."""
         torch.cuda.empty_cache()
 
+    # -- K24 / K25 / K26: BAIT --------------------------------------------------------------------------------
+    BAIT_MAX_CLASSES = 16      # K26 keeps each row's C x C forms in shared memory and C accumulators in registers
+
+    @classmethod
+    def bait_bytes(cls, n: int, c: int, d: int) -> int:
+        """Device memory a BAIT query over n rows with C classes and D features needs: the dense A, F and scratch at
+        8 dim^2 each (dim = C D), plus the two per-row C x C forms at 8 n C^2 each."""
+        dim = int(c) * int(d)
+        return 3 * 8 * dim * dim + 2 * 8 * int(n) * int(c) * int(c)
+
+    def bait_guard(self, n: int, c: int, d: int):
+        """AlqError naming C, D, the bytes needed and the bytes free when bait_bytes(n, C, D) does not fit the device, or
+        C is outside [2, BAIT_MAX_CLASSES]; before anything is allocated."""
+        c, d = int(c), int(d)
+        _check_fits(self, "bait", n, self.bait_bytes(n, c, d), f"C={c} classes x D={d} features: A, F and scratch at "
+                    f"8 (C D)^2 each, the per-row forms at 8 n C^2 each", "model (C D) or subset_unlabeled")
+        if not 2 <= c <= self.BAIT_MAX_CLASSES:
+            raise AlqError(f"bait: C={c} classes outside [2, {self.BAIT_MAX_CLASSES}] (D={d})")
+
+    def _bait_rows(self, logits: torch.Tensor, emb: torch.Tensor, method: str):
+        zl, h = _f32c(logits, "logits").contiguous(), _f32c(emb, "emb").contiguous()
+        if zl.dim() != 2 or h.dim() != 2 or zl.shape[0] != h.shape[0] or zl.shape[0] == 0:
+            raise AlqError(f"{method}: need logits [n, C] and emb [n, D] with n >= 1, got {tuple(zl.shape)} and "
+                           f"{tuple(h.shape)}")
+        return zl, h
+
+    def bait_fisher(self, logits: torch.Tensor, emb: torch.Tensor):
+        """K24: (p, F): p float64 CUDA [n, C] the fp64 softmax of logits [n, C], F float64 CUDA [C D, C D] the pool's mean
+        Fisher (1/n) sum_x (diag p_x - p_x p_x^T) (x) h_x h_x^T of the raw embeddings emb [n, D] (both float32 CUDA),
+        exactly symmetric.  bait_guard runs first; AlqError (ALQ_ERR_NUMERIC) for a row with a NaN or infinity."""
+        zl, h = self._bait_rows(logits, emb, "bait_fisher")
+        (n, c), d = zl.shape, h.shape[1]
+        self.bait_guard(n, c, d)
+        p = torch.empty((n, c), dtype=torch.float64, device=zl.device)
+        F = torch.empty((c * d, c * d), dtype=torch.float64, device=zl.device)
+        self._check(self.lib.alq_bait_fisher(self._h, _ptr(zl), n, c, c, _ptr(h), d, _ptr(p), _ptr(F), self._stream()),
+                    "alq_bait_fisher")
+        return p, F
+
+    def bait_init(self, emb: torch.Tensor, F: torch.Tensor, lamb: float):
+        """K25: (A, At, Gt) from A = I / lamb: A float64 CUDA [C D, C D], and per row of emb [n, D] the C x C forms
+        At_x = |h_x|^2 / lamb I and Gt_x[a, b] = h_x^T F_ab h_x / lamb^2 (float64 CUDA [n, C, C])."""
+        from .query_strategies.bait import bait_lamb
+        lamb = bait_lamb(lamb)
+        h = _f32c(emb, "emb").contiguous()
+        dim = F.shape[0] if F.dim() == 2 else -1
+        if (h.dim() != 2 or not F.is_cuda or F.dtype != torch.float64 or F.shape != (dim, dim) or not F.is_contiguous()
+                or dim % h.shape[1]):
+            raise AlqError(f"bait_init: need emb [n, D] and a contiguous float64 F [C D, C D], got {tuple(h.shape)} and "
+                           f"{tuple(F.shape)}")
+        n, d = h.shape
+        c = dim // d
+        A = torch.empty_like(F)
+        At = torch.empty((n, c, c), dtype=torch.float64, device=F.device)
+        Gt = torch.empty_like(At)
+        lh = C.c_double(lamb)
+        self._check(self.lib.alq_bait_init(self._h, _ptr(h), n, c, d, _ptr(F), C.byref(lh), _ptr(A), _ptr(At), _ptr(Gt),
+                                           self._stream()), "alq_bait_init")
+        return A, At, Gt
+
+    def bait_select(self, emb: torch.Tensor, p: torch.Tensor, F: torch.Tensor, state, lab_pos, cand_pos, budget: int,
+                    phase_ms: Optional[np.ndarray] = None):
+        """K26: BAIT's picks over the rows of emb [n, D] with bait_fisher's p and F and bait_init's state (A, At, Gt,
+        consumed): the rows lab_pos absorbed in order, then T = min(2 budget, len(cand_pos)) forward picks among cand_pos
+        (ascending positions) and T - budget backward removals (spec: tests/bait_oracle.py).  Returns (picks: host int64
+        array, the remaining list in forward-pick order; the forward picks [T], host int64; the forward scores [T] and
+        backward scores [T - budget] of the chosen rows, float64 host arrays).  phase_ms, a float32 host array of 3, receives the device milliseconds of the
+        absorption, the forward and the backward pass."""
+        A, At, Gt = state
+        if phase_ms is not None and (phase_ms.dtype != np.float32 or phase_ms.size < 3 or not phase_ms.flags.c_contiguous):
+            raise AlqError("bait_select: phase_ms must be a contiguous float32 host array of at least 3 entries")
+        h = _f32c(emb, "emb").contiguous()
+        n, d = h.shape
+        c = p.shape[1] if p.dim() == 2 else -1
+        dim = c * d
+        for name, t, shape in (("p", p, (n, c)), ("F", F, (dim, dim)), ("A", A, (dim, dim)), ("At", At, (n, c, c)),
+                               ("Gt", Gt, (n, c, c))):
+            if not t.is_cuda or t.dtype != torch.float64 or tuple(t.shape) != shape or not t.is_contiguous():
+                raise AlqError(f"bait_select: {name} must be a contiguous float64 CUDA tensor of shape {shape}")
+        lab = torch.as_tensor(np.asarray(lab_pos, dtype=np.int32), device=h.device)
+        cand = np.asarray(cand_pos, dtype=np.int64)
+        if len(cand) and (np.any(np.diff(cand) <= 0) or cand[0] < 0 or cand[-1] >= n):
+            raise AlqError("bait_select: cand_pos must be ascending pool positions")
+        cand_t = torch.as_tensor(cand.astype(np.int32), device=h.device)
+        budget = int(budget)
+        T = min(2 * budget, len(cand))
+        picks = torch.empty(max(budget, 1), dtype=torch.int32, device=h.device)
+        fwd_list = torch.empty(max(T, 1), dtype=torch.int32, device=h.device)
+        fwd = torch.empty(max(T, 1), dtype=torch.float64, device=h.device)
+        bwd = torch.empty(max(T - budget, 1), dtype=torch.float64, device=h.device)
+        k = C.c_int64(0)
+        self._check(self.lib.alq_bait_select(self._h, _ptr(h), _ptr(p), n, c, d, _ptr(F), _ptr(A), _ptr(At), _ptr(Gt),
+                                             _ptr(lab) if len(lab) else None, len(lab),
+                                             _ptr(cand_t) if len(cand) else None, len(cand), budget, _ptr(picks),
+                                             C.byref(k), _ptr(fwd_list), _ptr(fwd), _ptr(bwd),
+                                             None if phase_ms is None else phase_ms.ctypes.data_as(C.c_void_p),
+                                             self._stream()), "alq_bait_select")
+        return (picks[:k.value].cpu().numpy().astype(np.int64), fwd_list[:T].cpu().numpy().astype(np.int64),
+                fwd[:T].cpu().numpy(), bwd[:max(T - budget, 0)].cpu().numpy())
+
     # -- K15 / K16 / K17: TypiClust ----------------------------------------------------------------------
     KMEANS_MAX_ITER = 100
 

@@ -17,6 +17,7 @@ from __future__ import annotations
 from .query_strategies.coreset import (BADGEQuery, CoresetQuery, PartitionedBADGEQuery,
                                        PartitionedCoresetQuery)
 from .query_strategies.alfamix import ALFAMixQuery
+from .query_strategies.bait import BAITQuery
 from .query_strategies.balanced_random import BalancedRandomQuery
 from .query_strategies.cal import CALQuery
 from .query_strategies.balancing import BalancingQuery
@@ -46,6 +47,7 @@ _MIXINS = {
     "CALSampler": CALQuery,
     "ALFAMixSampler": ALFAMixQuery,
     "MaxHerdingSampler": MaxHerdingQuery,
+    "BAITSampler": BAITQuery,
 }
 
 

@@ -228,7 +228,7 @@ class CoresetQuery(EngineMixin):
 
 class PoolQuery(CoresetQuery):
     """The query body of the samplers that pick from CoreSet's pool by a rule of their own (ProbCover, TypiClust, CAL,
-    ALFA-Mix, MaxHerding).
+    ALFA-Mix, MaxHerding, BAIT).
 
     The pool is CoreSet's (`get_idxs_for_coreset`: the same two shuffles, subset_labeled / subset_unlabeled honoured) and
     the budget is clamped to its available rows; a budget <= 0 returns ([], 0) before anything else runs.  A subclass's

@@ -2,9 +2,10 @@
 `get_strategy(name)` returns the class called `name`.  Every class name the reference dispatches is implemented: the
 thirteen accelerated samplers (the seven of the north-star path plus MASE / BASE / Balancing, SURVEY.md section 8f,
 MarginClustering, VAAL and BalancedRandom) and the default RandomSampler.  ProbCoverSampler, TypiClustSampler,
-CALSampler, ALFAMixSampler and MaxHerdingSampler are this project's additions (no reference counterpart; ProbCoverSampler
-needs the sampler kwarg `delta`, MaxHerdingSampler the sampler kwarg `sigma`)."""
+CALSampler, ALFAMixSampler, MaxHerdingSampler and BAITSampler are this project's additions (no reference counterpart;
+ProbCoverSampler needs the sampler kwarg `delta`, MaxHerdingSampler the sampler kwarg `sigma`)."""
 from .alfamix_sampler import ALFAMixSampler  # noqa: F401
+from .bait_sampler import BAITSampler  # noqa: F401
 from .badge_sampler import BADGESampler  # noqa: F401
 from .balanced_random_sampler import BalancedRandomSampler  # noqa: F401
 from .balancing_sampler import BalancingSampler  # noqa: F401
@@ -28,7 +29,7 @@ ACCELERATED = ("MarginSampler", "ConfidenceSampler", "EntropySampler", "CoresetS
                "PartitionedCoresetSampler", "BADGESampler", "PartitionedBADGESampler", "MASESampler", "BASESampler",
                "BalancingSampler", "MarginClusteringSampler", "VAALSampler", "BalancedRandomSampler",
                "ProbCoverSampler", "TypiClustSampler", "CALSampler", "ALFAMixSampler",
-               "MaxHerdingSampler")
+               "MaxHerdingSampler", "BAITSampler")
 NOT_ON_THIS_PATH = ()
 
 

@@ -615,6 +615,35 @@ int alq_herding_select(alq_ctx* ctx, const float* k, int64_t n, int64_t ldk, con
                        int64_t budget, int32_t* picks, float* m, int64_t* n_picks_host, int64_t* sum_s_host,
                        void* stream);
 
+/* ---- K24 / K25 / K26: BAIT (Ash, Goel, Krishnamurthy & Kakade, NeurIPS 2021) ------------------------------------------
+ * All fp64 (the NumPy statement is tests/bait_oracle.py).  n pool rows, C classes (2 <= C <= 16), D features, dim = C D
+ * (below 2^26); emb[n, D] fp32 contiguous rows; a row's Fisher embedding V_x = R_x (x) h_x^T with R_x = diag(sqrt p_x)
+ * (I - 1 p_x^T), coordinate (c, d) at c D + d.  Dense matrices are row-major dim x dim fp64, the per-row forms at, gt
+ * [n, C, C] fp64.  Anything else is ALQ_ERR_INVALID.
+ * alq_bait_fisher (K24): p[n, C] = the softmax of logits (ldl >= C) in fp64 (m + log sum exp(z - m), as alq_cal_scores)
+ *   and fisher = (1/n) sum_x (diag p_x - p_x p_x^T) (x) h_x h_x^T, exactly symmetric.  A row with a non-finite logit or
+ *   embedding entry is ALQ_ERR_NUMERIC (naming how many).  Synchronous (one 4-byte copy).
+ * alq_bait_init (K25): a = I / lamb, at_x = |h_x|^2 / lamb I, gt_x[a, b] = h_x^T fisher_ab h_x / lamb^2 (fisher_ab its
+ *   D x D block).  *lamb_host finite and > 0.  Asynchronous.
+ * alq_bait_select (K26): absorbs the n_lab rows lab_pos (int32, device) in order at scale 1 / sqrt(n_lab + budget), then
+ *   T = min(2 budget, n_cand) forward picks among cand_pos (int32, device, ascending) at scale s = sqrt(budget / (n_lab +
+ *   budget)) -- each the largest tr((s^2 R G R^T)(I + s^2 R A R^T)^-1) over the forms, lowest position on ties, then
+ *   absorbed -- and T - budget backward removals from that list -- each the first entry of the largest
+ *   tr((s^2 R G R^T)(-I + s^2 R A R^T)^-1), then removed.  Every absorption or removal is the rank-C update of a, at and
+ *   gt, consumed in place.  picks[0 .. *n_picks_host) (int32, device) = the remaining list in forward-pick order
+ *   (budget entries); fwd_list[T] (int32, device, may be NULL) the forward picks in order; fwd_scores[T] and
+ *   bwd_scores[T - budget] (fp64, device, may be NULL) the chosen score of every step.  phase_ms_host (may be NULL) receives the device milliseconds of the absorption, the forward and the backward
+ *   pass (CUDA events).  0 <= budget <= n_cand.  A C x C Cholesky factor whose pivot is not > 0 is ALQ_ERR_NUMERIC.  Ordinary launches
+ *   on one stream (about nine per step), synchronous at the end only. */
+int alq_bait_fisher(alq_ctx* ctx, const float* logits, int64_t n, int32_t c, int64_t ldl, const float* emb, int32_t d,
+                    double* p, double* fisher, void* stream);
+int alq_bait_init(alq_ctx* ctx, const float* emb, int64_t n, int32_t c, int32_t d, const double* fisher,
+                  const double* lamb_host, double* a, double* at, double* gt, void* stream);
+int alq_bait_select(alq_ctx* ctx, const float* emb, const double* p, int64_t n, int32_t c, int32_t d, const double* fisher,
+                    double* a, double* at, double* gt, const int32_t* lab_pos, int64_t n_lab, const int32_t* cand_pos,
+                    int64_t n_cand, int64_t budget, int32_t* picks, int64_t* n_picks_host, int32_t* fwd_list,
+                    double* fwd_scores, double* bwd_scores, float* phase_ms_host, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
